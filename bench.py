@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench.py -- learner gradient-steps/sec of the D4PG hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            # B200 arm (torchrun for N>1)
+    python bench.py --gpus N --steps K --warmup W            # GPU arm (torchrun for N>1)
+    python bench.py --steps K --dump-outputs DIR             # also write the last timed step's outputs as DIR/*.npy
     python bench.py --impl reference --steps K --warmup W    # CPU arm: the reference's own DDPG.train (oracle/_ref)
 
 Workload (config.workload = "c2"): |s|=17 |a|=6, 51 atoms, batch 256 per GPU, prioritized
-replay capacity 2^20 per GPU (full), fp32-accurate arithmetic (3xTF32 on tcgen05, fp32 accumulate: the 1e-5
+replay capacity 2^20 per GPU (full), fp32-accurate arithmetic (3xTF32 on wgmma, fp32 accumulate: the 1e-5
 parity bar of the golden tests).  One step = everything DDPG.train() does (ddpg.py:200-255).  Weak scaling:
 every rank owns a replay shard and a 256-row minibatch; the flat gradient is summed over the ranks once per
 step (fused into the dW / Adam kernels over NVLink peer memory; NCCL all-reduce as fallback).  `value` counts
@@ -62,7 +63,8 @@ def peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], tf=p.get("bf16_tflops_sustained", p.get("bf16_tflops")), src="measured")
-    return dict(hbm=6650.0, tf=1590.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm=3350.0, tf=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
@@ -106,8 +108,8 @@ def synth(cfg, n, seed):
 
 
 # ------------------------------------------------------------------------------------------
-# CPU arm: the oracle port of the reference's DDPG.train (the reference itself is Python and
-# cannot travel to the GPU box; oracle/ is pinned bit-exact to it, see oracle/__init__.py)
+# CPU arm: the oracle port of the reference's DDPG.train, used where oracle/_ref was not built
+# (oracle/ is pinned bit-exact to the reference, see oracle/__init__.py)
 # ------------------------------------------------------------------------------------------
 def cpu_arm(cfg, steps, warmup, budget_s=25.0):
     import torch
@@ -145,7 +147,7 @@ def cpu_arm(cfg, steps, warmup, budget_s=25.0):
 
 
 def cpu_arm_reference(cfg, steps, warmup, budget_s=25.0, n_fill=1 << 17):
-    """The UNMODIFIED reference (oracle/_ref = its modules byte-compiled by oracle/build_ref.py, or /root/reference where
+    """The UNMODIFIED reference (oracle/_ref = its modules byte-compiled by oracle/build_ref.py, or the reference sources where
     that exists) behind the 4-item compat shim, wired as main.py:382-392 wires it, driven through its public API only:
     PrioritizedReplayBuffer.add() x n_fill, then DDPG.train(global).  The buffer has the workload's capacity (tree depth
     20 for 2^20) but is filled with `n_fill` transitions: a million Python add() calls would not fit the time budget."""
@@ -189,13 +191,32 @@ def cpu_baseline(cfg, name, steps, warmup, budget_s):
                    "sample": "%d DDPG.train() calls of the UNMODIFIED reference (ddpg.py:200-255 + prioritized_replay_memory.py, "
                              "%s) on workload %s: PER capacity %d (tree depth %d), %d transitions added through add(); host has %d "
                              "cores, best of torch threads {1,%d} = %d" % (
-                                 r["done"], "from /root/reference" if ref_shim.source_available() else "oracle/_ref, byte-compiled from /root/reference",
+                                 r["done"], "from its sources" if ref_shim.source_available() else "oracle/_ref, its byte-compiled modules",
                                  name, cfg["cap"], int(np.ceil(np.log2(cfg["cap"]))), r["n_fill"], ncores, ncores, r["cores"])}
     r = cpu_arm(cfg, steps, warmup, budget_s)
     return r, {"value": r["value"], "unit": "steps/s", "cores": r["cores"], "kind": "port",
                "sample": "%d steps of the oracle port (restatement of ddpg.py:200-255 + PER, pinned bit-for-bit to the reference; "
                          "oracle/_ref was not present), workload %s, buffer full; host has %d cores, best of torch threads {1,%d} = %d" % (
                              r["done"], name, ncores, ncores, r["cores"])}
+
+
+def dump_outputs(dd, out_dir):
+    """What a caller of the timed path (DDPG.train_n) receives after its last step: both losses, the sampled batch
+    (indices, importance weights, TD errors, new priorities) and the parameters of the four networks, one .npy file
+    each, float32 or float64 (about 5 MB for c2)."""
+    lc, la = dd.last_losses()
+    arrays = {"losses": np.array([lc, la], dtype=np.float64)}
+    for k, v in dd.last_batch_info().items():
+        v = v.detach().cpu().numpy()
+        arrays["batch_" + k] = v.astype(np.float64 if v.dtype.kind in "iu" or v.dtype == np.float64 else np.float32)
+    for net in ("actor", "critic", "actor_target", "critic_target"):
+        for k, v in getattr(dd, net).state_dict().items():
+            arrays["%s.%s" % (net, k)] = v.detach().cpu().numpy().astype(np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, "outputs of %d bytes exceed the 64 MB dump limit" % total
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def reference_main(args):
@@ -216,7 +237,7 @@ def reference_main(args):
 
 
 # ------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------
 def gpu_main(args):
     import torch
@@ -272,8 +293,8 @@ def gpu_main(args):
     sampler = ClockSampler(local)
     sampler.start()
     # the timed region = EXACTLY K steps between barrier + synchronize on both sides, CUDA events on the learner stream,
-    # max over ranks.  A region of K = 20 steps lasts ~2 ms, so it is measured R times back to back and the MEDIAN
-    # region is reported (every region is a complete, valid measurement; all of them are listed)
+    # max over ranks.  With --repeats R > 1 the region is measured R times back to back and the MEDIAN region is
+    # reported (every region is a complete, valid measurement; all of them are listed)
     regions = []
     for _ in range(max(1, args.repeats)):
         barrier()
@@ -285,6 +306,8 @@ def gpu_main(args):
             e1.record(stream)
         barrier()
         regions.append(max_over_ranks(e0.elapsed_time(e1)))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(dd, args.dump_outputs)
     ms = float(np.median(regions))
     kernels = dd.kernels_per_step()
     exchange = comm.exchange_mode() if comm is not None else "single"
@@ -330,7 +353,7 @@ def gpu_main(args):
         n_gemm = len([k for k in prof if k.startswith("gemm_launch")])
         for k in prof:
             if k.startswith("gemm_launch"):
-                kinds[k] = ("%s (MLP level, %d launches/step)" % ("gemm_ffma_kernel" if args.precision == "fp32" else "gemm_tc2_kernel", n_gemm),
+                kinds[k] = ("%s (MLP level, %d launches/step)" % ("gemm_ffma_kernel" if args.precision == "fp32" else "gemm_tc_kernel", n_gemm),
                             alg["gemm_bytes"] / max(n_gemm, 1), "level")
     roofline = None
     if kinds:
@@ -346,17 +369,13 @@ def gpu_main(args):
             t_ms = float(np.mean(list(mlp_ms.values())))
             flops = alg["flops"] / len(mlp_ms)
         ach = nbytes / (t_ms * 1e-3) / 1e9
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get(name.split(" ")[0] + ":" + kinds[top][2])
         # the MLP layers are dense contractions: the roof that bounds them is the tensor pipe (SURVEY.md section 8d);
         # `achieved` = algorithmic FLOPs of the launch (2*M*N*K of its layers, the fp32 math -- the 3xTF32 split issues 3x
         # as many tensor-core MACs at the TF32 rate, half the bf16 rate) / its CUDA-event duration; the HBM view is kept
         tf = flops / (t_ms * 1e-3) / 1e12
         roofline = {"kernel": name, "bound": "tensor", "achieved": tf, "peak": pk["tf"], "unit": "TFLOP/s",
-                    "frac": tf / pk["tf"], "traffic": traffic,
-                    "peak_source": pk["src"] + " (sustained dense bf16 cuBLAS; no TF32 figure is measured on this pool, nominal TF32 = bf16 / 2)",
+                    "frac": tf / pk["tf"],
+                    "peak_source": pk["src"] + " (dense BF16; the TF32 rate the 3xTF32 split runs at is half of it)",
                     "avg_launch_us": t_ms * 1e3, "algorithmic_flops_per_launch": int(flops),
                     "algorithmic_bytes_per_launch": int(nbytes),
                     "hbm": {"achieved": ach, "peak": pk["hbm"], "unit": "GB/s", "frac": ach / pk["hbm"]}}
@@ -414,7 +433,7 @@ def gpu_main(args):
                 "replicas_identical": replicas_identical,
                 "implementation": {"step_plan": "levels (one launch per dependency level; the library's plan above 512 rows)" if (B > 512 or not args.chain) else "cluster chains",
                            "gradient_exchange": exchange,
-                           "precision": {"fp32": "exact fp32 FFMA tiles", "tf32x3": "3xTF32 on tcgen05 tensor cores (hi/lo split, fp32 accumulate in TMEM; meets the 1e-5 parity bar)", "tf32": "one TF32 tcgen05 pass (not parity-grade)"}[args.precision],
+                           "precision": {"fp32": "exact fp32 FFMA tiles", "tf32x3": "3xTF32 on wgmma tensor cores (hi/lo split, fp32 accumulate in registers; meets the 1e-5 parity bar)", "tf32": "one TF32 wgmma pass (not parity-grade)"}[args.precision],
                            "l2": "inputs larger than L2: replay store %.0f MB + trees %.0f MB per GPU, rows sampled at "
                                  "random; parameters (%.1f MB) are L2-resident by design" % (
                                      cap * ((2 * cfg["obs"] + cfg["act"]) * 4 + 9) / 1e6, 16 * cap / 1e6 * 1.05, alg["P"] * 16 / 1e6)},
@@ -442,9 +461,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="c2", choices=sorted(CFG))
     ap.add_argument("--no-cpu", action="store_true")
-    ap.add_argument("--repeats", type=int, default=5, help="timed regions of K steps each; the median region is reported")
+    ap.add_argument("--repeats", type=int, default=1, help="timed regions of K steps each; the median region is reported")
     ap.add_argument("--precision", default="tf32x3", choices=["fp32", "tf32x3", "tf32"])
     ap.add_argument("--chain", type=int, default=1, help="MLP step plan: 1 = cluster-fused chains, 0 = one launch per level")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last of them computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         reference_main(args)

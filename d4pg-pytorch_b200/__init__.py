@@ -1,4 +1,4 @@
-"""d4pg-pytorch_b200 -- B200-native (sm_100a) D4PG learner hot path behind the reference's
+"""d4pg-pytorch_b200 -- H100-native (sm_90a) D4PG learner hot path behind the reference's
 Python API (ajgupta93/d4pg-pytorch: ddpg.py, models.py, prioritized_replay_memory.py,
 replay_memory.py, shared_adam.py).
 

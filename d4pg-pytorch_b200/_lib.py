@@ -1,6 +1,6 @@
-"""ctypes binding of libd4pg_sm100.so (the C ABI declared in include/d4pg_b200.h).
+"""ctypes binding of libd4pg_sm90.so (the C ABI declared in include/d4pg_b200.h).
 
-There is NO CPU fallback: if the shared library is missing or no sm_100 device is
+There is NO CPU fallback: if the shared library is missing or no sm_90 device is
 present, every compute entry point raises.  (Host-only bookkeeping -- layouts,
 state_dict plumbing -- works without a GPU so the CPU test-suite can exercise it.)
 """
@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libd4pg_sm100.so")
+LIB_PATH = os.path.join(_HERE, "libd4pg_sm90.so")
 
 OK, EINVAL, ECUDA, ENOTSUP, ENCCL, ESTATE = 0, -1, -2, -3, -4, -5
 PROJ_TARGET_IS_PROBS, PROJ_Q_IS_PROBS = 1, 2
@@ -169,7 +169,7 @@ def require_cuda():
     """Every compute path calls this first: fail loudly, never fall back."""
     import torch
     if not torch.cuda.is_available():
-        raise D4PGError("no CUDA device: the D4PG hot path runs only on sm_100a (B200); there is no CPU fallback")
+        raise D4PGError("no CUDA device: the D4PG hot path runs only on sm_90a (H100); there is no CPU fallback")
     lib()
 
 
@@ -182,7 +182,7 @@ def ptr(t):
 
 def raw_stream(device_index=None):
     """cudaStream_t of torch's current stream as an int.  torch.cuda.current_stream() builds a Stream object through
-    several Python layers (~7 us per call, twice per training step); the raw getter is ~0.3 us."""
+    several Python layers, twice per training step; the raw getter skips them."""
     import torch
     if device_index is None:
         device_index = torch.cuda.current_device()

@@ -13,8 +13,7 @@ int pdl_mode() {
   return m;
 }
 bool pdl_enabled() {
-  // measured on B200 (profiles/README.md): +17 % step time for the FFMA path, -5 % for the tcgen05 path
-  // -> opt-in.  D4PG_PDL=1 enables it.
+  // opt-in: D4PG_PDL=1 enables it (tools/ab_pdl.sh compares the modes).
   static const bool on = getenv("D4PG_PDL") != nullptr;
   return on;
 }
@@ -94,6 +93,14 @@ extern "C" int32_t d4pg_device_sm(void) {
   D4PG_CUDA_OK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
   return major * 10 + minor;
 }
+namespace d4pg {
+int device_sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 1;
+  return n > 0 ? n : 1;
+}
+}  // namespace d4pg
 
 extern "C" int32_t d4pg_actor_layout(int32_t obs_dim, int32_t act_dim, d4pg_net_layout_t* out) {
   D4PG_REQUIRE(out && obs_dim > 0 && act_dim > 0, D4PG_EINVAL, "d4pg_actor_layout: bad arguments");

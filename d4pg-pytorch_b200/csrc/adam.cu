@@ -1,6 +1,6 @@
 // Fused Adam (beta=(0.9,0.9) by default) + Polyak soft target update over flat fp32 buffers.
 //
-// Replaces (reference, relative to /root/reference):
+// Replaces (reference, relative to its repository root):
 //   shared_adam.py:3-17 + torch.optim.Adam.step as called at ddpg.py:232,244.  Arithmetic follows
 //     torch 2.11 `_single_tensor_adam` (the form the reference executes in this image):
 //       m <- lerp(m, g, 1-b1); v <- v*b2 + (1-b2)*g*g;
@@ -36,7 +36,7 @@ int launch_adam(const AdamArgs& a_in, cudaStream_t st) {
   int64_t nmax = 0;
   for (int i = 0; i < a.nseg; ++i) nmax = a.seg[i].n > nmax ? a.seg[i].n : nmax;
   int blocks = int((nmax / 4 + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > 4 * device_sm_count()) blocks = 4 * device_sm_count();     // grid-stride: 4 CTAs per SM
   if (blocks < 1) blocks = 1;
   D4PG_MAX_CARVEOUT(adam_polyak_kernel);
   const int tail = ((a.clock || a.loss_out) && !a.skip_tail) ? 1 : 0;
@@ -75,7 +75,7 @@ __global__ void polyak_kernel(float* t, const float* s, int64_t n, float tau, fl
 
 extern "C" int32_t d4pg_polyak(float* target, const float* src, int64_t n, double tau, d4pg_stream_t stream) {
   D4PG_REQUIRE(target && src && n > 0, D4PG_EINVAL, "d4pg_polyak: bad arguments");
-  int blocks = int(std::min<int64_t>(592, (n + 255) / 256));
+  int blocks = int(std::min<int64_t>(4 * d4pg::device_sm_count(), (n + 255) / 256));   // grid-stride
   polyak_kernel<<<blocks, 256, 0, as_stream(stream)>>>(target, src, n, float(tau), float(1.0 - tau));
   D4PG_LAUNCH_OK();
   return D4PG_OK;

@@ -101,7 +101,7 @@ struct PeerInfo {
   const float* mc; float* mc_uc;
 };
 
-// tcgen05 chains (mlp_tc_chain.cu): the updated weights are ALSO written as the tensor cores' forward operand images
+// tensor-core chains (mlp_tc_chain.cu): the updated weights are ALSO written as the tensor cores' forward operand images
 // (hi / lo tf32 parts, 32 x 32 K-major SWIZZLE_128B blocks), for the online network and -- the Polyak output -- its
 // target, so that the next step's forward chains need no separate pack launch.  One entry per weight matrix.
 struct AdamImgLayer { int64_t w_off, w_end; int ld, nchunks; uint8_t* img; uint8_t* img_t; };

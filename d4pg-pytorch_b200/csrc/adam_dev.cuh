@@ -82,7 +82,7 @@ __device__ __forceinline__ void adam_segment(const AdamArgs& a, int seg, int bx,
     }
     p4[i] = p; m4[i] = m; v4[i] = v;
     if (s.target) t4[i] = t;
-    if (s.nimg) {                                             // forward operand images of the tcgen05 chains
+    if (s.nimg) {                                             // forward operand images of the tensor-core chains
       const int64_t e = i << 2;
 #pragma unroll
       for (int L = 0; L < 4; ++L) {

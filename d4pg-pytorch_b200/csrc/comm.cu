@@ -161,7 +161,7 @@ int comm_peer_reduce_scatter(d4pg_comm* c, int parity, cudaStream_t st) {
   a.half_off = int64_t(parity) * info.n;
   for (int r = 0; r < info.world; ++r) { a.g[r] = info.x[r]; a.red[r] = info.red[r]; }
   a.my_f1 = info.flag[info.rank]; a.sig2 = comm_peer_signal(info, 1);
-  const int blocks = int(std::max<int64_t>(1, std::min<int64_t>(296, (a.hi4 - a.lo4 + 255) / 256)));
+  const int blocks = int(std::max<int64_t>(1, std::min<int64_t>(2 * device_sm_count(), (a.hi4 - a.lo4 + 255) / 256)));
   peer_reduce_scatter_kernel<<<blocks, 256, 0, st>>>(a);
   D4PG_LAUNCH_OK();
   return D4PG_OK;
@@ -199,7 +199,7 @@ int comm_mc_reduce_bcast(d4pg_comm* c, int parity, cudaStream_t st) {
   a.mc_half = info.mc + int64_t(parity) * info.n;
   a.mc_red = const_cast<float*>(info.mc) + 2 * info.n;
   a.my_f1 = info.flag[info.rank]; a.sig2 = comm_peer_signal(info, 1);
-  const int blocks = int(std::max<int64_t>(1, std::min<int64_t>(296, (a.hi4 - a.lo4 + 255) / 256)));
+  const int blocks = int(std::max<int64_t>(1, std::min<int64_t>(2 * device_sm_count(), (a.hi4 - a.lo4 + 255) / 256)));
   mc_reduce_bcast_kernel<<<blocks, 256, 0, st>>>(a);
   D4PG_LAUNCH_OK();
   return D4PG_OK;

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libd4pg_sm100.so (sm_100a only).
+// Shared host/device helpers for libd4pg_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,8 +35,7 @@ void set_error(const char* fmt, ...);
 
 // All kernels of a step ask for the same (maximum) shared-memory carve-out: a step mixes kernels
 // with 0 KB, 14 KB, 32 KB and 197 KB of shared memory, and letting the driver pick a per-kernel
-// L1/shared split makes every kernel boundary an SM reconfiguration (ncu: ~17 us of a 20 us
-// gemm_tc2 launch had no active SM cycles).
+// L1/shared split makes every kernel boundary an SM reconfiguration.
 #define D4PG_MAX_CARVEOUT(kernel)                                                                     \
   do {                                                                                                \
     static bool _carved = false;                                                                      \
@@ -60,6 +59,7 @@ __device__ __forceinline__ void pdl_trigger_raw() { asm volatile("griddepcontrol
 __device__ __forceinline__ void pdl_trigger(int mode) { if (mode == 1) pdl_trigger_raw(); }
 __device__ __forceinline__ void pdl_trigger_end(int mode) { if (mode == 2) pdl_trigger_raw(); }
 int pdl_mode();                      // 0 off, 1 early trigger, 2 late trigger (env D4PG_PDL)
+int device_sm_count();               // SMs of the current device (grid-stride kernels size their grids by it)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 bool pdl_enabled();
 template <typename... KArgs, typename... Args>

@@ -28,8 +28,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_ffma_kernel(const __grid
 }
 
 // Every dW of a step in one launch (mlp_chain.cuh: GemmWideBatch).  Only the asynchronous dW tile is
-// compiled in, which needs no staging registers: 3 CTAs per SM (304 tiles at config 2 are ONE wave; at
-// 2 CTAs per SM the last 8 tiles were a second wave that doubled the launch's duration).
+// compiled in, which needs no staging registers: 3 CTAs per SM (the 304 tiles of config 2 are ONE wave on
+// 132 SMs; at 2 CTAs per SM they would take two, doubling the launch's duration).
 template <bool ALLOW_SPLIT>
 __global__ void __launch_bounds__(GEMM_THREADS, 3) gemm_wide_kernel(const __grid_constant__ GemmWideBatch batch) {
   extern __shared__ __align__(16) float smem[];        // DW_SMEM_FLOATS
@@ -86,7 +86,7 @@ GemmProblem gemm_dw(const float* dZ, int lddz, const float* X, int ldx, float* d
   p.mode = GEMM_DW; p.epi = EPI_NONE;
   return p;
 }
-void gemm_batch_begin(GemmBatch& b) { b.n = 0; b.total_tiles = 0; b.all_tma = 0; b.trace = nullptr; }
+void gemm_batch_begin(GemmBatch& b) { b.n = 0; b.total_tiles = 0; b.trace = nullptr; }
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static void prepare_problem(GemmProblem& p) {
   // 128-bit staging is legal when rows start 16-B aligned and the contiguous extent is a multiple of 4
@@ -162,7 +162,7 @@ bool gemm_batch_has_splitk(const GemmBatch& b) {
 }
 int gemm_launch(GemmBatch& b, int precision, cudaStream_t st) {
   if (precision == 0) return gemm_batch_launch(b, st);
-  gemm_tc_prepare(b);                 // picks the kernel variant and tiles the problems accordingly
+  gemm_tc_prepare(b);                 // retiles the problems for the wgmma tiles and encodes the TMA maps
   return gemm_tc_batch_launch(b, precision == 1 ? 3 : 1, st);
 }
 int gemm_batch_launch(const GemmBatch& b, cudaStream_t st) {

@@ -35,11 +35,10 @@ struct GemmBatch {
   GemmProblem p[GEMM_MAX_PROBLEMS];
   int n;
   int total_tiles;
-  // tcgen05 path only: TMA descriptors of the operands that qualify (16-B aligned rows, K-major)
+  // tensor-core path only: TMA descriptors of the operands that qualify (16-B aligned rows, K-major)
   alignas(64) CUtensorMap tmap_a[GEMM_MAX_PROBLEMS];
   alignas(64) CUtensorMap tmap_b[GEMM_MAX_PROBLEMS];
   alignas(64) CUtensorMap tmap_a2[GEMM_MAX_PROBLEMS];   // concatenated tail of A (critic fc2's action columns)
-  int all_tma;                                           // every operand of every problem is TMA-fed -> v2 kernel
   unsigned long long* trace;                             // optional %globaltimer phase stamps of CTA 0 (D4PG_TC_TRACE)
   int pdl;                                               // programmatic-dependent-launch trigger position (0/1/2)
 };
@@ -57,8 +56,8 @@ int gemm_batch_launch(const GemmBatch& b, cudaStream_t st);                    /
 void gemm_batch_retile(GemmBatch& b, int bm, int bn);
 bool gemm_batch_has_splitk(const GemmBatch& b);
 void gemm_tc_prepare(GemmBatch& b);                                             // TMA eligibility + tensor maps
-int gemm_tc_batch_launch(const GemmBatch& b, int passes, cudaStream_t st);      // tcgen05 (128x32 tiles)
-// precision: 0 = fp32 FFMA, 1 = 3xTF32 tcgen05 (fp32-accurate), 2 = 1xTF32 tcgen05
+int gemm_tc_batch_launch(const GemmBatch& b, int passes, cudaStream_t st);      // wgmma (128x32 tiles)
+// precision: 0 = fp32 FFMA, 1 = 3xTF32 wgmma (fp32-accurate), 2 = 1xTF32 wgmma
 int gemm_launch(GemmBatch& b, int precision, cudaStream_t st);
 
 }  // namespace d4pg

@@ -27,8 +27,8 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ---- operand staging ---------------------------------------------------------------------------
-// Two source shapes, each with a 128-bit fast path (ncu of the first version: 42 % of all issued
-// instructions were address arithmetic / predicate / constant-bank loads of the scalar staging):
+// Two source shapes, each with a 128-bit fast path (scalar staging spends most of its instructions on address
+// arithmetic, predicates and constant-bank loads):
 //   K-contiguous  src[row*ld + k]  (rows = tile dim): thread reads 2 float4 along k
 //   row-contiguous src[k*ld + col] (cols = tile dim): thread reads 2 float4 along the tile dim
 // Everything is read into registers first (all loads of a chunk in flight together), then

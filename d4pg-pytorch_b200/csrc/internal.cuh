@@ -1,4 +1,4 @@
-// Cross-translation-unit internals of libd4pg_sm100.so (not part of the C ABI).
+// Cross-translation-unit internals of libd4pg_sm90.so (not part of the C ABI).
 #pragma once
 #include "common.cuh"
 #include "adam.cuh"

@@ -105,7 +105,7 @@ struct d4pg_learner {
   // profiling (d4pg_learner_profile_step): CUDA-event pair around every launch of an eager step
   cudaStream_t side; cudaEvent_t ev_fork, ev_join;
   ChainArgs chain_fwd_args, chain_bwd_args;
-  // tcgen05 chains (precision >= 1): library-owned weight images + the per-step pack / chain descriptors
+  // tensor-core chains (precision >= 1): library-owned weight images + the per-step pack / chain descriptors
   // weight images: forward ones (packed at the start of a graph launch, then kept current by the Adam kernel) and the
   // transposed ones of the dX chains (packed every step on the side branch, off the critical path)
   uint8_t* tcc_images; TccPackArgs tcc_pack_fwd, tcc_pack_dx; TccImage tcc_img[32]; bool tcc_ok;
@@ -130,9 +130,8 @@ struct d4pg_learner {
 };
 
 // step plan: 0 = one grouped launch per dependency level, 1 = cluster-fused chains (mlp_chain.cu exact fp32 /
-// mlp_tc_chain.cu tcgen05).  The chain plans pay off while the batch fits one wave of clusters: measured
-// on B200, batch 1024 (config 3) 409 us with chains vs 320 us per level, batch 4096 (config 5) 906 vs 733 us
-// (tcgen05 levels), so batches above 512 rows always run plan 0.
+// mlp_tc_chain.cu wgmma).  The chain plans pay off while the batch fits one wave of clusters (a 64-row cluster chain
+// is a latency design; 128-row level tiles suit larger batches), so batches above 512 rows always run plan 0.
 static int step_plan(const d4pg_learner_config_t& c) { return c.batch > 512 ? 0 : c.chain; }
 // prefetch pipeline: batch t+1 is sampled on a side branch of step t (device-side sampling only)
 static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 1; }
@@ -144,13 +143,13 @@ static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0
 static bool host_pipe(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 0 && c.use_graph != 0; }
 static bool piped(const d4pg_learner_config_t& c) { return prefetching(c) || host_pipe(c); }
 struct d4pg_learner;
-static bool inline_wait(const d4pg_learner* L);     // the warm host-pipeline graph polls the sampler's epochs itself (tcgen05 chain plan)
+static bool inline_wait(const d4pg_learner* L);     // the warm host-pipeline graph polls the sampler's epochs itself (tensor-core chain plan)
 
-// weight matrices as the tcgen05 chains consume them (F = forward image, D = transposed image for dX)
+// weight matrices as the tensor-core chains consume them (F = forward image, D = transposed image for dX)
 enum { U_A_F1, U_A_F2, U_A_F22, U_A_F3, U_A_D3, U_A_D22, U_A_D2, U_AT_F1, U_AT_F2, U_AT_F22, U_AT_F3,
        U_C_F1, U_C_F2, U_C_F22, U_C_F3, U_C_D3, U_C_D22, U_C_D2H, U_C_D2A, U_CT_F1, U_CT_F2, U_CT_F22, U_CT_F3, U_COUNT };
 
-// tcgen05 chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
+// tensor-core chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
 static bool tcc_shapes_ok(const d4pg_learner_config_t& c) {
   return c.chain == 1 && c.batch <= 512 && c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256;
 }
@@ -204,7 +203,7 @@ static int tcc_setup(d4pg_learner* L) {
   return D4PG_OK;
 }
 
-// ---- tcgen05 chain builders (mlp_tc_chain.cu) ----------------------------------------------------------------------
+// ---- tensor-core chain builders (mlp_tc_chain.cu) ------------------------------------------------------------------
 struct TccCtx {
   d4pg_learner* L; const Workspace* w; const NetDims* da; const NetDims* dc;
   const float *Wa, *Wat, *Wc, *Wct;
@@ -362,20 +361,20 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   const float* Wa = b.actor; const float* Wat = b.actor_target; const float* Wc = b.critic; const float* Wct = b.critic_target;
   GemmBatch g;
   const int plan = step_plan(c);
-  const bool tcc = plan == 1 && c.precision >= 1 && L->tcc_ok;       // tcgen05 cluster chains
+  const bool tcc = plan == 1 && c.precision >= 1 && L->tcc_ok;       // tensor-core cluster chains
   // corrected-semantics switch (SURVEY.md H7, loss_flags & 4): the actor gradient goes through the critic AFTER this
   // step's critic update (the reference uses the stale local copy, ddpg.py:229-247).  Two half steps: critic forward /
   // loss / backward / Adam, then the policy pass through the updated critic, actor backward / Adam.
   const bool h7 = (c.loss_flags & 4) != 0;
-  D4PG_REQUIRE(!h7 || (tcc && c.world_size <= 1), D4PG_ENOTSUP, "post-update-critic actor gradient needs the tcgen05 chain plan (precision tf32x3 / tf32, chain plan, batch <= 512) on one GPU");
+  D4PG_REQUIRE(!h7 || (tcc && c.world_size <= 1), D4PG_ENOTSUP, "post-update-critic actor gradient needs the tensor-core chain plan (precision tf32x3 / tf32, chain plan, batch <= 512) on one GPU");
   const bool chain = plan == 1 && !tcc;
   static const bool no_pre = getenv("D4PG_NO_PRE") != nullptr;          // A/B switch
   const bool pre_ok = chain && c.precision == 0 && A <= 8 && !no_pre;   // pre-layers: fp32 tile, |a| <= 8
   if (tcc) {
     // 2''. the same three forward chains on the tensor cores (mlp_tc_chain.cu): clusters of 8 CTAs own 64 rows,
-    // every layer a tcgen05.mma tile.  The hi/lo weight images are re-packed first (Adam / Polyak changed them).
+    // every layer a wgmma tile.  The hi/lo weight images are re-packed first (Adam / Polyak changed them).
     if (pack_fwd) RUN(launch_tcc_pack(L->tcc_pack_fwd, st));
-    // the transposed images of the dX chains are needed ~35 us from now: packed on the side branch
+    // the transposed images of the dX chains are needed only after the forward chains and heads: packed on the side branch
     D4PG_CUDA_OK(cudaEventRecord(L->ev_fork2, st));
     D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork2, 0));
     RUN(launch_tcc_pack(L->tcc_pack_dx, L->side));
@@ -390,7 +389,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     tcc_build_Q(fa, 2, cx, w.a, w.h1[2], w.h2[2], w.h3[2], w.out[2]);   // chain 2  Q: critic(s, a)
     if (host_pipe(c) && !cold && inline_wait(L)) {
       // warm host-pipeline variant: the batch comes from the ingest stream's sample kernel; instead of a stream event
-      // (event + graph start: ~6 us after the sample ends) every CTA polls the epochs that kernel publishes
+      // (event + graph start after the sample ends) every CTA polls the epochs that kernel publishes
       fa.wait_epoch = w.pipe_epoch; fa.wait_clock = reinterpret_cast<const long long*>(&w.clock->steps_done);
       fa.wait_n = cdiv(B, SAMPLE_ROWS);
     }
@@ -401,8 +400,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     //   chain 1  P: actor(s) -> critic(s, actor(s))                ddpg.py:236-238 (fc1 of the critic is recomputed: K=|s|)
     //   chain 2  Q: critic(s, a)                                   ddpg.py:208
     // The block scheduler fills SMs in launch order: the two 8-layer chains come first so that each of their CTAs
-    // gets an SM of its own, and the short 4-layer chain is the one that doubles up (measured with %smid: in the
-    // order T,Q,P 38 SMs hosted a T and a P CTA while 52 SMs hosted a lone Q CTA; forward launch 49 us)
+    // gets an SM of its own, and the short 4-layer chain is the one that doubles up
     ChainArgs& ca = L->chain_fwd_args;
     chain_args_begin(ca, B, w.xchg, c.precision);
     ChainSlot sl; int at3 = -1, ct1, q1, a3 = -1, c1;
@@ -547,14 +545,14 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   const int gpar = pf ? par : int(L->steps_done & 1);
   const bool inline_sync_possible = chain || tcc;
   // Exchange shapes (D4PG_COMM_MODE=mc|mc2|pull|rs; default: "mc" from D4PG_COMM_MC_FROM = 3 ranks up when the communicator
-  // set up a multicast object, else "pull"):
+  // set up a multicast object, else "pull").  These defaults were chosen on another GPU generation and have NOT been
+  // validated on Hopper (no multi-GPU H100 measurement exists yet; tools/ab_mc8.sh compares the modes):
   //   "mc"   in-switch reduction: ONE hop and 1.15 MB inbound per rank -- the Adam kernel's multimem.ld_reduce over an NVLS
-  //          multicast object returns the sum over all ranks, added by the NVSwitch (8 ranks: 101.6 us/step);
+  //          multicast object returns the sum over all ranks, added by the NVSwitch;
   //   "mc2"  its two-phase form: every rank ld_reduces its 1/N slice and multimem.st's it to everyone (2 x 1.15 MB per GPU
-  //          whatever N), then a second flag hop (8 ranks: 100.9 us; 2 ranks: 98.9 vs 90.5 for "mc");
-  //   "pull" one hop, every rank sums all N halves inside Adam (N x 1.15 MB inbound over NVLink; 2 ranks 89.2 us -- the
-  //          fastest there -- 8 ranks 111.9);
-  //   "rs"   reduce-scatter + all-gather over peer memory: TWO hops of 16-B remote accesses (loses everywhere: 130.7 us at 8).
+  //          whatever N), then a second flag hop;
+  //   "pull" one hop, every rank sums all N halves inside Adam (N x 1.15 MB inbound over NVLink);
+  //   "rs"   reduce-scatter + all-gather over peer memory: TWO hops of 16-B remote accesses.
   static const int comm_mode = [] { const char* e = getenv("D4PG_COMM_MODE");
                                     return !e ? 0 : (e[0] == 'p' ? 1 : (e[0] == 'r' ? 2 : (e[0] == 'm' && e[1] == 'c' && e[2] == '2' ? 4 : 3))); }();
   static const int mc_from = [] { const char* e = getenv("D4PG_COMM_MC_FROM"); return e ? atoi(e) : 3; }();
@@ -698,7 +696,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     }
   }
   aa.nseg = 2;
-  if (tcc) {                                                    // keep the forward weight images of the tcgen05 chains current
+  if (tcc) {                                                    // keep the forward weight images of the tensor-core chains current
     const TccImage* U = L->tcc_img;
     const NetDims* nd[2] = {&da, &dc};
     const int base[2] = {U_A_F1, U_C_F1}, tbase[2] = {U_AT_F1, U_CT_F1};
@@ -766,11 +764,11 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   D4PG_REQUIRE(cfg->v_max > cfg->v_min, D4PG_EINVAL, "d4pg_learner_create: v_max <= v_min");
   D4PG_REQUIRE(cfg->proj_mode == 0 || cfg->proj_mode == 1, D4PG_EINVAL, "d4pg_learner_create: proj_mode must be 0/1");
   D4PG_REQUIRE(cfg->precision >= 0 && cfg->precision <= 2, D4PG_ENOTSUP,
-               "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 tcgen05, 2 TF32 tcgen05)", cfg->precision);
+               "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma)", cfg->precision);
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
   D4PG_REQUIRE(!(cfg->loss_flags & 4) || (tcc_shapes_ok(*cfg) && cfg->world_size <= 1), D4PG_ENOTSUP,
-               "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tcgen05 chain plan: precision 1/2, chain 1, "
+               "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1/2, chain 1, "
                "batch <= 512, obs_dim <= 32, act_dim <= 32, on one GPU");
   D4PG_REQUIRE(buf->actor && buf->actor_target && buf->critic && buf->critic_target && buf->grad_actor && buf->grad_critic &&
                buf->adam_m_actor && buf->adam_v_actor && buf->adam_m_critic && buf->adam_v_critic &&
@@ -1039,7 +1037,7 @@ extern "C" int32_t d4pg_learner_read_losses(d4pg_learner_t* L, float* out4, d4pg
 }
 
 // Back-to-back steps with nothing in between: warm prefetch steps are replayed RUN_UNROLL at a time from one graph
-// (a graph launch boundary costs ~5 us of idle GPU; inside a graph consecutive steps are ordinary dependent nodes).
+// (a graph launch boundary leaves the GPU idle; inside a graph consecutive steps are ordinary dependent nodes).
 constexpr int RUN_UNROLL = 8;
 extern "C" int32_t d4pg_learner_run(d4pg_learner_t* L, int32_t n_steps, d4pg_stream_t stream) {
   D4PG_REQUIRE(L && n_steps > 0, D4PG_EINVAL, "d4pg_learner_run: bad arguments");

@@ -1,12 +1,12 @@
 // Cluster-fused MLP chains: every dependent layer of a network chain in ONE launch.
 //
 // At batch 256 the actor/critic passes of DDPG.train (models.py:32-41,76-88 forward, ddpg.py:230,242
-// backward) are 14 dependent layer levels; as separate grouped-GEMM launches each level costs ~7 us of
-// which most is the kernel boundary (profiles/README.md).  Here a thread-block CLUSTER of 8 CTAs owns
+// backward) are 14 dependent layer levels; as separate grouped-GEMM launches most of each level's time is
+// the kernel boundary.  Here a thread-block CLUSTER of 8 CTAs owns
 // 32 batch rows for a whole chain (e.g. actor_target fc1..fc3 -> critic_target fc1..fc3): CTA r of the
 // cluster computes the 32-column slice r of each 256-wide layer, publishes it k-major into an
-// L2-resident exchange plane, and a cluster barrier (barrier.cluster arrive.release / wait.acquire,
-// ~0.2 us) replaces the kernel boundary.  The next layer's first weight chunk is prefetched between
+// L2-resident exchange plane, and a cluster barrier (barrier.cluster arrive.release / wait.acquire)
+// replaces the kernel boundary.  The next layer's first weight chunk is prefetched between
 // the arrive and the wait.  Rows never mix, so clusters are independent: no grid-wide barrier, no
 // co-residency requirement beyond the cluster itself.
 //
@@ -96,8 +96,7 @@ __device__ __forceinline__ void fetch_weights(float* Ws, const float* __restrict
 // One 32x32 tile of one slot with A and W resident for the whole K.  The order of the additions is
 // gemm_tile's: within every 64-deep chunk warp w owns k = 8w..8w+7, partial tiles are summed w = 0..7.
 // ---- tensor-core variant of the tile (PREC 1 = 3xTF32, fp32-accurate; PREC 2 = one TF32 pass) --------------------
-// mma.sync.m16n8k8 (the warp-level MMA that exists for a 32-row tile; tcgen05 tiles start at 64-128 rows).  On sm_100a
-// it issues every 8.1 cycles per sub-partition (tests/probe/dsmem_probe.cu): 4x the FFMA rate, and the operand
+// mma.sync.m16n8k8 (the warp-level MMA that exists for a 32-row tile; wgmma tiles start at 64 rows): the operand
 // fragments cost 16 LDS.32 per 8-deep k-step instead of 96 LDS wavefronts for the FFMA lane tiles.
 // 3xTF32: x = hi + lo with hi = tf32(x), lo = tf32(x - hi);  D += Al*Bh + Ah*Bl + Ah*Bh  (~2^-21 relative).
 __device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
@@ -480,8 +479,7 @@ int launch_mlp_chain(ChainArgs& a, cudaStream_t st) {
   }
   const size_t smem = size_t(a.a_floats + 2 * a.w_floats) * sizeof(float);
   // NOT padded to force one CTA per SM: 16 clusters of 8 at one CTA per SM need two free 8-SM groups in every
-  // GPC; a single foreign CTA (the concurrent tree update) pushes clusters into a second wave (measured: the dX
-  // launch took 38 us while every chain in it finished within 25 us).
+  // GPC; a single foreign CTA (the concurrent tree update) pushes clusters into a second wave.
   D4PG_REQUIRE(smem <= 220 * 1024, D4PG_ENOTSUP, "launch_mlp_chain: %zu B of shared memory needed", smem);
   D4PG_REQUIRE(a.precision >= 0 && a.precision <= 2, D4PG_EINVAL, "launch_mlp_chain: precision %d", a.precision);
   static size_t smem_set[3] = {0, 0, 0};

@@ -1,28 +1,28 @@
-// tcgen05 cluster chains: every dependent layer of an actor/critic network chain in ONE launch, each layer a
-// tcgen05.mma (UTCHMMA) tile with a TMEM accumulator, operands brought in by TMA bulk copies.
+// Cluster chains on the Hopper tensor cores: every dependent layer of an actor/critic network chain in ONE launch,
+// each layer a set of wgmma tiles with register accumulators, operands brought in by bulk copies (cp.async.bulk).
 //
 // Reference ops: actor.forward / critic.forward (models.py:32-41,76-88) for the five forward passes of
 // DDPG.train (ddpg.py:205-208,236) and the two backward passes of ddpg.py:230,242 (dX only; dW is gemm_wide).
 //
-// Decomposition.  A thread-block CLUSTER of 8 CTAs owns 64 batch rows (UMMA M = 64) for a whole chain.  CTA r
-// owns output features [32r, 32r+32) of every 256-wide layer (UMMA N = 32), so a layer is eight 64x32xK tiles
-// and the layer-to-layer dependency is an all-gather of the 64x256 activation plane inside the cluster.
+// Decomposition.  A thread-block CLUSTER of 8 CTAs owns 64 batch rows (wgmma M = 64) for a whole chain.  CTA r
+// owns output features [32r, 32r+32) of every 256-wide layer, so a layer is eight 64x32xK tiles and the
+// layer-to-layer dependency is an all-gather of the 64x256 activation plane inside the cluster.
 //
 // Precision.  3xTF32: x = hi + lo, hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi);
-// D += Al*Bh + Ah*Bl + Ah*Bh with fp32 accumulation in TMEM (~2^-21 relative, meets the 1e-5 parity bar).
+// D += Al*Bh + Ah*Bl + Ah*Bh with fp32 accumulation (~2^-21 relative, meets the 1e-5 parity bar).
 // Nothing is split on the critical path:
 //   * weights: hi/lo parts are PRE-PACKED once per step (tcc_pack_kernel, right after Adam changed them) into the
 //     exact shared-memory image the MMA reads (K-major SWIZZLE_128B, 32x32 blocks) -- for the backward pass the
 //     transposed image -- so a CTA's weight slice of a layer is ONE contiguous cp.async.bulk;
-//   * activations: the epilogue that PRODUCES a layer output (tcgen05.ld -> bias/ReLU/tanh/mask) writes it three
-//     times: row-major fp32 (for the loss kernel / dW), and as hi and lo images of its 64x32 tile = K-chunk r of
-//     the next layer's A operand, already swizzled.  The consumers fetch chunk c with one 16-KB cp.async.bulk.
+//   * activations: the epilogue that PRODUCES a layer output (bias/ReLU/tanh/mask on the accumulator registers)
+//     writes it three times: row-major fp32 (for the loss kernel / dW), and as hi and lo images of its 64x32 tile
+//     = K-chunk r of the next layer's A operand, already swizzled.  The consumers fetch chunk c with one 16-KB
+//     cp.async.bulk.
 //
-// Per CTA: warp 0 = loader (one lane issues every bulk copy: weight slice one slot ahead, A chunks into an
-// 8-deep ring, completion on mbarriers by byte count), warp 1 = TMEM owner + the single MMA-issuing lane (12
-// tcgen05.mma per 32-deep chunk and group; tcgen05.commit releases ring buffers and signals the accumulator),
-// warps 2..9 = epilogue (lane quarter = warp % 4, 16 accumulator columns each).  A slot boundary is a cluster
-// barrier (arrive.release / wait.acquire): outputs in L2 are visible, ring and weight buffers are free.
+// Per CTA: warpgroups 0 and 1 = consumers (warpgroup g issues the wgmmas of output group g of a slot and runs
+// its epilogue), warp 8 = loader (one lane issues every bulk copy: weight slices one slot ahead, A chunks into
+// direct-mapped buffers, completion on mbarriers by byte count).  A slot boundary is a cluster barrier
+// (arrive.release / wait.acquire): outputs in L2 are visible, A and weight buffers are free.
 #include "mlp_tc_chain.cuh"
 #include "tc_common.cuh"
 #include <stdlib.h>
@@ -37,7 +37,8 @@ constexpr uint32_t TCC_OFF_A = 0;
 constexpr uint32_t TCC_OFF_W = TCC_ABUFS * TCC_A_CHUNK;
 constexpr uint32_t TCC_OFF_BAR = TCC_OFF_W + TCC_MAX_CHUNKS * TCC_W_CHUNK;
 constexpr uint32_t TCC_SMEM = TCC_OFF_BAR + 256 + 1024;      // barriers + alignment slack
-constexpr int TCC_TMEM_COLS = TCC_MAX_GROUPS * 2 * TCC_BN; // one 128-lane x 64-column fp32 accumulator per group
+static_assert(TCC_SMEM <= 227 * 1024, "the chain kernel's shared memory exceeds what a Hopper CTA may use");
+constexpr int TCC_CONSUMERS = 256;                         // two warpgroups
 constexpr int TCC_TRACE_PER_SLOT = 12;
 
 __device__ __forceinline__ void tcc_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
@@ -73,7 +74,7 @@ __device__ __forceinline__ void tcc_wait(uint64_t* bar, uint32_t parity, unsigne
           dbg[1] = (unsigned long long)code | ((unsigned long long)parity << 24) | ((unsigned long long)blockIdx.x << 32);
           dbg[2] = aux;
         }
-        const unsigned kind = code & 0xFFu;                 // and the first one of every kind (5 kinds, 2 words each)
+        const unsigned kind = code & 0xFFu;                 // and the first one of every kind (2 words each)
         if (kind < 6 && atomicCAS(dbg + 4 + 2 * kind, 0ull, 1ull) == 0ull) {
           dbg[4 + 2 * kind] = (unsigned long long)code | ((unsigned long long)parity << 24) | ((unsigned long long)blockIdx.x << 32);
           dbg[5 + 2 * kind] = aux;
@@ -85,54 +86,17 @@ __device__ __forceinline__ void tcc_wait(uint64_t* bar, uint32_t parity, unsigne
   }
 }
 #define TCC_CODE(kind, slot, rank) (unsigned(kind) | (unsigned(slot) << 8) | (unsigned(rank) << 16))
-enum { WD_LOADER_DFULL = 2, WD_MMA_WFULL = 3, WD_MMA_FULL = 4, WD_EPI_DFULL = 5 };
+enum { WD_LOADER_DFULL = 2, WD_MMA_WFULL = 3, WD_MMA_FULL = 4 };
 
 // generic-proxy writes (shared AND global) -> ordered before later async-proxy (TMA / tensor core) accesses
 __device__ __forceinline__ void tcc_fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-// The MMA-issuing code runs WARP-UNIFORM (all 32 lanes execute the loop with identical values, so descriptors live in
-// uniform registers) and only the instruction is predicated on an elected lane: measured on B200 (tests/probe/
-// mma_probe2.cu) 25 cycles per 64x32x8 tcgen05.mma this way vs 50 from a single-lane branch and 150+ with per-thread
-// integer arithmetic (R2UR round trips) in the loop.
-// The descriptors are passed as their LOW words (start address >> 4 | LBO << 16); the high word of a K-major
-// SWIZZLE_128B descriptor (SBO = 1024, version 1, layout 2) is the constant 0x40004040, so the compiler moves two
-// instead of four values into uniform registers per instruction.
-constexpr uint32_t TCC_DESC_HI = 0x40004040u;
-constexpr uint32_t TCC_DESC_LO = 1u << 16;                 // LBO = 16 bytes (unused by swizzled K-major layouts)
-__device__ __forceinline__ void tcc_mma_elect(uint32_t tmem_d, uint32_t adesc_lo, uint32_t bdesc_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(adesc_lo), "r"(bdesc_lo), "r"(idesc), "r"(accumulate), "r"(TCC_DESC_HI) : "memory");
-}
-__device__ __forceinline__ void tcc_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 16 columns of fp32 accumulators (no wait: several loads may be in flight, then tcc_tmem_ld_wait)
-__device__ __forceinline__ void tcc_tmem_ld16(uint32_t taddr, float (&r)[16]) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tcc_tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ float4 tcc_hi4(float4 v) { return make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w)); }
 __device__ __forceinline__ float4 tcc_lo4(float4 v, float4 h) {
   return make_float4(tf32_lo(v.x, h.x), tf32_lo(v.y, h.y), tf32_lo(v.z, h.z), tf32_lo(v.w, h.w));
 }
 
-// [64 rows x 32 k] chunk of a row-major fp32 array -> hi / lo SWIZZLE_128B K-major images (256 epilogue threads)
+// [64 rows x 32 k] chunk of a row-major fp32 array -> hi / lo SWIZZLE_128B K-major images (the 256 consumer threads)
 __device__ __forceinline__ void tcc_convert_chunk(uint8_t* dst, const float* __restrict__ src, int ld, int k0, int ncols,
                                                   int m0, int B, int et) {
 #pragma unroll
@@ -184,7 +148,6 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
   uint64_t* full = bars;                 // [TCC_ABUFS]  bytes of the copy that starts at this buffer have landed
   uint64_t* wfull = bars + TCC_ABUFS;    // weight slices of the current slot have landed
   uint64_t* dfull = wfull + 1;           // all MMAs of the current slot have completed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dfull + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int rank = int(tcc_ctarank());
@@ -196,7 +159,6 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
   const int n0 = rank * TCC_BN;
   uint8_t* planes = args.xchg + (size_t(chain) * args.row_blocks + rb) * (size_t(TCC_PLANES) * TCC_PLANE_BYTES);
   const int npre = CH.pre ? (CH.precols + TCC_KC - 1) / TCC_KC : 0;
-  const int passes = args.passes;
   unsigned long long* tr0 = (args.trace && int(blockIdx.x) == args.trace_cta) ? args.trace : nullptr;
   if (args.wait_epoch) {                 // host pipeline: the sample kernel of this step publishes per-CTA epochs
     if (tid < args.wait_n) {
@@ -208,44 +170,38 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
   }
   step_stamp(args.step_trace, args.step_slot);
 
-  if (tid == 0) {
+  if (tid == TCC_CONSUMERS) {
     for (int i = 0; i < TCC_ABUFS + 2; ++i) mbar_init(&bars[i], 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TCC_TMEM_COLS);
-  if (warp >= 2) {
-    const int et = tid - 64;
-    if (CH.x0) tcc_convert_chunk(Xb, CH.x0, CH.x0ld, 0, CH.x0cols, m0, B, et);
-    for (int p = 0; p < npre; ++p) tcc_convert_chunk(Ab + p * TCC_A_CHUNK, CH.pre, CH.preld, p * TCC_KC, CH.precols, m0, B, et);
+  if (tid < TCC_CONSUMERS) {
+    if (CH.x0) tcc_convert_chunk(Xb, CH.x0, CH.x0ld, 0, CH.x0cols, m0, B, tid);
+    for (int p = 0; p < npre; ++p) tcc_convert_chunk(Ab + p * TCC_A_CHUNK, CH.pre, CH.preld, p * TCC_KC, CH.precols, m0, B, tid);
     fence_proxy_async();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_d = *tmem_slot;
 
-  // the pre-converted chunks: complete the first phase of their `full` barriers (the MMA issuer waits on them like on a copy)
-  if (tid == 0)
+  // the pre-converted chunks: complete the first phase of their `full` barriers (the consumers wait on them like on a copy)
+  if (tid == TCC_CONSUMERS)
     for (int p = 0; p < npre; ++p) mbar_arrive(&full[p]);
-  // per-role state.  fph: bit b = parity of the NEXT completion of full[b] this thread will wait for (MMA issuer)
+  // per-role state.  fph: bit b = parity of the NEXT completion of full[b] the consumers will wait for
   uint32_t fph = 0;
   int nact = 0;                          // slots this CTA took part in so far: phase of wfull / dfull
-  if (warp == 0 && lane == 0 && tcc_slot_active(CH.slot[0], n0)) tcc_issue_weights(CH.slot[0], rank, n0, Wb, wfull, args.flags);
+  if (tid == TCC_CONSUMERS && tcc_slot_active(CH.slot[0], n0)) tcc_issue_weights(CH.slot[0], rank, n0, Wb, wfull, args.flags);
 
   for (int l = 0; l < ns; ++l) {
     const TccSlot& S = CH.slot[l];
-    const bool act0 = tcc_group_active(S, 0, n0), act1 = tcc_group_active(S, 1, n0);
-    const bool active = act0 || act1;
+    const bool active = tcc_slot_active(S, n0);
     unsigned long long* tr = tr0 ? tr0 + TCC_TRACE_PER_SLOT * l : nullptr;
-    bool arrived = false;                  // this thread already arrived on the slot's cluster barrier (hi epilogue warps)
+    bool arrived = false;                  // this thread already arrived on the slot's cluster barrier
 
-    if (warp == 0) {
+    if (tid >= TCC_CONSUMERS) {
       // ============================== loader ==========================================================
       // Every A buffer is free here: the previous slot's MMAs completed before anyone passed the cluster barrier.
       if (lane == 0) {
         if (tr) tr[0] = tcc_gtime();
         if (active && S.nloads > 0) {
-          // the cluster's generic-proxy stores to the planes (acquired by the barrier above) -> this thread's TMA reads
+          // the cluster's stores to the planes (acquired by the barrier above) -> this thread's bulk-copy reads
           if (args.flags & 4) tcc_fence_proxy_async_all(); else asm volatile("fence.proxy.async.global;" ::: "memory");
           for (int i = 0; i < S.nloads; ++i) {
             const TccLoad L = S.ld[i];
@@ -263,227 +219,153 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
         }
       }
       __syncwarp();
-    } else if (warp == 1) {
-      // ============================== MMA issuer (warp-uniform, elected lane issues) =====================
+    } else {
+      // ============================== consumers: warpgroup g = output group g =========================
+      const int g = warp >> 2, wq = warp & 3;
+      const bool mine = tcc_group_active(S, g, n0);
+      const int rl = 16 * wq + (lane >> 2);                // accumulator rows rl and rl + 8 of the cluster's 64-row block
+      const int cl = 2 * (lane & 3);                       // accumulator columns cl + 8 j + {0, 1}, j = 0..3
       if (active) {
-        // ONE instruction per 8-deep k-step computes all partial products of the 3xTF32 split: the A chunk holds the hi
-        // image (64 rows) directly followed by the lo image (64 rows) = a 128-row operand, the weight chunk hi (32 rows)
-        // then lo (32 rows) = a 64-row operand.  D[128 x 64] = [Ah; Al] . [Bh; Bl]^T: rows 0-63 / columns 0-31 = Ah.Bh,
-        // columns 32-63 = Ah.Bl, rows 64-127 / columns 0-31 = Al.Bh (and Al.Bl, ~2^-22 relative, unused).  4 MMAs per
-        // chunk instead of 12: the issue rate of tcgen05.mma (~50 cycles with fresh descriptors) is what bounds a slot.
-        const uint32_t idesc = make_idesc(FMT_TF32, false, false, 2 * TCC_ROWS, 2 * TCC_BN);
-        // (TCC_DESC_HI << 32 | TCC_DESC_LO) == make_smem_desc(0, 16, 1024, 2)
+        const TccGroup& G = S.g[g];
+        // 3xTF32 in two wgmmas per 8-deep k-step: the weight chunk holds the hi image (32 rows) directly followed by
+        // the lo image (32 rows) = a 64-row B operand, so d1[64 x 64] = Ah . [Bh; Bl]^T (columns 0-31 Ah.Bh, 32-63
+        // Ah.Bl) and d2[64 x 32] = Al . Bh^T (Al.Bl, ~2^-22 relative, is not formed).
+        float d1[32], d2[16];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d1[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d2[i] = 0.f;
+        // this thread's epilogue operands do not depend on the chain: fetch them before the accumulator is ready
+        float eop[2][8];
+        const int npad = mine ? (G.N + 3) & ~3 : 0;
+        const bool fwd = G.epi == EPI_BIAS || G.epi == EPI_BIAS_RELU || G.epi == EPI_BIAS_TANH;
+        const bool msk = G.epi == EPI_RELU_MASK || G.epi == EPI_TANH_MASK;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int gi = m0 + rl + 8 * rr;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int gj = n0 + 8 * j + cl;
+            float2 v = make_float2(0.f, 0.f);
+            if (gj < npad) {
+              if (fwd) v = __ldg(reinterpret_cast<const float2*>(G.bias + gj));
+              else if (msk && gi < B) v = __ldg(reinterpret_cast<const float2*>(G.aux + size_t(gi) * G.ldaux + gj));
+            }
+            eop[rr][2 * j] = v.x; eop[rr][2 * j + 1] = v.y;
+          }
+        }
         const int nch = S.nchunks, boff = S.boff;
         const uint32_t wait_mask = S.wait_mask;
-        const uint32_t gstride = (uint32_t(nch) * TCC_W_CHUNK) >> 4;
-        const uint32_t w_base = (smem_u32(Wb) >> 4) | TCC_DESC_LO;
-        const uint32_t a_base = ((smem_u32(Ab) >> 4) + uint32_t(boff) * (TCC_A_CHUNK >> 4)) | TCC_DESC_LO;
-        // lane 0 waits, the warp re-converges on __syncwarp: the issue code below then runs provably converged, which is
-        // what lets the compiler keep descriptors in the uniform datapath instead of R2UR round trips per instruction
-        if (lane == 0) {
+        if (mine) {
           tcc_wait(wfull, nact & 1, args.watchdog, TCC_CODE(WD_MMA_WFULL, l, rank), nact);
-          if (tr) tr[2] = tcc_gtime();
-        }
-        __syncwarp();
-        // Chunk c of the slot's K lives in A buffer c + boff (checked at launch) and every index below derives from
-        // kernel parameters and the loop counter only.
-        for (int c = 0; c < nch; ++c) {
-          if ((wait_mask >> c) & 1u) {                    // first chunk of a bulk copy / a pre-converted chunk
-            const int b = c + boff;
-            if (lane == 0) {
+          if (tr && tid == 0) tr[2] = tcc_gtime();
+          const uint32_t w_base = smem_u32(Wb) + uint32_t(g * nch) * TCC_W_CHUNK;
+          const uint32_t a_base = smem_u32(Ab) + uint32_t(boff) * TCC_A_CHUNK;
+          wg_fence_regs(d1); wg_fence_regs(d2);
+          // Chunk c of the slot's K lives in A buffer c + boff (checked at launch)
+          for (int c = 0; c < nch; ++c) {
+            if ((wait_mask >> c) & 1u) {                  // first chunk of a bulk copy / a pre-converted chunk
+              const int b = c + boff;
               tcc_wait(&full[b], (fph >> b) & 1u, args.watchdog, TCC_CODE(WD_MMA_FULL, l, rank), b);
-              if (tr && c == 0) tr[3] = tcc_gtime();
+              if (tr && tid == 0 && c == 0) tr[3] = tcc_gtime();
             }
-            fph ^= 1u << b;
-            __syncwarp();
-          }
-          tc_fence_after_sync();
-          const uint32_t a_d = a_base + uint32_t(c) * (TCC_A_CHUNK >> 4);
-          const uint32_t acc = c != 0;
+            const uint32_t a_hi = a_base + uint32_t(c) * TCC_A_CHUNK, a_lo = a_hi + TCC_A_HALF;
+            const uint32_t w = w_base + uint32_t(c) * TCC_W_CHUNK;
+            wg_fence();
 #pragma unroll
-          for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-            if (!(g == 0 ? act0 : act1)) continue;
-            const uint32_t b_d = w_base + g * gstride + uint32_t(c) * (TCC_W_CHUNK >> 4);
-            const uint32_t d0 = tmem_d + uint32_t(g * 2 * TCC_BN);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) tcc_mma_elect(d0, a_d + 2 * ks, b_d + 2 * ks, idesc, ks ? 1u : acc);
+            for (int ks = 0; ks < 4; ++ks) {
+              const uint64_t bd = wg_desc(w + 32 * ks);
+              wg_mma_n64(d1, wg_desc(a_hi + 32 * ks), bd);
+              wg_mma_n32(d2, wg_desc(a_lo + 32 * ks), bd);
+            }
+            wg_commit();
           }
+          wg_wait<0>();
+          wg_fence_regs(d1); wg_fence_regs(d2);
+          if (tr && tid == 0) tr[4] = tcc_gtime();
         }
-        tcc_commit_elect(dfull);
-        if (tr && lane == 0) tr[4] = tcc_gtime();
-      }
-      __syncwarp();
-    } else {
-      // ============================== epilogue ========================================================
-      // TMEM lane quarter q = warp % 4.  Quarters 0/1 hold accumulator rows 0-63 (A hi image: Ah.Bh | Ah.Bl), quarters
-      // 2/3 rows 64-127 (A lo image: Al.Bh): the "lo" warp of a pair hands its 32 x 16 partial sums to the "hi" warp
-      // through shared memory (A buffer g: free, every MMA of the slot has completed), which adds the three partial
-      // products, applies the epilogue and stores.  Pair = (q, q + 2) of one 16-column half: named barrier 1 + half * 2 + (q & 1).
-      const int et = tid - 64;
-      const int q = warp & 3, half = (warp - 2) >> 2;
-      const bool hi_warp = q < 2;
-      const int row = 32 * (q & 1) + lane;                 // batch row inside the cluster's 64-row block
-      const int gi = m0 + row;
-      const bool row_ok = gi < B;
-      constexpr int SCP = 36;                              // scratch row pitch in floats (16-B aligned, spreads the banks)
-      if (active) {
-        // this thread's epilogue operands do not depend on the chain: fetch them before the accumulator is ready
-        float eop[TCC_MAX_GROUPS][16];
-#pragma unroll
-        for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) eop[g][j] = 0.f;
-          if (!hi_warp || !(g == 0 ? act0 : act1)) continue;
-          const TccGroup& G = S.g[g];
-          const int npad = (G.N + 3) & ~3;
-          const bool fwd = G.epi == EPI_BIAS || G.epi == EPI_BIAS_RELU || G.epi == EPI_BIAS_TANH;
-          const bool msk = G.epi == EPI_RELU_MASK || G.epi == EPI_TANH_MASK;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int gj = n0 + half * 16 + 4 * i;
-            if (gj >= npad) continue;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (fwd) v = __ldg(reinterpret_cast<const float4*>(G.bias + gj));
-            else if (msk && row_ok) v = __ldg(reinterpret_cast<const float4*>(G.aux + size_t(gi) * G.ldaux + gj));
-            eop[g][4 * i] = v.x; eop[g][4 * i + 1] = v.y; eop[g][4 * i + 2] = v.z; eop[g][4 * i + 3] = v.w;
-          }
-        }
-        tcc_wait(dfull, nact & 1, args.watchdog, TCC_CODE(WD_EPI_DFULL, l, rank), nact);
-        tc_fence_after_sync();
-        if (tr && et == 0) tr[5] = tcc_gtime();
+        // both warpgroups' MMAs are done: the A buffers may be overwritten and the weight buffer refilled
+        for (int c = 0; c < nch; ++c)
+          if ((wait_mask >> c) & 1u) fph ^= 1u << (c + boff);
+        asm volatile("bar.sync 1, %0;" ::"n"(TCC_CONSUMERS) : "memory");
+        if (tid == 0) mbar_arrive(dfull);
+        if (tr && tid == 0) tr[5] = tcc_gtime();
         // the resident X chunk is re-used for another array (critic fc2's action columns) now that this slot's MMAs are
         // done -- before any thread arrives on the slot's barrier
         if (S.xsrc) {
-          tcc_convert_chunk(Xb, S.xsrc, S.xld, 0, S.xcols, m0, B, et);
+          tcc_convert_chunk(Xb, S.xsrc, S.xld, 0, S.xcols, m0, B, tid);
           fence_proxy_async();                             // shared-memory writes -> the tensor core's async-proxy reads
         }
-        const uint32_t tq = tmem_d + (uint32_t(32 * q) << 16) + uint32_t(half * 16);
-        if (!hi_warp) {
-          // ---- lo rows: Al.Bh partial sums -> scratch ---------------------------------------------------------
+        if (mine) {
+          // ---- Ah.Bh + Ah.Bl + Al.Bh, epilogue ---------------------------------------------------------------
+          const int epi = G.epi;
+          float x[16];                                     // x[4 j + 2 rr + e] = (row rl + 8 rr, column cl + 8 j + e)
 #pragma unroll
-          for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-            if (!(g == 0 ? act0 : act1)) continue;
-            float t[16];
-            tcc_tmem_ld16(tq + uint32_t(g * 2 * TCC_BN), t);
-            tcc_tmem_ld_wait();
-            float* sc = reinterpret_cast<float*>(Ab + g * TCC_A_CHUNK) + row * SCP + half * 16;
+          for (int i = 0; i < 16; ++i) x[i] = (d1[i + 16] + d2[i]) + d1[i];   // the two small cross terms first
+          // the epilogue kind is decided ONCE per group, around whole loops (a per-element switch compiles to an
+          // indirect branch per element)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(sc + 4 * i) = make_float4(t[4 * i], t[4 * i + 1], t[4 * i + 2], t[4 * i + 3]);
+          for (int i = 0; i < 16; ++i) {
+            const float e = eop[(i >> 1) & 1][2 * (i >> 2) + (i & 1)];
+            if (epi == EPI_BIAS || epi == EPI_BIAS_RELU || epi == EPI_BIAS_TANH) x[i] += e;
+            else if (epi == EPI_RELU_MASK) x[i] = (e > 0.f) ? x[i] : 0.f;
+            else if (epi == EPI_TANH_MASK) x[i] *= (1.f - e * e);
           }
-          asm volatile("bar.sync %0, 64;" ::"r"(1 + half * 2 + (q & 1)) : "memory");
-        } else {
-          // ---- hi rows: Ah.Bh + Ah.Bl (TMEM) + Al.Bh (scratch), epilogue, stores -----------------------------------
-          float r[TCC_MAX_GROUPS][16], r2[TCC_MAX_GROUPS][16];
+          if (epi == EPI_BIAS_RELU) {
 #pragma unroll
-          for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-            if (!(g == 0 ? act0 : act1)) continue;
-            tcc_tmem_ld16(tq + uint32_t(g * 2 * TCC_BN), r[g]);
-            tcc_tmem_ld16(tq + uint32_t(g * 2 * TCC_BN + TCC_BN), r2[g]);
+            for (int i = 0; i < 16; ++i) x[i] = fmaxf(x[i], 0.f);
+          } else if (epi == EPI_BIAS_TANH) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+              if (n0 + 8 * (i >> 2) + cl + (i & 1) < G.N) x[i] = tanhf(x[i]);   // the action columns only
           }
-          tcc_tmem_ld_wait();
-          if (tr && et == 64) tr[6] = tcc_gtime();
-          asm volatile("bar.sync %0, 64;" ::"r"(1 + half * 2 + (q & 1)) : "memory");
-          bool any_pub = false;
 #pragma unroll
-          for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-            if (!(g == 0 ? act0 : act1)) continue;
-            const TccGroup& G = S.g[g];
-            const float* sc = reinterpret_cast<const float*>(Ab + g * TCC_A_CHUNK) + row * SCP + half * 16;
-            const int epi = G.epi;
-            float x16[16];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 t = *reinterpret_cast<const float4*>(sc + 4 * i);
-              x16[4 * i] = t.x; x16[4 * i + 1] = t.y; x16[4 * i + 2] = t.z; x16[4 * i + 3] = t.w;
-            }
-            // the epilogue kind is decided ONCE per group, around whole loops (a per-element switch compiles to an
-            // indirect branch per element: 32 BRX per group cost 1.7 us of a 5 us slot)
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x16[j] = (r2[g][j] + x16[j]) + r[g][j];   // the two small cross terms first, then the leading product
-            if (epi == EPI_BIAS || epi == EPI_BIAS_RELU || epi == EPI_BIAS_TANH) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) x16[j] += eop[g][j];
-              if (epi == EPI_BIAS_RELU) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) x16[j] = fmaxf(x16[j], 0.f);
-              } else if (epi == EPI_BIAS_TANH) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                  if (n0 + half * 16 + j < G.N) x16[j] = tanhf(x16[j]);             // warp-uniform guard: the 6 action columns only
-              }
-            } else if (epi == EPI_RELU_MASK) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) x16[j] = (eop[g][j] > 0.f) ? x16[j] : 0.f;
-            } else if (epi == EPI_TANH_MASK) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) x16[j] *= (1.f - eop[g][j] * eop[g][j]);
-            }
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int gj = n0 + half * 16 + j;
-              x16[j] = (row_ok && gj < G.N) ? x16[j] : 0.f; // pad rows / columns stay zero in the images
-              r[g][j] = x16[j];                            // kept for the row-major store after the barrier arrive
-            }
-            if (G.pub >= 0) {
-              // K-chunk `rank` of the consumers' A operand: the hi and lo images of this 64 x 32 tile are ONE contiguous
-              // 16-KB block of the plane -> staged in shared memory (A buffer 2 + g, free) in the image layout and
-              // written with a single TMA bulk store (scattered 16-B st.global cost 32 L2 transactions per warp store)
-              any_pub = true;
-              uint8_t* stg = Ab + (2 + g) * TCC_A_CHUNK;
-              const uint32_t rbase = uint32_t((row >> 3) * 1024 + (row & 7) * 128);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float4 v = make_float4(x16[4 * i], x16[4 * i + 1], x16[4 * i + 2], x16[4 * i + 3]);
-                const float4 h = tcc_hi4(v);
-                const uint32_t off = rbase + uint32_t((((half * 4 + i) ^ (row & 7)) & 7) << 4);
-                *reinterpret_cast<float4*>(stg + off) = h;
-                *reinterpret_cast<float4*>(stg + TCC_A_HALF + off) = tcc_lo4(v, h);
-              }
-            }
+          for (int i = 0; i < 16; ++i) {
+            const int gi = m0 + rl + 8 * ((i >> 1) & 1), gj = n0 + 8 * (i >> 2) + cl + (i & 1);
+            x[i] = (gi < B && gj < G.N) ? x[i] : 0.f;      // pad rows / columns stay zero in the images
           }
-          if (tr && et == 64) tr[7] = tcc_gtime();
-          if (any_pub) {                                   // uniform over the hi warps (depends on the slot only)
-            fence_proxy_async();                           // staged tiles (generic proxy) -> TMA store (async proxy)
-            asm volatile("bar.sync 5, 128;" ::: "memory"); // the four hi warps
-            if (et == 64) {
+          if (tr && tid == 0) tr[6] = tcc_gtime();
+          if (G.pub >= 0) {
+            // K-chunk `rank` of the consumers' A operand: the hi and lo images of this 64 x 32 tile are ONE contiguous
+            // 16-KB block of the plane -> staged in shared memory (A buffer 2 + g, free) in the image layout and
+            // written with a single bulk store
+            uint8_t* stg = Ab + (2 + g) * TCC_A_CHUNK;
 #pragma unroll
-              for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-                if (!(g == 0 ? act0 : act1) || S.g[g].pub < 0) continue;
-                uint8_t* img = planes + size_t(S.g[g].pub) * TCC_PLANE_BYTES + size_t(rank) * TCC_A_CHUNK;
-                asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                             ::"l"(img), "r"(smem_u32(Ab + (2 + g) * TCC_A_CHUNK)), "r"(TCC_A_CHUNK) : "memory");
-              }
+            for (int i = 0; i < 16; i += 2) {
+              const int r = rl + 8 * ((i >> 1) & 1), k = 8 * (i >> 2) + cl;
+              const float2 v = make_float2(x[i], x[i + 1]);
+              const float2 h = make_float2(tf32_hi(v.x), tf32_hi(v.y));
+              const uint32_t off = sw128_kmajor_off(r, k);
+              *reinterpret_cast<float2*>(stg + off) = h;
+              *reinterpret_cast<float2*>(stg + TCC_A_HALF + off) = make_float2(tf32_lo(v.x, h.x), tf32_lo(v.y, h.y));
+            }
+            fence_proxy_async();                           // staged tile (generic proxy) -> bulk store (async proxy)
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+            if ((tid & 127) == 0) {
+              uint8_t* img = planes + size_t(G.pub) * TCC_PLANE_BYTES + size_t(rank) * TCC_A_CHUNK;
+              asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                           ::"l"(img), "r"(smem_u32(stg)), "r"(TCC_A_CHUNK) : "memory");
               asm volatile("cp.async.bulk.commit_group;" ::: "memory");
               asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // writes complete: visible before the barrier arrive
             }
           }
-          if (tr && et == 64) tr[8] = tcc_gtime();
-          tc_fence_before_sync();                          // accumulator reads done before the next slot's MMAs overwrite it
+          if (tr && tid == 0) tr[8] = tcc_gtime();
           // The row-major outputs are read by later kernels only: they are stored AFTER this thread's barrier arrive, so
           // the cluster does not wait for them to drain.
           if (l + 1 < ns) { tcc_cluster_arrive(); arrived = true; }
+          if (G.C) {
 #pragma unroll
-          for (int g = 0; g < TCC_MAX_GROUPS; ++g) {
-            if (!(g == 0 ? act0 : act1)) continue;
-            const TccGroup& G = S.g[g];
-            if (G.C && row_ok) {
-              const int npad = (G.N + 3) & ~3;
-              float* crow = G.C + size_t(gi) * G.ldc;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int gj = n0 + half * 16 + 4 * i;
-                if (gj < npad) *reinterpret_cast<float4*>(crow + gj) = make_float4(r[g][4 * i], r[g][4 * i + 1], r[g][4 * i + 2], r[g][4 * i + 3]);
-              }
+            for (int i = 0; i < 16; i += 2) {
+              const int gi = m0 + rl + 8 * ((i >> 1) & 1), gj = n0 + 8 * (i >> 2) + cl;
+              if (gi < B && gj < npad) *reinterpret_cast<float2*>(G.C + size_t(gi) * G.ldc + gj) = make_float2(x[i], x[i + 1]);
             }
           }
         }
-        tc_fence_before_sync();                            // accumulator reads done before the next slot's MMAs overwrite it
-      }
-      if (!active && S.xsrc) {                             // (an inactive CTA did not read X in this slot)
-        tcc_convert_chunk(Xb, S.xsrc, S.xld, 0, S.xcols, m0, B, et);
+      } else if (S.xsrc) {                                 // (an inactive CTA did not read X in this slot)
+        tcc_convert_chunk(Xb, S.xsrc, S.xld, 0, S.xcols, m0, B, tid);
         fence_proxy_async();
       }
-      if (tr && et == 0) tr[9] = tcc_gtime();
+      if (tr && tid == 0) tr[9] = tcc_gtime();
     }
     if (active) ++nact;
     if (l + 1 < ns) {
@@ -492,9 +374,6 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
       if (tr && tid == 0) tr[10] = tcc_gtime();
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_d, TCC_TMEM_COLS);
   step_stamp(args.step_trace, args.step_slot + 16);
 }
 
@@ -555,7 +434,7 @@ unsigned long long* tcc_watchdog_device() {
   return dev;
 }
 }  // namespace d4pg
-// the watchdog record of the tcgen05 chain kernel (host-mapped memory: readable after a trapped launch killed the context)
+// the watchdog record of the chain kernel (host-mapped memory: readable after a trapped launch killed the context)
 extern "C" int32_t d4pg_debug_watchdog(unsigned long long* out16) {
   if (!out16) return D4PG_EINVAL;
   for (int i = 0; i < 16; ++i) out16[i] = d4pg::g_tcc_watchdog_host ? d4pg::g_tcc_watchdog_host[i] : 0ull;
@@ -682,7 +561,6 @@ int launch_mlp_tc_chain(TccArgs& a, cudaStream_t st) {
           else s.ld[s.nloads++] = TccLoad{k.plane, k.chunk, k.buf, 1};
         }
       }
-      s.nacc = 1;
       // MMA-side view: chunk c <-> A buffer c + boff, wait on full[c + boff] where a copy (or a pre-converted chunk) starts
       s.boff = s.ch[0].buf;
       s.wait_mask = 0;

@@ -1,20 +1,20 @@
-// tcgen05 cluster chains: a whole actor/critic network chain per launch with every layer on the 5th-generation
-// tensor cores (models.py:32-41,76-88 forward; autograd of ddpg.py:230,242 backward).  See mlp_tc_chain.cu.
+// Cluster chains: a whole actor/critic network chain per launch with every layer on the Hopper tensor cores (wgmma)
+// (models.py:32-41,76-88 forward; autograd of ddpg.py:230,242 backward).  See mlp_tc_chain.cu.
 #pragma once
 #include "gemm_ffma.cuh"
 
 namespace d4pg {
 
-constexpr int TCC_ROWS = 64;          // batch rows owned by one cluster (= UMMA M)
+constexpr int TCC_ROWS = 64;          // batch rows owned by one cluster (= wgmma M)
 constexpr int TCC_CLUSTER = 8;        // CTAs per cluster: CTA r owns output features [32r, 32r+32) of a layer
-constexpr int TCC_BN = 32;            // UMMA N of one group
+constexpr int TCC_BN = 32;            // output columns of one group per CTA
 constexpr int TCC_KC = 32;            // k per chunk (one 128-B SWIZZLE_128B row of tf32)
 constexpr int TCC_ABUFS = 9;          // A-chunk buffers per CTA: 0..7 one per K chunk of a 256-wide plane, 8 = the resident / tail chunk
 constexpr int TCC_MAX_SLOTS = 8, TCC_MAX_CHAINS = 3, TCC_MAX_GROUPS = 2, TCC_MAX_CHUNKS = 9, TCC_PLANES = 8;
 constexpr uint32_t TCC_A_HALF = TCC_ROWS * 128, TCC_A_CHUNK = 2 * TCC_A_HALF;      // hi image then lo image
 constexpr uint32_t TCC_W_HALF = TCC_BN * 128, TCC_W_CHUNK = 2 * TCC_W_HALF;
 constexpr uint32_t TCC_PLANE_BYTES = TCC_CLUSTER * TCC_A_CHUNK;                    // one published layer output
-constexpr int TCC_THREADS = 320;      // warp 0 loader, warp 1 MMA issuer / TMEM owner, warps 2..9 epilogue
+constexpr int TCC_THREADS = 288;      // warpgroups 0, 1: MMA + epilogue of output group 0, 1; warp 8: loader
 
 enum { TCC_SRC_IMG = 0, TCC_SRC_X = 1, TCC_SRC_PRE = 2 };
 
@@ -36,7 +36,6 @@ struct TccSlot {
   TccChunk ch[TCC_MAX_CHUNKS];
   TccLoad ld[TCC_MAX_CHUNKS];
   int ngroups, nchunks, nloads;
-  int nacc;                              // TMEM accumulators per group (1)
   int boff; unsigned wait_mask;          // MMA issuer: chunk c <-> A buffer c + boff; bit c: wait on full[c + boff] first
   const float* xsrc; int xld, xcols;     // after this slot's MMAs: re-convert the resident X chunk from this array
 };

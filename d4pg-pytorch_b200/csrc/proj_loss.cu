@@ -2,7 +2,7 @@
 // (+ the policy-loss head).  One warp per batch row; the atom support is staged in shared
 // memory and every row reduction is a warp shuffle.
 //
-// Replaces (reference, relative to /root/reference):
+// Replaces (reference, relative to its repository root):
 //   ddpg.py:142-185  DDPG.reproject2              (proj_mode 0, the live projection)
 //   ddpg.py:122-140  DDPG.reproj_categorical_dist (proj_mode 1, gamma**n, config 5)
 //   ddpg.py:217      qdist_loss = -(m*log(q+1e-10)).sum(1).mean()

@@ -1,6 +1,6 @@
 // GPU-resident prioritized replay: fp32 sum/min segment trees + SoA transition storage.
 //
-// Replaces (reference, relative to /root/reference):
+// Replaces (reference, relative to its repository root):
 //   prioritized_replay_memory.py:33-113   SegmentTree (__setitem__, reduce, _reduce_helper)
 //   prioritized_replay_memory.py:114-162  SumSegmentTree.sum/find_prefixsum_idx, MinSegmentTree.min
 //   prioritized_replay_memory.py:164-222  ReplayBuffer.add/_encode_sample
@@ -403,7 +403,7 @@ extern "C" int32_t d4pg_replay_create(int64_t size, int32_t obs_dim, int32_t act
   h->stage_host = nullptr; h->stage_dev = nullptr; h->stage_bytes = 0; h->stage_slot = 0;
   for (int i = 0; i < 2; ++i) { h->stage_ev[i] = nullptr; h->stage_busy[i] = false; }
   h->gate_flag = nullptr; h->gate_target = 0; h->gate_pending = false; h->order_ev = nullptr;
-  tree_init_kernel<<<296, 256, 0, as_stream(stream)>>>(h->sum, h->mn, h->scratch,
+  tree_init_kernel<<<2 * device_sm_count(), 256, 0, as_stream(stream)>>>(h->sum, h->mn, h->scratch,
                                                         reinterpret_cast<ReplayState*>(h->state), h->cap);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("d4pg_replay_create: %s", cudaGetErrorString(e)); delete h; return D4PG_ECUDA; }
@@ -648,7 +648,7 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
   const int64_t start = h->next_idx;
   const int64_t new_len = std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n));
   const int64_t new_next = (start + n) % h->size;
-  const int blocks = int(std::min<int64_t>(148 * 4, (n * h->obs_dim + 255) / 256));
+  const int blocks = int(std::min<int64_t>(4 * device_sm_count(), (n * h->obs_dim + 255) / 256));   // grid-stride
   ring_write_kernel<<<blocks, 256, 0, st>>>(h->obs, h->act, h->rew, h->obs2, h->done, obs, act, rew, obs2, done,
                                              n, h->obs_dim, h->act_dim, h->size, start,
                                              reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
@@ -685,11 +685,11 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
         D4PG_LAUNCH_OK();
       }
     } else {
-      leaf_fill_kernel<<<296, 256, 0, st>>>(h->sum, h->mn, h->cap, h->size, start, n,
+      leaf_fill_kernel<<<2 * device_sm_count(), 256, 0, st>>>(h->sum, h->mn, h->cap, h->size, start, n,
                                             reinterpret_cast<const ReplayState*>(h->state), h->alpha_f32);
       D4PG_LAUNCH_OK();
       for (int64_t c = h->cap / 2; c >= 1; c /= 2) {
-        const int b = int(std::min<int64_t>(296, (c + 255) / 256));
+        const int b = int(std::min<int64_t>(2 * device_sm_count(), (c + 255) / 256));
         level_rebuild_kernel<<<b, 256, 0, st>>>(h->sum, h->mn, c, c);
         D4PG_LAUNCH_OK();
       }

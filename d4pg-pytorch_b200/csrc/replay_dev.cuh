@@ -292,7 +292,7 @@ __device__ __forceinline__ void tree_write_body(const TreeArgs& a, float* red) {
 }
 
 // ---- update_priorities for up to 512 leaves with ONE round trip to L2 -------------------------------------
-// tree_write_body pays an L2 round trip per level (20 at capacity 2^20: 30-50 us, and the next step's sampler
+// tree_write_body pays an L2 round trip per level (20 at capacity 2^20, and the next step's sampler
 // waits for it).  Here every thread owns one updated leaf and first fetches the OLD value of the sibling of every
 // node on its leaf-to-root path (2 x log2(cap) independent loads, in flight together, kept in registers).  The
 // walk up is then done entirely in shared memory: at each level the new values of the touched nodes go into a

@@ -1,7 +1,6 @@
-// Blackwell (sm_100a) tensor-core primitives used by the MLP kernels: tcgen05.mma with TMEM
-// accumulators, UMMA shared-memory / instruction descriptors, mbarrier, TMA.  Thin inline-PTX
-// wrappers; bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor" tables (the
-// same fields CUTLASS names in cute/arch/mma_sm100_desc.hpp).
+// Hopper (sm_90a) tensor-core primitives used by the MLP kernels: wgmma with register accumulators,
+// the wgmma shared-memory descriptor, mbarrier, TMA.  Thin inline-PTX wrappers; bit layouts follow the
+// PTX ISA "warpgroup-level matrix shared memory layout / matrix descriptor" sections.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,33 +36,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // generic-proxy smem writes -> visible to the async proxy (tensor core / TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM -------------------------------------------------------------------------------------
-// columns: power of two >= 32.  One warp (all 32 lanes) executes alloc / dealloc.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread (thread t = lane base+t)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float (&r)[32]) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]),
-        "=r"(u[16]), "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]),
-        "=r"(u[24]), "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // ---- TMA ---------------------------------------------------------------------------------------
 // 2-D tiled bulk tensor load global -> shared (SWIZZLE_128B encoded in the tensor map), completion
 // signalled on an mbarrier by byte count.  c0 = inner (contiguous) coordinate, c1 = row coordinate.
@@ -76,65 +48,51 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 
-// ---- descriptors ------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64-bit), SWIZZLE_128B layouts only:
-//   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4     [46,48) version = 1 (Blackwell)
-//   [49,52) base offset = 0 (tiles are 1024-B aligned)      [61,64) layout type: 2 = SWIZZLE_128B
-// K-major   (rows = M/N index, 128-B rows of 32 tf32 / 64 bf16 along K):  LBO unused (=1), SBO = 8-row group stride
-// MN-major  (rows = K index,   128-B rows of 32 tf32 along M/N):          LBO = stride between 128-B M/N chunks,
-//                                                                          SBO = stride between 8-row K groups
-// layout_type: 2 = SWIZZLE_128B (16-B swizzle base), 1 = SWIZZLE_128B_BASE32B (32-B base; the only
-// MN-major layout the hardware accepts for 32-bit (tf32) operands: atoms of 4 K-rows x 128 B)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type = 2) {
-  uint64_t d = 0;
-  d |= uint64_t((saddr >> 4) & 0x3FFF);
-  d |= uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= uint64_t(1) << 46;
-  d |= uint64_t(layout_type & 7) << 61;
-  return d;
+// ---- wgmma ----------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (64-bit) of a K-major SWIZZLE_128B operand (the only layout the kernels use):
+//   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4 (unused by swizzled K-major: 1)
+//   [32,46) stride-dim byte offset >> 4 = 1024 B between 8-row groups      [49,52) base offset = 0 (tiles are
+//   1024-B aligned)      [62,64) layout type: 1 = SWIZZLE_128B
+// A 128-B row holds 32 tf32 along K; the k8 step of one wgmma advances the start address by 32 B.
+constexpr uint32_t WG_DESC_HI = (1024u >> 4) | (1u << 30);
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+  return uint64_t(((saddr >> 4) & 0x3FFFu) | (1u << 16)) | (uint64_t(WG_DESC_HI) << 32);
 }
-
-// Instruction descriptor (32-bit) for kind::tf32 / kind::f16 with fp32 accumulation:
-//   [4,6) D format: 1 = F32    [7,10) A format, [10,13) B format: 0 = F16, 1 = BF16, 2 = TF32
-//   [15] A major (0 = K, 1 = MN)   [16] B major   [17,23) N >> 3   [24,29) M >> 4
-enum : uint32_t { FMT_F16 = 0, FMT_BF16 = 1, FMT_TF32 = 2 };
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, bool a_mn, bool b_mn, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (uint32_t(a_mn) << 15) | (uint32_t(b_mn) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
+// all 128 threads of the warpgroup execute these (.sync.aligned)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across wgmma fences and waits
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues on behalf of the CTA
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
+// D[64 x N] += A[64 x 8] . B[N x 8]^T, tf32 operands from shared memory, fp32 accumulators in registers.
+// Thread t of the warpgroup holds d[i] = D[16 (t / 32) + (t % 32) / 4 + 8 ((i >> 1) & 1)][8 (i >> 2) + 2 (t % 4) + (i & 1)].
+__device__ __forceinline__ void wg_mma_n32(float (&d)[16], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(uint32_t(accumulate)) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b) : "memory");
 }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
+__device__ __forceinline__ void wg_mma_n64(float (&d)[32], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(uint32_t(accumulate)) : "memory");
-}
-// all previously issued MMAs of this thread -> arrive on an mbarrier when complete
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b) : "memory");
 }
 
-// ---- SWIZZLE_128B addressing (generic-proxy staging into the canonical UMMA layouts) ------------
+// ---- SWIZZLE_128B addressing (generic-proxy staging into the canonical wgmma layouts) ------------
 // K-major tile: element (r, k32) of a [rows x 32 fp32] block (128 B per row, 8-row groups 1024 B)
 __device__ __forceinline__ uint32_t sw128_kmajor_off(int r, int k) {
   return uint32_t((r >> 3) * 1024 + (r & 7) * 128 + ((((k >> 2) ^ (r & 7)) & 7) << 4) + ((k & 3) << 2));
 }
-// MN-major tf32 block (SWIZZLE_128B_BASE32B): element (k, mn32) of a [k rows x 32 fp32] block, 128 B per
-// k row, swizzle atom = 4 rows (512 B): the 32-B chunk index is XORed with (row & 3)
-__device__ __forceinline__ uint32_t sw128b32_mnmajor_off(int k, int mn) {
-  return uint32_t((k >> 2) * 512 + (k & 3) * 128 + ((((mn >> 3) ^ (k & 3)) & 3) << 5) + ((mn & 7) << 2));
-}
-
 // tf32 split: hi = x with the low 13 mantissa bits cleared (exactly representable in tf32),
 // lo = tf32(x - hi).  x ~= hi + lo to 2^-22 relative; A*B ~= Ah*Bh + Ah*Bl + Al*Bh.
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }

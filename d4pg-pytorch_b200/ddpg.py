@@ -1,6 +1,6 @@
 """`DDPG` with the reference's constructor and method names (ddpg.py:15-255); the body of
-`train()` is one `d4pg_learner_step` call into libd4pg_sm100.so (a CUDA graph of hand-written
-sm_100a kernels), not Python/NumPy/ATen.
+`train()` is one `d4pg_learner_step` call into libd4pg_sm90.so (a CUDA graph of hand-written
+sm_90a kernels), not Python/NumPy/ATen.
 
 Reference behaviours kept on purpose (SURVEY.md H3-H9), each switchable only explicitly:
   * importance weights are sampled but NOT used by the loss                (ddpg.py:217)
@@ -72,7 +72,7 @@ class _Learner(object):
         cfg.use_graph = 1 if ddpg.use_graph else 0
         cfg.loss_flags = ((1 if ddpg.importance_weighted else 0) | (2 if ddpg.priority == "ce" else 0) |
                           (4 if ddpg.actor_critic == "post_update" else 0))
-        # plan 1: fp32 = FFMA chain tiles; tf32x3 / tf32 = tcgen05 chain tiles (mlp_tc_chain.cu); plan 0: one launch per level
+        # plan 1: fp32 = FFMA chain tiles; tf32x3 / tf32 = wgmma chain tiles (mlp_tc_chain.cu); plan 0: one launch per level
         cfg.chain = {"levels": 0, "cluster": 1, False: 0, True: 1, 0: 0, 1: 1}[ddpg.chain]
         # device sampling: step t samples batch t+1 on a side branch; reference sampling (host-drawn uniforms): the host
         # pipeline -- train() samples batch k on the learner's ingest stream, behind the add()s issued there, while step
@@ -169,7 +169,7 @@ class DDPG:
     def __init__(self, obs_dim, act_dim, env=None, memory_size=50000, batch_size=64,
                  lr_critic=1e-4, lr_actor=1e-4, gamma=0.99, tau=0.001, prioritized_replay=True,
                  critic_dist_info=None, n_steps=1,
-                 # ---- B200 build extensions (keyword-only in spirit; reference callers never pass them)
+                 # ---- GPU build extensions (keyword-only in spirit; reference callers never pass them)
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
                  importance_weighted=False, priority="reference", actor_critic="reference"):
@@ -187,7 +187,7 @@ class DDPG:
         self.sampling, self.projection, self.precision = sampling, projection, precision
         self.use_graph, self.philox_seed, self.comm = use_graph, philox_seed, comm
         # step plan of the MLP passes: "cluster" (default) cluster-fused layer chains (exact FFMA tiles for fp32,
-        # tcgen05 tiles for tf32x3 / tf32), "levels" one launch per dependency level
+        # wgmma tiles for tf32x3 / tf32), "levels" one launch per dependency level
         self.chain = chain
         # device-side sampling only: step t already samples batch t+1 behind its own backward pass (identical results)
         self.prefetch = prefetch
@@ -196,7 +196,7 @@ class DDPG:
         assert priority in ("reference", "ce") and actor_critic in ("reference", "post_update")
         self.importance_weighted, self.priority = bool(importance_weighted), priority
         # "post_update": the actor gradient flows through the critic AFTER this step's critic update (corrected SURVEY.md
-        # H7); "reference": through the stale pre-update copy, as ddpg.py:229-247 does.  tcgen05 chain plan, one GPU.
+        # H7); "reference": through the stale pre-update copy, as ddpg.py:229-247 does.  Tensor-core chain plan, one GPU.
         self.actor_critic = actor_critic
 
         self.dist_type = critic_dist_info["type"]

@@ -37,7 +37,7 @@ def broadcast_bytes(payload, nbytes, src=0, device="cpu"):
 
 
 class Comm(object):
-    """NCCL communicator owned by libd4pg_sm100.so (d4pg_comm_*), bootstrapped through the
+    """NCCL communicator owned by libd4pg_sm90.so (d4pg_comm_*), bootstrapped through the
     torch.distributed default group."""
 
     def __init__(self, rank=None, world_size=None, device=None):

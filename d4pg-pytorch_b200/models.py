@@ -5,7 +5,7 @@ The flat buffer (layout from `d4pg_actor_layout` / `d4pg_critic_layout`) is what
 learner, the fused Adam/Polyak kernel and the gradient all-reduce operate on; the
 `fc1/fc2/fc2_2/fc3` `nn.Parameter`s are views into it, so `state_dict()` /
 `load_state_dict()` / `torch.save` interchange `.pth` files with the reference
-(main.py:367-368).  `forward` runs the sm_100a kernels through the C ABI; there is no
+(main.py:367-368).  `forward` runs the sm_90a kernels through the C ABI; there is no
 eager/CPU fallback -- on a box without a GPU the modules can be built and (de)serialised
 but `forward` raises.
 """
@@ -51,7 +51,7 @@ class _LinearView(nn.Module):
 
 
 class _FlatNet(nn.Module):
-    precision = 0        # 0 fp32 FFMA, 1 3xTF32 tcgen05, 2 TF32 tcgen05 (set per instance to switch forward())
+    precision = 0        # 0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma (set per instance to switch forward())
 
     def __init__(self, dims, device=None):
         super().__init__()

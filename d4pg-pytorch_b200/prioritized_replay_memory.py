@@ -7,7 +7,7 @@
   PrioritizedReplayBuffer(size, alpha).add/.sample(B, beta)/.update_priorities/__len__   :224-335
 
 Transitions live in SoA device arrays (obs/obs2 f32, act f32, reward f64, done u8) and the
-sum/min trees are fp32 device arrays; every operation is a call into libd4pg_sm100.so.
+sum/min trees are fp32 device arrays; every operation is a call into libd4pg_sm90.so.
 `add()` stages rows in pinned host memory and flushes them with one H2D copy + one kernel
 before anything reads the buffer, so the observable behaviour is the reference's.
 Seeded-index parity: `sample()` draws its B uniforms from Python's global `random`

@@ -1,11 +1,11 @@
 /*
- * d4pg_b200.h -- C ABI of libd4pg_sm100.so: the B200 (sm_100a) D4PG learner hot path.
+ * d4pg_b200.h -- C ABI of libd4pg_sm90.so: the H100 (sm_90a) D4PG learner hot path.
  *
  * The reference (ajgupta93/d4pg-pytorch) is pure Python and has no FFI of its own; its
  * boundary for this path is the Python class API (SURVEY.md section 8b).  Each entry point
  * below replaces the *body* of one reference method; the Python classes in
  * `d4pg-pytorch_b200/` keep the reference signatures and bind these symbols with ctypes
- * (INTEGRATION.md shows the stub).  Citations are relative to /root/reference.
+ * (INTEGRATION.md shows the stub).  Citations are relative to the reference repository's root.
  *
  * Conventions
  *   - every function returns 0 on success or a negative D4PG_E* code; never throws.
@@ -43,7 +43,7 @@ int32_t     d4pg_version(void);            /* 10000*major + 100*minor + patch */
 /* sizeof of the structs that cross this ABI by pointer (0 d4pg_learner_config_t, 1 d4pg_learner_buffers_t,
  * 2 d4pg_net_layout_t; -1 otherwise): lets a binding verify that its mirror of the struct is current */
 int32_t     d4pg_struct_size(int32_t which);
-/* compute capability of the current device as 10*major+minor (100 on B200), or <0 */
+/* compute capability of the current device as 10*major+minor (90 on H100), or <0 */
 int32_t     d4pg_device_sm(void);
 
 /* ---------------------------------------------------------------------------------------
@@ -203,7 +203,7 @@ int32_t d4pg_replay_set_len(d4pg_replay_t* h, int64_t len, int64_t next_idx, int
 /* ---------------------------------------------------------------------------------------
  * Actor / critic forward (inference entry points).  Replace actor.forward (models.py:32-41)
  * and critic.forward (models.py:76-88).  `params` = flat buffer in d4pg_*_layout order.
- * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 tcgen05 (fp32-accurate), 2 one TF32 tcgen05 pass.
+ * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 wgmma (fp32-accurate), 2 one TF32 wgmma pass.
  * ------------------------------------------------------------------------------------- */
 int32_t d4pg_actor_forward(const float* params, int32_t obs_dim, int32_t act_dim,
                            const float* s, int32_t B, float* action, float* workspace,
@@ -241,8 +241,8 @@ typedef struct {
   int32_t prioritized;        /* 1 = PrioritizedReplayBuffer path, 0 = uniform Replay path */
   double  per_beta0, per_beta_final; int64_t per_beta_iters;   /* LinearSchedule, ddpg.py:81-86 */
   double  prio_eps;           /* ddpg.py:87 */
-  int32_t precision;          /* 0 exact fp32 FFMA, 1 3xTF32 tcgen05 (hi/lo split, fp32-accurate: meets the 1e-5 parity bar),
-                                 2 one TF32 tcgen05 pass (not parity-grade) */
+  int32_t precision;          /* 0 exact fp32 FFMA, 1 3xTF32 wgmma (hi/lo split, fp32-accurate: meets the 1e-5 parity bar),
+                                 2 one TF32 wgmma pass (not parity-grade) */
   int32_t sample_mode;        /* 0 = caller uniforms/positions (parity), 1 = device Philox */
   uint64_t philox_seed;
   int32_t world_size;         /* >1: gradients are averaged over ranks before Adam */
@@ -252,11 +252,11 @@ typedef struct {
                                      ignores them, ddpg.py:217), 2 = priority = CE_i + eps instead of
                                      |sum_j m_ij q_ij| + eps (ddpg.py:221-222,253), 4 = the actor gradient flows
                                      through the critic AFTER this step's critic update (the reference uses the stale
-                                     pre-update local copy, ddpg.py:229-247); needs the tcgen05 chain plan, one GPU */
+                                     pre-update local copy, ddpg.py:229-247); needs the tensor-core chain plan, one GPU */
   int32_t chain;              /* step plan of the MLP passes (batches above 512 rows always use plan 0): 0 = one grouped launch per dependency
                                  level (18 kernels/step); 1 = cluster-fused layer chains: forward passes, dX passes
                                  and all dW are ONE launch each (7 kernels/step; precision 0: FFMA tiles, bit-identical
-                                 to plan 0; precision 1/2: tcgen05 tiles, 64-row clusters, pre-packed hi/lo weight images) */
+                                 to plan 0; precision 1/2: wgmma tiles, 64-row clusters, pre-packed hi/lo weight images) */
   int32_t prefetch;           /* 1 (sample_mode 1 only): step t samples batch t+1 on a side branch, right after its own
                                  priorities are in the trees, while its backward pass and Adam still run.  Same
                                  Philox counters and the same trees as sampling at the start of step t+1, so results
@@ -333,7 +333,7 @@ int64_t d4pg_learner_steps_done(const d4pg_learner_t* h);
  * step, which would serialise the pipeline): a caller that touched the buffer on another stream (add, update_priorities,
  * set_leaves ...) calls d4pg_replay_order_after(replay, that_stream, ingest_stream) before the next step. */
 void* d4pg_learner_ingest_stream(const d4pg_learner_t* h);
-/* The tcgen05 plans consume pre-split hi/lo weight IMAGES that the library's Adam / Polyak kernel keeps current.  Every
+/* The tensor-core plans consume pre-split hi/lo weight IMAGES that the library's Adam / Polyak kernel keeps current.  Every
  * CUDA-graph step that samples in the graph re-packs them from the fp32 parameters first (any external write is picked
  * up); the host pipeline's steps (above) re-pack only after this call -- make it whenever actor / critic / target
  * parameters were written from outside the library (state_dict load, hard update, manual edits) since the last step.
@@ -346,7 +346,7 @@ int32_t d4pg_learner_set_counters(d4pg_learner_t* h, int64_t adam_step, int64_t 
 /* ---------------------------------------------------------------------------------------
  * Data-parallel communicator (one process per GPU).  The reference has no collective (its
  * multi-worker mode is Hogwild over shared CPU memory, main.py:394-405, ddpg.py:104-108);
- * the B200 build is synchronous DP: one all-reduce of the flat [P_a+P_c] gradient per step.
+ * this build is synchronous DP: one all-reduce of the flat [P_a+P_c] gradient per step.
  * NCCL is resolved at run time (dlopen of the torch-bundled libnccl.so.2).
  * ------------------------------------------------------------------------------------- */
 int32_t d4pg_comm_unique_id(uint8_t* id128);                       /* ncclGetUniqueId, 128 bytes */
@@ -380,16 +380,15 @@ int32_t d4pg_comm_mc_ready(const d4pg_comm_t* c);
 int32_t d4pg_comm_mc_disable(d4pg_comm_t* c);
 int32_t d4pg_comm_mc_selftest(d4pg_comm_t* c, const float* src, float* out, int64_t n, d4pg_stream_t stream);
 
-/* Debug: %globaltimer (ns) phase stamps written by CTA 0 of the most recent tcgen05 GEMM launch when
+/* Debug: %globaltimer (ns) phase stamps written by the step kernels when
  * the environment variable D4PG_TC_TRACE is set (out16 = 32 x uint64, host memory). */
 int32_t d4pg_debug_tc_trace(unsigned long long* out16);
 /* first n (<= 512) stamps of the same buffer: the chain kernels write 6-8 per layer slot of one CTA */
 int32_t d4pg_debug_trace_read(unsigned long long* out, int32_t n);
-/* Watchdog record of the tcgen05 chain kernels (16 x uint64, host memory): every mbarrier wait inside them is bounded;
+/* Watchdog record of the tensor-core chain kernels (16 x uint64, host memory): every mbarrier wait inside them is bounded;
  * a wait that times out traps the launch and leaves {1, code | slot<<8 | rank<<16 | parity<<24 | block<<32, aux, ...}
  * in host-mapped memory, readable here even after the failed launch invalidated the context; words [4 + 2k, 5 + 2k] hold
- * the first timed-out wait of kind k = 1..5 (loader: ring buffer free / accumulator done, MMA: weights / A chunk landed,
- * epilogue: accumulator done).  All zero = never fired. */
+ * the first timed-out wait of kind k = 1..5 (loader: MMAs of the slot done, MMA: weights / A chunk landed).  All zero = never fired. */
 int32_t d4pg_debug_watchdog(unsigned long long* out16);
 
 #ifdef __cplusplus

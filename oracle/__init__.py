@@ -6,12 +6,11 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s `cpu_baseline` /
 
 Parity status: PINNED.  The reference has no tests or golden vectors of its own
 (SURVEY.md section 4), so the pin is the reference code itself, imported unmodified
-from /root/reference behind the 4-item compat shim in `oracle/ref_shim.py` and
-run in the build container:
+behind the 4-item compat shim in `oracle/ref_shim.py`:
   * `tests/golden/make_golden.py` dumps reference outputs to `tests/golden/*.npz`
     (NumPy 2.3.5 / torch 2.11.0 CPU dtype semantics, see SURVEY.md H11);
-  * `tests/test_oracle_vs_reference.py` re-checks the oracle against the live
-    reference whenever /root/reference exists (i.e. in the build container);
+  * `tests/test_oracle_vs_reference.py` checks the oracle against further reference
+    outputs on randomised inputs (`tests/golden/reference_live.npz`);
   * `tests/test_oracle_golden.py` checks the oracle against the committed
-    fixtures everywhere (GPU box included).
+    fixtures.
 """

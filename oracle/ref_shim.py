@@ -1,6 +1,6 @@
-"""Import the UNMODIFIED reference behind the compat shim: from /root/reference where it exists (the build
-container), else from `oracle/_ref/` -- the same modules byte-compiled by oracle/build_ref.py, which travel to the GPU
-box as build output (bench.py's CPU arm; the `-m gpu` tests never need them).
+"""Import the UNMODIFIED reference behind the compat shim: from a reference checkout (D4PG_REFERENCE_PATH) where it
+exists, else from `oracle/_ref/` -- the same modules byte-compiled by oracle/build_ref.py (bench.py's CPU arm and
+tests/golden/make_golden.py; no test needs them).
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
@@ -66,7 +66,7 @@ def load():
         nn.Module.zero_grad = zero_grad
 
     # The reference's module names (utils, models, ...) are generic: import them
-    # with /root/reference first on sys.path, then restore sys.path and move the
+    # with the reference first on sys.path, then restore sys.path and move the
     # modules out of sys.modules' generic names so they cannot shadow anything.
     names = ["utils", "models", "random_process", "replay_memory",
              "prioritized_replay_memory", "shared_adam", "ddpg"]

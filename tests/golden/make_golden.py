@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by RUNNING THE UNMODIFIED REFERENCE (/root/reference)
-behind oracle/ref_shim.py.  Only runs in the build container; the fixtures it
-writes are committed and travel to the GPU box.
+"""Generate tests/golden/*.npz by RUNNING THE UNMODIFIED REFERENCE (D4PG_REFERENCE_PATH)
+behind oracle/ref_shim.py.  Needs a reference checkout (D4PG_REFERENCE_PATH, or
+the modules byte-compiled under oracle/_ref); the fixtures it writes are committed,
+so the tests themselves never need the reference.
 
     python tests/golden/make_golden.py
 
@@ -333,7 +334,7 @@ def gen_nstep(ref):
 
 
 def gen_baseline_sizes(ref):
-    """Fixtures at the BASELINE.json sizes (VERDICT r1 item 6): c2 as configured (B=256), config-3 shapes
+    """Fixtures at the BASELINE.json sizes : c2 as configured (B=256), config-3 shapes
     (|s|=376, |a|=17, B=1024, small capacity), config-5 shapes (101 atoms, n_steps=5; train() at B=256 -- the live
     projection is reproject2 with gamma, SURVEY.md H5) and the n-step projection at B=4096."""
     gen_train(ref, "per_c2_b256", 17, 6, INFO51, 256, 2048, 2048, True, 3, 0.05, seed=21, store_data=False)
@@ -352,14 +353,79 @@ def gen_baseline_sizes(ref):
     print("projection_c5_b4096.npz:", len(out), "arrays")
 
 
+def digest(arr):
+    """SHA-256 of an array's bytes: pins a large tensor bit-for-bit in 32 bytes."""
+    import hashlib
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(arr).tobytes()).digest(), dtype=np.uint8).copy()
+
+
+def gen_live(ref):
+    """What tests/test_oracle_vs_reference.py compares the oracle against: the reference's own projection,
+    n-step projection, five train() steps and pristine-tree sampling on the inputs those tests build."""
+    out = {}
+    info = INFO51
+    rng = np.random.RandomState(5)                     # test_projection_random_vs_reproject2
+    for trial in range(6):
+        B = 97
+        d = ref.ddpg.DDPG(3, 1, batch_size=B, critic_dist_info=info, prioritized_replay=False, memory_size=4)
+        p = torch.softmax(torch.from_numpy(rng.randn(B, 51).astype(np.float32) * 3), 1).numpy()
+        r = (-60 * rng.rand(B)) if trial % 2 else -rng.randint(0, 3, B).astype(np.float64)
+        done = np.zeros(B, bool) if trial < 4 else (rng.rand(B) < 0.3)
+        if trial == 5:
+            r = -40 * rng.rand(B)
+        out["proj%d_m" % trial] = d.reproject2(p, r, done)
+    rng = np.random.RandomState(6)                     # test_h5_live_projection_ignores_n_steps
+    B = 32
+    d = ref.ddpg.DDPG(3, 1, batch_size=B, critic_dist_info=info, prioritized_replay=False, memory_size=4, n_steps=5)
+    p = torch.softmax(torch.from_numpy(rng.randn(B, 51).astype(np.float32)), 1).numpy()
+    r = -3 * rng.rand(B)
+    done = np.zeros(B, bool)
+    out["h5_live_m"] = d.reproject2(p, r, done)
+    out["h5_nstep_m"] = d.reproj_categorical_dist(p.astype(np.float64), r, done.astype(np.float64))
+    # test_five_train_steps_vs_live_reference
+    B, mem = 48, 700
+    g, l, oa, oc = ref_shim.make_learner_pair(17, 6, info, B, mem, seed=21)
+    rng = np.random.RandomState(22)
+    for i in range(650):
+        s = rng.randn(17).astype(np.float32)
+        a = rng.uniform(-1, 1, 6).astype(np.float32)
+        r = float(np.float32(-3 * rng.rand()))
+        s2 = rng.randn(17).astype(np.float32)
+        l.replayBuffer.add(s, a, r, s2, False)
+    for net, mod in (("actor", l.actor), ("critic", l.critic)):
+        for k, v in mod.state_dict().items():
+            out["train_init_%s_%s" % (net, k)] = digest(v.numpy())
+    for t in range(5):
+        random.seed(300 + t)
+        l.train(g)
+        out["train_tree_sum_%d" % t] = np.array([float(x) for x in l.replayBuffer._it_sum._value])
+        for net, mod in (("actor", l.actor), ("critic", l.critic), ("actor_target", l.actor_target),
+                         ("critic_target", l.critic_target)):
+            for k, v in mod.state_dict().items():
+                out["train_%s_%s_%d" % (net, k, t)] = digest(v.numpy())
+    # test_pristine_tree_sampling_is_f64_at_scale
+    size = 1 << 16
+    buf = ref.prioritized_replay_memory.PrioritizedReplayBuffer(size, alpha=0.6)
+    z = np.zeros(1, np.float32)
+    for i in range(size - 3):
+        buf.add(z, z, 0.0, z, False)
+    random.seed(5)
+    out["pristine_idx"] = np.array(buf._sample_proportional(2000), dtype=np.int64)
+    np.savez_compressed(os.path.join(HERE, "reference_live.npz"), **out)
+    print("reference_live.npz:", len(out), "arrays")
+
+
 def main():
     ref = ref_shim.load()
     torch.set_num_threads(1)
-    if len(sys.argv) > 1 and sys.argv[1] == "baseline":      # only the BASELINE-size fixtures (added in round 2)
+    if len(sys.argv) > 1 and sys.argv[1] == "baseline":      # only the BASELINE-size fixtures
         gen_baseline_sizes(ref)
         return
     if len(sys.argv) > 1 and sys.argv[1] == "nstep":
         gen_nstep(ref)
+        return
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        gen_live(ref)
         return
     gen_projection(ref)
     gen_tree(ref)
@@ -372,6 +438,7 @@ def main():
     gen_train(ref, "uniform_c1", 3, 1, INFO_PEND, 64, 500, 400, False, 3, 0.0, seed=13)
     gen_baseline_sizes(ref)
     gen_nstep(ref)
+    gen_live(ref)
 
 
 if __name__ == "__main__":

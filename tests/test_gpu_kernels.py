@@ -1,5 +1,5 @@
-"""CUDA kernels vs oracle / golden fixtures, called through the C ABI (libd4pg_sm100.so).
-Run on the B200 box: `pytest -m gpu`."""
+"""CUDA kernels vs oracle / golden fixtures, called through the C ABI (libd4pg_sm90.so).
+Run on an H100: `pytest -m gpu`."""
 import ctypes as C
 import random
 
@@ -40,9 +40,9 @@ def _proj(d4pg, probs, r, done, v_min, v_max, N, disc, mode, want_bins=True):
 def test_extension_is_loaded_not_a_fallback(d4pg):
     from d4pg_b200 import _lib
     assert _lib.lib().d4pg_version() >= 100
-    assert _lib.lib().d4pg_device_sm() >= 100, "expected an sm_100 (B200) device"
+    assert _lib.lib().d4pg_device_sm() == 90, "expected an sm_90 (H100) device"
     maps = open("/proc/self/maps").read()
-    assert "libd4pg_sm100.so" in maps
+    assert "libd4pg_sm90.so" in maps
 
 
 def test_projection_bit_exact_vs_golden_and_oracle(d4pg):
@@ -317,7 +317,7 @@ def test_models_seeded_init_and_forward_vs_golden(d4pg):
 
 @pytest.mark.parametrize("precision,tol", [(1, 2e-6), (2, 5e-3)])
 def test_tensor_core_forward_vs_fp32_kernels(d4pg, precision, tol):
-    """tcgen05 path (1 = 3xTF32, 2 = single-pass TF32) against the exact-fp32 FFMA kernels, odd shapes
+    """wgmma path (1 = 3xTF32, 2 = single-pass TF32) against the exact-fp32 FFMA kernels, odd shapes
     included (|s|=376 not a multiple of 32, N=101 atoms, batch not a multiple of 128)."""
     for (S, A, N, B) in ((17, 6, 51, 256), (376, 17, 101, 200), (3, 1, 51, 64)):
         torch.manual_seed(7)

@@ -51,8 +51,8 @@ CASES += [("per_c2_b256", True, "fp32"), ("per_c2_b256", True, "tf32x3"), ("per_
 @pytest.mark.parametrize("tag,use_graph,precision", CASES)
 def test_train_steps_vs_reference_golden(tag, use_graph, precision):
     """precision fp32 = exact-FFMA kernels as cluster-fused layer chains; levels = the same tiles, one grouped launch per
-    dependency level; tf32x3 = the cluster chains on tcgen05 tensor cores with the 3xTF32 split (mlp_tc_chain.cu, the
-    benchmarked plan); tf32x3_levels = tcgen05 3xTF32, one launch per level.  All must meet the same 1e-5 bar against
+    dependency level; tf32x3 = the cluster chains on the tensor cores (wgmma) with the 3xTF32 split (mlp_tc_chain.cu, the
+    benchmarked plan); tf32x3_levels = wgmma 3xTF32, one launch per level.  All must meet the same 1e-5 bar against
     the reference's fp32 CPU results."""
     import d4pg_b200 as d4pg
     g = H.load("train_%s.npz" % tag)
@@ -114,7 +114,7 @@ def test_train_steps_vs_reference_golden(tag, use_graph, precision):
     for prm, k in zip(glob.critic.parameters(), H.NAMES):
         H.check_compact(g, "adam_v_critic_%s_%d" % (k, t), oc.state[prm]["exp_avg_sq"].cpu().numpy().reshape(-1), 1e-6)
     assert loc.kernels_per_step() > 0
-    # observed slack inside the tolerances (VERDICT r1 weak 6): a regression shows up here before it fails
+    # observed slack inside the tolerances: a regression shows up here before it fails
     print("\n[parity %s graph=%s %s] worst gradient rel-L2 %.2e (bar 1e-4), post-Adam parameters: max err %.2e (bar 2.5e-4), "
           "worst fraction of elements off by > 1e-5: %.4f (bar 0.1)" % (tag, use_graph, precision, stats["grad_rel_l2"],
                                                                          stats["param_max_err"], stats["param_outlier_frac"]))

@@ -25,7 +25,7 @@ def test_data_parallel_ranks_match_single_big_batch_oracle(world, precision):
 
 @pytest.mark.parametrize("world", [2, 4, 8])
 def test_data_parallel_device_sampling_replicas_stay_identical(world):
-    """The benchmark's DP configuration (device sampling + prefetch + fused peer-memory gradient exchange, 3xTF32 tcgen05)."""
+    """The benchmark's DP configuration (device sampling + prefetch + fused peer-memory gradient exchange, 3xTF32 wgmma)."""
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
     env = dict(os.environ, D4PG_PRECISION="tf32x3", D4PG_DP_MODE="device")

@@ -1,4 +1,4 @@
-"""The tcgen05 cluster chains (d4pg-pytorch_b200/csrc/mlp_tc_chain.cu, precision="tf32x3") against a plain
+"""The wgmma cluster chains (d4pg-pytorch_b200/csrc/mlp_tc_chain.cu, precision="tf32x3") against a plain
 PyTorch float64 restatement of the same layers (models.py:32-41,76-88 forward, autograd of ddpg.py:230,242
 backward): every hidden activation, logit, delta and parameter gradient of one eager DDPG.train() step.
 Tolerance: 1e-5 absolute scaled by max(1, |ref|max) -- the 3xTF32 split is ~2^-21 relative per layer."""
