@@ -303,13 +303,11 @@ unsigned long long* debug_trace_buffer() {
   return tracing ? g_trace : nullptr;
 }
 void gemm_tc_prepare(GemmBatch& b) {
-  static const bool disabled = getenv("D4PG_NO_TMA") != nullptr;
   b.trace = debug_trace_buffer();
   gemm_batch_retile(b, TC_BM, TC_BN);
   for (int i = 0; i < b.n; ++i) {
     GemmProblem& p = b.p[i];
     p.flags &= ~(GEMM_A_TMA | GEMM_B_TMA);
-    if (disabled) continue;
     if (p.mode != GEMM_DW && tma_ok(p.A, p.lda) && encode_kmajor(&b.tmap_a[i], p.A, p.K1, p.M, p.lda, TC_BM))
       p.flags |= GEMM_A_TMA;
     if (p.mode == GEMM_FWD && tma_ok(p.Bm, p.ldb) && encode_kmajor(&b.tmap_b[i], p.Bm, p.K, p.N, p.ldb, TC_BN))

@@ -46,9 +46,27 @@ struct Workspace {
   int64_t total;
 };
 
+// The step plan, decided once from the config:
+//   PLAN_LEVELS    one grouped launch per dependency level;
+//   PLAN_CHAIN     cluster-fused chains of mlp_chain.cu: exact FFMA tiles at fp32, mma.sync 3xTF32 / TF32 tiles otherwise;
+//   PLAN_TC_CHAIN  cluster-fused wgmma chains of mlp_tc_chain.cu, with pre-packed hi/lo weight images.
+// The chain plans pay off while the batch fits one wave of clusters (a 64-row cluster chain is a latency design; 128-row
+// level tiles suit larger batches), so batches above CHAIN_MAX_BATCH rows always run the level plan.
+enum StepPlan { PLAN_LEVELS, PLAN_CHAIN, PLAN_TC_CHAIN };
+constexpr int CHAIN_MAX_BATCH = 512;
+static StepPlan step_plan(const d4pg_learner_config_t& c) {
+  if (c.batch > CHAIN_MAX_BATCH || c.chain != 1) return PLAN_LEVELS;
+  // the wgmma chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
+  if (c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256) return PLAN_TC_CHAIN;
+  return PLAN_CHAIN;
+}
+// The warm host-pipeline graph of the wgmma plan waits for the sampler by polling its per-CTA epochs from the forward
+// chains' threads (one epoch per thread)
+static_assert((CHAIN_MAX_BATCH + SAMPLE_ROWS - 1) / SAMPLE_ROWS <= TCC_THREADS, "sampler epochs exceed the chain CTA's threads");
+
 // Every 2-D plane has a row pitch that is a multiple of 4 floats (16-B rows): |s|=17 -> 20,
 // |a|=6 -> 8, N=51 -> 52.  That makes every GEMM operand TMA- and float4-addressable.
-static Workspace carve(float* base, int B, int S, int A, int N, bool chain, bool prefetch) {
+static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, bool prefetch) {
   Workspace w{};
   int64_t off = 0;
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += align4(n); return p; };
@@ -70,7 +88,7 @@ static Workspace carve(float* base, int B, int S, int A, int N, bool chain, bool
   w.a_dz3 = take(int64_t(B) * Ap); w.a_dz22 = take(int64_t(B) * H); w.a_dh2 = take(int64_t(B) * H);
   w.a_dz1 = take(int64_t(B) * H);
   w.clock = reinterpret_cast<LearnerClock*>(take(sizeof(LearnerClock) / 4 + 4));
-  w.xchg = chain ? take(std::max(chain_xchg_floats(B), tcc_xchg_floats(B))) : nullptr;
+  w.xchg = plan != PLAN_LEVELS ? take(std::max(chain_xchg_floats(B), tcc_xchg_floats(B))) : nullptr;
   w.pipe_epoch = reinterpret_cast<unsigned long long*>(take(2 * int64_t((B + SAMPLE_ROWS - 1) / SAMPLE_ROWS)));
   if (prefetch) {
     w.s_b = take(int64_t(B) * Sp); w.a_b = take(int64_t(B) * Ap); w.s2_b = take(int64_t(B) * Sp);
@@ -90,6 +108,7 @@ struct d4pg_learner {
   d4pg_learner_buffers_t buf;
   d4pg_replay* replay;
   d4pg_comm* comm;
+  StepPlan plan;
   Workspace ws;
   NetDims da, dc;
   cudaGraphExec_t graph_exec[4];   // [batch parity * 2 + cold]; only [0] without the prefetch pipeline
@@ -105,10 +124,10 @@ struct d4pg_learner {
   // profiling (d4pg_learner_profile_step): CUDA-event pair around every launch of an eager step
   cudaStream_t side; cudaEvent_t ev_fork, ev_join;
   ChainArgs chain_fwd_args, chain_bwd_args;
-  // tensor-core chains (precision >= 1): library-owned weight images + the per-step pack / chain descriptors
+  // wgmma chains (PLAN_TC_CHAIN): library-owned weight images + the per-step pack / chain descriptors
   // weight images: forward ones (packed at the start of a graph launch, then kept current by the Adam kernel) and the
   // transposed ones of the dX chains (packed every step on the side branch, off the critical path)
-  uint8_t* tcc_images; TccPackArgs tcc_pack_fwd, tcc_pack_dx; TccImage tcc_img[32]; bool tcc_ok;
+  uint8_t* tcc_images; TccPackArgs tcc_pack_fwd, tcc_pack_dx; TccImage tcc_img[32];
   cudaEvent_t ev_fork2, ev_join2;
   TccArgs tcc_fwd_args, tcc_bwd_args;
   GemmWideBatch dw_batch;
@@ -129,10 +148,6 @@ struct d4pg_learner {
   std::vector<int> ev_reps;        // how many times the launch between the event pair was repeated
 };
 
-// step plan: 0 = one grouped launch per dependency level, 1 = cluster-fused chains (mlp_chain.cu exact fp32 /
-// mlp_tc_chain.cu wgmma).  The chain plans pay off while the batch fits one wave of clusters (a 64-row cluster chain
-// is a latency design; 128-row level tiles suit larger batches), so batches above 512 rows always run plan 0.
-static int step_plan(const d4pg_learner_config_t& c) { return c.batch > 512 ? 0 : c.chain; }
 // prefetch pipeline: batch t+1 is sampled on a side branch of step t (device-side sampling only)
 static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 1; }
 // host pipeline (host-drawn uniforms / positions, cfg.prefetch): the host-facing step samples batch k on the library's
@@ -142,22 +157,14 @@ static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0
 // (update_priorities(k-1) -> add(k) -> sample(k), main.py / ddpg.py:200-255).
 static bool host_pipe(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 0 && c.use_graph != 0; }
 static bool piped(const d4pg_learner_config_t& c) { return prefetching(c) || host_pipe(c); }
-struct d4pg_learner;
-static bool inline_wait(const d4pg_learner* L);     // the warm host-pipeline graph polls the sampler's epochs itself (tensor-core chain plan)
 
 // weight matrices as the tensor-core chains consume them (F = forward image, D = transposed image for dX)
 enum { U_A_F1, U_A_F2, U_A_F22, U_A_F3, U_A_D3, U_A_D22, U_A_D2, U_AT_F1, U_AT_F2, U_AT_F22, U_AT_F3,
        U_C_F1, U_C_F2, U_C_F22, U_C_F3, U_C_D3, U_C_D22, U_C_D2H, U_C_D2A, U_CT_F1, U_CT_F2, U_CT_F22, U_CT_F3, U_COUNT };
 
-// tensor-core chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
-static bool tcc_shapes_ok(const d4pg_learner_config_t& c) {
-  return c.chain == 1 && c.batch <= 512 && c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256;
-}
+// the weight images of the wgmma chains (PLAN_TC_CHAIN only)
 static int tcc_setup(d4pg_learner* L) {
-  L->tcc_ok = false; L->tcc_images = nullptr;
   const d4pg_learner_config_t& c = L->cfg;
-  static const bool off = getenv("D4PG_NO_TCC") != nullptr;      // A/B switch: mma.sync chain tiles instead
-  if (!tcc_shapes_ok(c) || off) return D4PG_OK;
   const d4pg_learner_buffers_t& b = L->buf;
   const NetDims& da = L->da; const NetDims& dc = L->dc;
   const int S = c.obs_dim, A = c.act_dim, N = c.n_atoms, H = D4PG_HIDDEN;
@@ -199,7 +206,6 @@ static int tcc_setup(d4pg_learner* L) {
   tcc_pack_set_base(pd, L->tcc_images, fwd_bytes);
   for (int i = 0; i < U_COUNT; ++i) L->tcc_img[i] = tcc_image(is_dx[i] ? pd : pf, use_of[i]);
   (void)tcc_watchdog_device();                         // allocate outside of any stream capture
-  L->tcc_ok = true;
   return D4PG_OK;
 }
 
@@ -360,17 +366,13 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
 
   const float* Wa = b.actor; const float* Wat = b.actor_target; const float* Wc = b.critic; const float* Wct = b.critic_target;
   GemmBatch g;
-  const int plan = step_plan(c);
-  const bool tcc = plan == 1 && c.precision >= 1 && L->tcc_ok;       // tensor-core cluster chains
+  const StepPlan plan = L->plan;
   // corrected-semantics switch (SURVEY.md H7, loss_flags & 4): the actor gradient goes through the critic AFTER this
   // step's critic update (the reference uses the stale local copy, ddpg.py:229-247).  Two half steps: critic forward /
   // loss / backward / Adam, then the policy pass through the updated critic, actor backward / Adam.
-  const bool h7 = (c.loss_flags & 4) != 0;
-  D4PG_REQUIRE(!h7 || (tcc && c.world_size <= 1), D4PG_ENOTSUP, "post-update-critic actor gradient needs the tensor-core chain plan (precision tf32x3 / tf32, chain plan, batch <= 512) on one GPU");
-  const bool chain = plan == 1 && !tcc;
-  static const bool no_pre = getenv("D4PG_NO_PRE") != nullptr;          // A/B switch
-  const bool pre_ok = chain && c.precision == 0 && A <= 8 && !no_pre;   // pre-layers: fp32 tile, |a| <= 8
-  if (tcc) {
+  const bool h7 = (c.loss_flags & 4) != 0;                            // PLAN_TC_CHAIN on one GPU (checked at create)
+  const bool pre_ok = plan == PLAN_CHAIN && c.precision == 0 && A <= 8;   // pre-layers: fp32 tile, |a| <= 8
+  if (plan == PLAN_TC_CHAIN) {
     // 2''. the same three forward chains on the tensor cores (mlp_tc_chain.cu): clusters of 8 CTAs own 64 rows,
     // every layer a wgmma tile.  The hi/lo weight images are re-packed first (Adam / Polyak changed them).
     if (pack_fwd) RUN(launch_tcc_pack(L->tcc_pack_fwd, st));
@@ -379,7 +381,6 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork2, 0));
     RUN(launch_tcc_pack(L->tcc_pack_dx, L->side));
     D4PG_CUDA_OK(cudaEventRecord(L->ev_join2, L->side));
-    const TccImage* U = L->tcc_img;
     TccArgs& fa = L->tcc_fwd_args;
     tcc_args_begin(fa, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); fa.step_slot = 1;
     TccCtx cx{L, &w, &da, &dc, Wa, Wat, Wc, Wct, B, S, A, N, Sp, Ap, Np};
@@ -387,14 +388,14 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     if (h7) tcc_build_actor(fa, 1, cx, nullptr);                 // chain 1  (post-update plan) the actor alone; the critic pass follows the critic's Adam
     else tcc_build_P(fa, 1, cx);                                 // chain 1  P: actor(s) -> critic(s, actor(s))
     tcc_build_Q(fa, 2, cx, w.a, w.h1[2], w.h2[2], w.h3[2], w.out[2]);   // chain 2  Q: critic(s, a)
-    if (host_pipe(c) && !cold && inline_wait(L)) {
+    if (host_pipe(c) && !cold) {
       // warm host-pipeline variant: the batch comes from the ingest stream's sample kernel; instead of a stream event
       // (event + graph start after the sample ends) every CTA polls the epochs that kernel publishes
       fa.wait_epoch = w.pipe_epoch; fa.wait_clock = reinterpret_cast<const long long*>(&w.clock->steps_done);
       fa.wait_n = cdiv(B, SAMPLE_ROWS);
     }
     RUN(launch_mlp_tc_chain(fa, st));
-  } else if (chain) {
+  } else if (plan == PLAN_CHAIN) {
     // 2'. the three forward chains of the step as ONE cluster launch (mlp_chain.cu):
     //   chain 0  T: actor_target(s') -> critic_target(s', .)      ddpg.py:205-206
     //   chain 1  P: actor(s) -> critic(s, actor(s))                ddpg.py:236-238 (fc1 of the critic is recomputed: K=|s|)
@@ -509,12 +510,6 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   if (c.prioritized || pf) {
     D4PG_CUDA_OK(cudaEventRecord(L->ev_fork, st));
     D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork, 0));
-    static const bool copy_first = getenv("D4PG_PIPE_COPY_FIRST") != nullptr;      // A/B switch
-    if (pf && copy_first) {
-      D4PG_CUDA_OK(cudaMemcpyAsync(b.idx, bidx, size_t(B) * sizeof(int32_t), cudaMemcpyDeviceToDevice, L->side));
-      if (b.weights && c.prioritized)
-        D4PG_CUDA_OK(cudaMemcpyAsync(b.weights, bwts, size_t(B) * sizeof(float), cudaMemcpyDeviceToDevice, L->side));
-    }
     // host pipeline: the write-back also opens the ingest gate of step k+1 (its tree add / presample wait for this step's
     // loss kernel -- which advanced the sampler clock -- and for the priorities)
     if (c.prioritized) RUN(launch_tree_update(L->replay, B, bidx, b.prio, L->side, host_pipe(c) ? L->gate_flag : nullptr));
@@ -528,7 +523,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
                          q ? o.s_b : o.s, q ? o.a_b : o.a, q ? o.r_b : o.r, q ? o.s2_b : o.s2, q ? o.done_b : o.done,
                          Sp, Ap, q, L->side));
     }
-    if (pf && !copy_first) {                           // the caller-visible copies of this step's indices / IS weights (off the
+    if (pf) {                           // the caller-visible copies of this step's indices / IS weights (off the
       // path to the next batch: after the write-back and the prefetch)
       D4PG_CUDA_OK(cudaMemcpyAsync(b.idx, bidx, size_t(B) * sizeof(int32_t), cudaMemcpyDeviceToDevice, L->side));
       if (b.weights && c.prioritized)
@@ -543,7 +538,6 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   PeerInfo peers{};
   const bool peer_mode = c.world_size > 1 && comm_peer_info(L->comm, &peers);
   const int gpar = pf ? par : int(L->steps_done & 1);
-  const bool inline_sync_possible = chain || tcc;
   // Exchange shapes (D4PG_COMM_MODE=mc|mc2|pull|rs; default: "mc" from D4PG_COMM_MC_FROM = 3 ranks up when the communicator
   // set up a multicast object, else "pull").  These defaults were chosen on another GPU generation and have NOT been
   // validated on Hopper (no multi-GPU H100 measurement exists yet; tools/ab_mc8.sh compares the modes):
@@ -557,7 +551,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
                                     return !e ? 0 : (e[0] == 'p' ? 1 : (e[0] == 'r' ? 2 : (e[0] == 'm' && e[1] == 'c' && e[2] == '2' ? 4 : 3))); }();
   static const int mc_from = [] { const char* e = getenv("D4PG_COMM_MC_FROM"); return e ? atoi(e) : 3; }();
   static const int mc2_from = [] { const char* e = getenv("D4PG_COMM_MC2_FROM"); return e ? atoi(e) : 1000; }();
-  const bool mc_avail = peer_mode && peers.mc != nullptr && inline_sync_possible;
+  const bool mc_avail = peer_mode && peers.mc != nullptr && plan != PLAN_LEVELS;
   const bool peer_mc2 = mc_avail && (comm_mode == 4 || (comm_mode == 0 && peers.world >= mc2_from));
   const bool peer_mc = mc_avail && !peer_mc2 && (comm_mode == 3 || (comm_mode == 0 && peers.world >= mc_from));
   const bool peer_rs = peer_mode && !peer_mc && !peer_mc2 && comm_mode == 2;
@@ -567,9 +561,8 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   if (peer_mode) { Ga = (use_mc_buf ? peers.mc_uc : peers.x[peers.rank]) + int64_t(gpar) * peers.n; Gc = Ga + da.total; }
   if (B >= 1024)                // dW levels run split-K with fp32 atomics: the gradient buffer must start at zero
     D4PG_CUDA_OK(cudaMemsetAsync(Ga, 0, size_t(da.total + dc.total) * sizeof(float), st));
-  if (tcc) {
+  if (plan == PLAN_TC_CHAIN) {
     // 5''. both dX chains on the tensor cores (transposed weight images; masks applied by the epilogue)
-    const TccImage* U = L->tcc_img;
     D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_join2, 0));       // transposed weight images are packed
     TccArgs& ba = L->tcc_bwd_args;
     tcc_args_begin(ba, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); ba.step_slot = 5;
@@ -578,7 +571,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     if (!h7) tcc_build_bwd_P(ba, 1, cx);                         // P: policy loss (PRE-update critic weights, SURVEY.md H7)
     RUN(launch_mlp_tc_chain(ba, st));
   }
-  if (chain) {
+  if (plan == PLAN_CHAIN) {
     // 5'. both dX chains as ONE cluster launch, then every dW of the step as ONE grouped launch
     //   C: critic loss  dlogits_q  -> fc3 -> fc2_2 -> fc2[:, :H]                         ddpg.py:230
     //   P: policy loss  dlogits_pi -> fc3 -> fc2_2 -> fc2[:, H:] (d action, tanh') ->
@@ -604,7 +597,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     sl = chain_dx(Wa + da.w_off[1], la[1], H, H, EPI_RELU_MASK, w.h1[3], H, w.a_dz1, H, 0); chain_src_plane(sl, t); chain_add(cb, 1, sl);
     RUN(launch_mlp_chain(cb, st));
   }
-  if (chain || tcc) {                     // every dW of the step as ONE grouped launch
+  if (plan != PLAN_LEVELS) {              // every dW of the step as ONE grouped launch
     GemmWideBatch& gw = L->dw_batch;
     PeerSignal sig1{};
     if (peer_mode) sig1 = comm_peer_signal(peers, 0);
@@ -666,7 +659,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   // 6. data-parallel gradient exchange: ONE all-reduce over the flat [P_a + P_c] buffer
   // every rank's half of this step must be complete before Adam sums them: the chain plans signal from the dW
   // kernel and wait inside the Adam kernel; the level plan (several dW launches) uses a small barrier launch
-  const bool inline_sync = peer_mode && (chain || tcc);
+  const bool inline_sync = peer_mode && plan != PLAN_LEVELS;
   if (peer_mode && !inline_sync) RUN(comm_peer_barrier(L->comm, st));
   // reduce-scatter + all-gather over peer memory: each rank reduces its 1/N slice and pushes it to everyone
   if (peer_mc2) RUN(comm_mc_reduce_bcast(L->comm, gpar, st));
@@ -696,7 +689,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     }
   }
   aa.nseg = 2;
-  if (tcc) {                                                    // keep the forward weight images of the tensor-core chains current
+  if (plan == PLAN_TC_CHAIN) {                                  // keep the forward weight images of the tensor-core chains current
     const TccImage* U = L->tcc_img;
     const NetDims* nd[2] = {&da, &dc};
     const int base[2] = {U_A_F1, U_C_F1}, tbase[2] = {U_AT_F1, U_CT_F1};
@@ -753,7 +746,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
 
 extern "C" int64_t d4pg_learner_workspace_floats(const d4pg_learner_config_t* cfg) {
   if (!cfg) return -1;
-  return carve(nullptr, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, step_plan(*cfg) == 1, piped(*cfg)).total;
+  return carve(nullptr, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, step_plan(*cfg), piped(*cfg)).total;
 }
 
 extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d4pg_learner_buffers_t* buf,
@@ -767,7 +760,7 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
                "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma)", cfg->precision);
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
-  D4PG_REQUIRE(!(cfg->loss_flags & 4) || (tcc_shapes_ok(*cfg) && cfg->world_size <= 1), D4PG_ENOTSUP,
+  D4PG_REQUIRE(!(cfg->loss_flags & 4) || (step_plan(*cfg) == PLAN_TC_CHAIN && cfg->world_size <= 1), D4PG_ENOTSUP,
                "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1/2, chain 1, "
                "batch <= 512, obs_dim <= 32, act_dim <= 32, on one GPU");
   D4PG_REQUIRE(buf->actor && buf->actor_target && buf->critic && buf->critic_target && buf->grad_actor && buf->grad_critic &&
@@ -776,21 +769,22 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
                "d4pg_learner_create: null device buffer");
   d4pg_learner* L = new (std::nothrow) d4pg_learner();
   D4PG_REQUIRE(L, D4PG_EINVAL, "d4pg_learner_create: out of host memory");
-  L->cfg = *cfg; L->buf = *buf; L->replay = replay; L->comm = comm;
+  L->cfg = *cfg; L->buf = *buf; L->replay = replay; L->comm = comm; L->plan = step_plan(*cfg);
   L->da = actor_dims(cfg->obs_dim, cfg->act_dim);
   L->dc = critic_dims(cfg->obs_dim, cfg->act_dim, cfg->n_atoms);
   if (buf->grad_critic != buf->grad_actor + L->da.total) {
     set_error("d4pg_learner_create: grad_critic must equal grad_actor + P_a (one flat gradient buffer)");
     delete L; return D4PG_EINVAL;
   }
-  L->ws = carve(buf->workspace, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, step_plan(*cfg) == 1, piped(*cfg));
+  L->ws = carve(buf->workspace, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, L->plan, piped(*cfg));
   for (int i = 0; i < 4; ++i) { L->graph_exec[i] = nullptr; L->graph_ready[i] = false; }
   for (int i = 0; i < 2; ++i) { L->multi_exec[i] = nullptr; L->multi_ready[i] = false; }
   L->pipe_par = 0; L->last_par = 0; L->prefetch_valid = false; L->seen_gen = -1;
   L->steps_done = 0; L->kernels_per_step = 0;
   L->profiling = false;
   (void)debug_trace_buffer();          // allocate outside of any stream capture
-  if (int rc = tcc_setup(L)) { delete L; return rc; }
+  if (L->plan == PLAN_TC_CHAIN)
+    if (int rc = tcc_setup(L)) { delete L; return rc; }
   L->host_steps = 0; L->host_losses = nullptr; L->ev_in = nullptr; L->ev_out = nullptr;
   for (int i = 0; i < 4; ++i) { L->host_u[i] = nullptr; L->host_pos[i] = nullptr; L->ev_h2d[i] = nullptr; }
   for (int i = 0; i < 2; ++i) { L->loss_ring[i] = nullptr; L->ev_loss[i] = nullptr; }
@@ -916,11 +910,6 @@ static int launch_variant(d4pg_learner* L, cudaStream_t st, int par, bool cold) 
   return D4PG_OK;
 }
 
-static bool inline_wait(const d4pg_learner* L) {
-  static const bool off = getenv("D4PG_PIPE_EVENT") != nullptr;      // A/B switch: stream event instead
-  return !off && step_plan(L->cfg) == 1 && L->cfg.precision >= 1 && L->tcc_ok && cdiv(L->cfg.batch, SAMPLE_ROWS) <= TCC_THREADS;
-}
-
 // host pipeline: sample + gather batch `par` from the device copy of this step's uniforms / positions (the launch the
 // cold graph variant starts with, issued on the ingest stream instead)
 static int presample(d4pg_learner* L, int par, const double* uniforms, const int32_t* positions, cudaStream_t st) {
@@ -931,7 +920,7 @@ static int presample(d4pg_learner* L, int par, const double* uniforms, const int
   return learner_sample(L->replay, c.batch, c.prioritized, uniforms, !c.prioritized ? positions : nullptr, c.philox_seed,
                         o.clock, cp, o.idx2[par], o.wts2[par], par ? o.s_b : o.s, par ? o.a_b : o.a, par ? o.r_b : o.r,
                         par ? o.s2_b : o.s2, par ? o.done_b : o.done, pitch4(c.obs_dim), pitch4(c.act_dim), par, st,
-                        getenv("D4PG_PIPE_NO_PDL") == nullptr, o.pipe_epoch);
+                        /*dependent=*/true, o.pipe_epoch);
 }
 
 // The host-facing step: stage this step's host inputs in pinned memory, H2D, the step, order the caller after it.
@@ -984,12 +973,13 @@ static int step_host_common(d4pg_learner_t* L, const double* uniforms, const uin
     D4PG_CUDA_OK(cudaEventRecord(L->ev_ing, L->ing));
     // forward weight images: the Adam kernel keeps them current, so they are re-packed only after the caller reported a
     // parameter write of its own (d4pg_learner_weights_changed) -- behind Adam(k-1), beside the ingest stream's tail
-    if (L->images_dirty && step_plan(L->cfg) == 1 && L->cfg.precision >= 1 && L->tcc_ok) {
+    if (L->images_dirty && L->plan == PLAN_TC_CHAIN) {
       rc = launch_tcc_pack(L->tcc_pack_fwd, ls);
       if (rc) return rc;
     }
     L->images_dirty = false;
-    if (!inline_wait(L)) D4PG_CUDA_OK(cudaStreamWaitEvent(ls, L->ev_ing, 0));
+    // the wgmma forward chains poll the sampler's epochs themselves; the other plans start after its event
+    if (L->plan != PLAN_TC_CHAIN) D4PG_CUDA_OK(cudaStreamWaitEvent(ls, L->ev_ing, 0));
     rc = launch_variant(L, ls, bpar, false);
   } else {
     rc = d4pg_learner_step(L, learner_stream);

@@ -88,9 +88,6 @@ __device__ __forceinline__ void tcc_wait(uint64_t* bar, uint32_t parity, unsigne
 #define TCC_CODE(kind, slot, rank) (unsigned(kind) | (unsigned(slot) << 8) | (unsigned(rank) << 16))
 enum { WD_LOADER_DFULL = 2, WD_MMA_WFULL = 3, WD_MMA_FULL = 4 };
 
-// generic-proxy writes (shared AND global) -> ordered before later async-proxy (TMA / tensor core) accesses
-__device__ __forceinline__ void tcc_fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
 __device__ __forceinline__ float4 tcc_hi4(float4 v) { return make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w)); }
 __device__ __forceinline__ float4 tcc_lo4(float4 v, float4 h) {
   return make_float4(tf32_lo(v.x, h.x), tf32_lo(v.y, h.y), tf32_lo(v.z, h.z), tf32_lo(v.w, h.w));
@@ -120,7 +117,7 @@ __device__ __forceinline__ bool tcc_group_active(const TccSlot& S, int g, int n0
 __device__ __forceinline__ bool tcc_slot_active(const TccSlot& S, int n0) { return tcc_group_active(S, 0, n0) || tcc_group_active(S, 1, n0); }
 
 // loader lane: the CTA's weight slices of one slot -> W buffer (one bulk copy per group)
-__device__ __forceinline__ void tcc_issue_weights(const TccSlot& S, int rank, int n0, uint8_t* Wb, uint64_t* wfull, int flags) {
+__device__ __forceinline__ void tcc_issue_weights(const TccSlot& S, int rank, int n0, uint8_t* Wb, uint64_t* wfull) {
   const uint32_t gbytes = uint32_t(S.nchunks) * TCC_W_CHUNK;
   uint32_t bytes = 0;
 #pragma unroll
@@ -129,12 +126,7 @@ __device__ __forceinline__ void tcc_issue_weights(const TccSlot& S, int rank, in
   mbar_expect_tx(wfull, bytes);
 #pragma unroll
   for (int g = 0; g < TCC_MAX_GROUPS; ++g)
-    if (tcc_group_active(S, g, n0)) {
-      if (flags & 1) {                           // debugging: one copy per chunk
-        for (int c = 0; c < S.nchunks; ++c)
-          tcc_bulk_load(Wb + g * gbytes + c * TCC_W_CHUNK, S.g[g].wimg + size_t(rank) * gbytes + size_t(c) * TCC_W_CHUNK, TCC_W_CHUNK, wfull);
-      } else tcc_bulk_load(Wb + g * gbytes, S.g[g].wimg + size_t(rank) * gbytes, gbytes, wfull);
-    }
+    if (tcc_group_active(S, g, n0)) tcc_bulk_load(Wb + g * gbytes, S.g[g].wimg + size_t(rank) * gbytes, gbytes, wfull);
 }
 
 __global__ void __cluster_dims__(TCC_CLUSTER, 1, 1) __launch_bounds__(TCC_THREADS, 1)
@@ -187,7 +179,7 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
   // per-role state.  fph: bit b = parity of the NEXT completion of full[b] the consumers will wait for
   uint32_t fph = 0;
   int nact = 0;                          // slots this CTA took part in so far: phase of wfull / dfull
-  if (tid == TCC_CONSUMERS && tcc_slot_active(CH.slot[0], n0)) tcc_issue_weights(CH.slot[0], rank, n0, Wb, wfull, args.flags);
+  if (tid == TCC_CONSUMERS && tcc_slot_active(CH.slot[0], n0)) tcc_issue_weights(CH.slot[0], rank, n0, Wb, wfull);
 
   for (int l = 0; l < ns; ++l) {
     const TccSlot& S = CH.slot[l];
@@ -202,7 +194,7 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
         if (tr) tr[0] = tcc_gtime();
         if (active && S.nloads > 0) {
           // the cluster's stores to the planes (acquired by the barrier above) -> this thread's bulk-copy reads
-          if (args.flags & 4) tcc_fence_proxy_async_all(); else asm volatile("fence.proxy.async.global;" ::: "memory");
+          asm volatile("fence.proxy.async.global;" ::: "memory");
           for (int i = 0; i < S.nloads; ++i) {
             const TccLoad L = S.ld[i];
             const uint32_t bytes = uint32_t(L.count) * TCC_A_CHUNK;
@@ -215,7 +207,7 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
         // next slot's weights travel while this slot's epilogue and the barrier run
         if (l + 1 < ns && tcc_slot_active(CH.slot[l + 1], n0)) {
           if (active) tcc_wait(dfull, nact & 1, args.watchdog, TCC_CODE(WD_LOADER_DFULL, l, rank), nact);  // the weight buffer is free
-          tcc_issue_weights(CH.slot[l + 1], rank, n0, Wb, wfull, args.flags);
+          tcc_issue_weights(CH.slot[l + 1], rank, n0, Wb, wfull);
         }
       }
       __syncwarp();
@@ -516,7 +508,7 @@ int tcc_slot_group(TccArgs& a, int c, int slot, const TccImage& img, int epi, co
 int launch_mlp_tc_chain(TccArgs& a, cudaStream_t st) {
   D4PG_REQUIRE(a.nchains > 0 && a.nchains <= TCC_MAX_CHAINS, D4PG_EINVAL, "launch_mlp_tc_chain: %d chains", a.nchains);
   D4PG_REQUIRE(a.passes == 1 || a.passes == 3, D4PG_EINVAL, "launch_mlp_tc_chain: passes %d", a.passes);
-  static const int gmax = [] { const char* e = getenv("D4PG_TCC_GROUP"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : (v > 8 ? 8 : v); }();
+  constexpr int gmax = 2;                            // chunks per bulk copy of a plane (see below)
   for (int c = 0; c < a.nchains; ++c) {
     TccChain& ch = a.chain[c];
     bool x_clobbered = false;
@@ -591,7 +583,6 @@ int launch_mlp_tc_chain(TccArgs& a, cudaStream_t st) {
     attr_set = true;
   }
   a.watchdog = tcc_watchdog_device();
-  { const char* e = getenv("D4PG_TCC_FLAGS"); a.flags = e ? atoi(e) : 0; }
   unsigned long long* dbg = debug_trace_buffer();
   a.trace = dbg ? dbg + (a.step_slot == 5 ? 384 : 256) : nullptr;
   a.step_trace = dbg ? dbg + STEP_TRACE_BASE : nullptr;

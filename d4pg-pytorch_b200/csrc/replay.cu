@@ -351,16 +351,14 @@ int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* p
   a.sum = h->sum; a.mn = h->mn; a.cap = h->cap; a.log2cap = h->log2cap; a.size = h->size;
   a.n = B; a.idx = idx; a.v0 = prio; a.alpha_f32 = h->alpha_f32; a.scratch = h->scratch; a.state = reinterpret_cast<ReplayState*>(h->state);
   a.trace = (st_is_side(st) && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
-  static const bool slow_tree = getenv("D4PG_TREE_SLOW") != nullptr;      // A/B switch for profiling
-  if (!slow_tree && B <= TREE_FAST_MAX && h->log2cap < TREE_FAST_LEVELS) {
+  if (B <= TREE_FAST_MAX && h->log2cap < TREE_FAST_LEVELS) {
     int hs = 64;
     while (hs < 2 * B) hs *= 2;
     const int threads = ((B + 31) / 32) * 32;
     const size_t smem = size_t(hs) * 2 * (sizeof(int) + sizeof(float2));     // 12 KB at B = 512
     D4PG_MAX_CARVEOUT(tree_update_fast_kernel);
     const int D = std::min(4, h->log2cap);                     // 2^D CTAs, one per top-level subtree
-    static const bool sig_kernel = getenv("D4PG_PIPE_SIGNAL_KERNEL") != nullptr;      // A/B switch: separate signal kernel
-    if (D > 0 && !sig_kernel) { a.gate = gate; gate = nullptr; }   // the last CTA opens the gate itself
+    if (D > 0) { a.gate = gate; gate = nullptr; }   // the last CTA opens the gate itself
     tree_update_fast_kernel<<<1 << D, threads, smem, st>>>(a, hs, D);
   } else {
     D4PG_MAX_CARVEOUT(tree_write_kernel<TREE_UPDATE>);
@@ -658,8 +656,7 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
     // the last launched learner step's priority write-back -- inside the first tree kernel when that is the 1-CTA fast one
     const int64_t n1g = std::min<int64_t>(n, h->size - start);
     const unsigned long long* gflag = nullptr; unsigned long long gtarget = 0;
-    static const bool gate_kernel = getenv("D4PG_PIPE_GATE_KERNEL") != nullptr;      // A/B switch: separate 1-thread gate kernel
-    if (h->gate_pending && !gate_kernel && n <= 65536 && n1g <= TREE_ADD_FAST_MAX && h->log2cap < 32) {
+    if (h->gate_pending && n <= 65536 && n1g <= TREE_ADD_FAST_MAX && h->log2cap < 32) {
       gflag = h->gate_flag; gtarget = h->gate_target; h->gate_pending = false;
     } else {
       int grc = replay_gate_consume(h, st); if (grc) return grc;
