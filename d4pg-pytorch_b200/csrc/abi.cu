@@ -75,7 +75,7 @@ __global__ void softmax_rows_kernel(const float* logits, float* probs, int B, in
 using namespace d4pg;
 
 extern "C" const char* d4pg_last_error(void) { return g_err; }
-extern "C" int32_t d4pg_version(void) { return 100; }   /* 0.1.0 */
+extern "C" int32_t d4pg_version(void) { return 200; }   /* 0.2.0 */
 /* sizeof of the structs that cross the ABI by pointer: a binding whose mirror has another size is out of date */
 extern "C" int32_t d4pg_struct_size(int32_t which) {
   switch (which) {
@@ -119,7 +119,7 @@ extern "C" int32_t d4pg_actor_forward(const float* params, int32_t obs_dim, int3
                                       const float* s, int32_t B, float* action, float* workspace,
                                       int32_t precision, d4pg_stream_t stream) {
   D4PG_REQUIRE(params && s && action && workspace && B > 0, D4PG_EINVAL, "d4pg_actor_forward: null/empty argument");
-  D4PG_REQUIRE(precision >= 0 && precision <= 2, D4PG_ENOTSUP, "d4pg_actor_forward: unknown precision %d", precision);
+  D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_actor_forward: unknown precision %d", precision);
   const NetDims d = actor_dims(obs_dim, act_dim);
   const int H = D4PG_HIDDEN;
   float* h1 = workspace; float* h2 = h1 + size_t(B) * H; float* h3 = h2 + size_t(B) * H;
@@ -142,7 +142,7 @@ extern "C" int32_t d4pg_critic_forward(const float* params, int32_t obs_dim, int
                                        const float* s, const float* a, int32_t B, float* probs, float* logits,
                                        float* workspace, int32_t precision, d4pg_stream_t stream) {
   D4PG_REQUIRE(params && s && a && workspace && B > 0 && (probs || logits), D4PG_EINVAL, "d4pg_critic_forward: null/empty argument");
-  D4PG_REQUIRE(precision >= 0 && precision <= 2, D4PG_ENOTSUP, "d4pg_critic_forward: unknown precision %d", precision);
+  D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_critic_forward: unknown precision %d", precision);
   D4PG_REQUIRE(n_atoms >= 2 && n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_critic_forward: n_atoms out of range");
   const NetDims d = critic_dims(obs_dim, act_dim, n_atoms);
   const int H = D4PG_HIDDEN;

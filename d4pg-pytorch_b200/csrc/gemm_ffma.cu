@@ -162,6 +162,7 @@ bool gemm_batch_has_splitk(const GemmBatch& b) {
 }
 int gemm_launch(GemmBatch& b, int precision, cudaStream_t st) {
   if (precision == 0) return gemm_batch_launch(b, st);
+  if (precision == 3) return gemm_bf16_batch_launch(b, st);
   gemm_tc_prepare(b);                 // retiles the problems for the wgmma tiles and encodes the TMA maps
   return gemm_tc_batch_launch(b, precision == 1 ? 3 : 1, st);
 }

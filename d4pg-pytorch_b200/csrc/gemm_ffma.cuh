@@ -57,7 +57,9 @@ void gemm_batch_retile(GemmBatch& b, int bm, int bn);
 bool gemm_batch_has_splitk(const GemmBatch& b);
 void gemm_tc_prepare(GemmBatch& b);                                             // TMA eligibility + tensor maps
 int gemm_tc_batch_launch(const GemmBatch& b, int passes, cudaStream_t st);      // wgmma (128x32 tiles)
-// precision: 0 = fp32 FFMA, 1 = 3xTF32 wgmma (fp32-accurate), 2 = 1xTF32 wgmma
+int gemm_bf16_batch_launch(GemmBatch& b, cudaStream_t st);                      // bf16 wgmma (retiles to 128x32)
+// precision: 0 = fp32 FFMA, 1 = 3xTF32 wgmma (fp32-accurate), 2 = 1xTF32 wgmma,
+//            3 = bf16 wgmma (operands rounded to bf16, fp32 accumulate)
 int gemm_launch(GemmBatch& b, int precision, cudaStream_t st);
 
 }  // namespace d4pg

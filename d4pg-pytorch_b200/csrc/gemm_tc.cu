@@ -17,7 +17,7 @@
 //   * split-K for dW over a large batch (slices accumulate into the pre-zeroed C with fp32 atomics),
 //   * epilogue straight from the accumulator registers: bias / ReLU / tanh / activation-derivative
 //     masks fused.
-#include "gemm_ffma.cuh"
+#include "gemm_tc_epi.cuh"
 #include "tc_common.cuh"
 #include <stdlib.h>
 
@@ -191,44 +191,8 @@ __device__ __forceinline__ void tc_tile(const GemmProblem& P, const CUtensorMap*
   wg_wait<0>();
   wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
 
-  // ---- epilogue from the accumulator registers: 2 x 2 rows x 8 column pairs per thread -------------
-  const float* bias = (P.epi == EPI_BIAS || P.epi == EPI_BIAS_RELU || P.epi == EPI_BIAS_TANH) ? P.bias : nullptr;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int gi = m0 + 64 * h + 16 * warp + (lane >> 2) + 8 * rr;
-      if (gi >= P.M) continue;
-      float* crow = P.C + size_t(gi) * P.ldc;
-      const float* arow = P.aux ? P.aux + size_t(gi) * P.ldaux : nullptr;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int gj = n0 + 8 * (i >> 1) + 2 * (lane & 3) + (i & 1);
-        if (gj >= P.N) continue;
-        float x = acc[h][(i >> 1) * 4 + rr * 2 + (i & 1)];
-        switch (P.epi) {
-          case EPI_BIAS: x += __ldg(bias + gj); break;
-          case EPI_BIAS_RELU: x = fmaxf(x + __ldg(bias + gj), 0.f); break;
-          case EPI_BIAS_TANH: x = tanhf(x + __ldg(bias + gj)); break;
-          case EPI_RELU_MASK: x = (__ldg(arow + gj) > 0.f) ? x : 0.f; break;
-          case EPI_TANH_MASK: { const float t = __ldg(arow + gj); x *= (1.f - t * t); } break;
-          default: break;
-        }
-        if (split) atomicAdd(crow + gj, x);        // C pre-zeroed
-        else crow[gj] = x;
-      }
-    }
-  }
-  // ---- dW: bias gradient = column sums of dZ (rows of A), exact fp32, tn == 0 tiles only -------------
-  if (MODE == GEMM_DW && P.bias_grad != nullptr && tn == 0) {
-    const int m = m0 + tid;                                   // 128 threads <-> 128 A rows
-    if (m < P.M) {
-      float s = 0.f;
-      for (int k = kbeg; k < kend; ++k) s += __ldg(P.A + size_t(k) * P.lda + m);    // coalesced across threads
-      if (split) atomicAdd(P.bias_grad + m, s);
-      else P.bias_grad[m] = s;
-    }
-  }
+  tc_epilogue(P, acc, m0, n0, split, warp, lane);
+  if (MODE == GEMM_DW && P.bias_grad != nullptr && tn == 0) tc_bias_grad(P, m0, kbeg, kend, split);
 }
 
 __global__ void __launch_bounds__(TC_THREADS) gemm_tc_kernel(const __grid_constant__ GemmBatch batch, int passes) {

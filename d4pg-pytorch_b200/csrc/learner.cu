@@ -47,7 +47,7 @@ struct Workspace {
 };
 
 // The step plan, decided once from the config:
-//   PLAN_LEVELS    one grouped launch per dependency level;
+//   PLAN_LEVELS    one grouped launch per dependency level (the only plan of precision 3, bf16);
 //   PLAN_CHAIN     cluster-fused chains of mlp_chain.cu: exact FFMA tiles at fp32, mma.sync 3xTF32 / TF32 tiles otherwise;
 //   PLAN_TC_CHAIN  cluster-fused wgmma chains of mlp_tc_chain.cu, with pre-packed hi/lo weight images.
 // The chain plans pay off while the batch fits one wave of clusters (a 64-row cluster chain is a latency design; 128-row
@@ -56,6 +56,7 @@ enum StepPlan { PLAN_LEVELS, PLAN_CHAIN, PLAN_TC_CHAIN };
 constexpr int CHAIN_MAX_BATCH = 512;
 static StepPlan step_plan(const d4pg_learner_config_t& c) {
   if (c.batch > CHAIN_MAX_BATCH || c.chain != 1) return PLAN_LEVELS;
+  if (c.precision == 3) return PLAN_LEVELS;             // bf16: the level kernel only (no bf16 chain tiles)
   // the wgmma chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
   if (c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256) return PLAN_TC_CHAIN;
   return PLAN_CHAIN;
@@ -756,12 +757,12 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   D4PG_REQUIRE(cfg->n_atoms >= 2 && cfg->n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_learner_create: n_atoms must be in [2,%d]", D4PG_MAX_ATOMS);
   D4PG_REQUIRE(cfg->v_max > cfg->v_min, D4PG_EINVAL, "d4pg_learner_create: v_max <= v_min");
   D4PG_REQUIRE(cfg->proj_mode == 0 || cfg->proj_mode == 1, D4PG_EINVAL, "d4pg_learner_create: proj_mode must be 0/1");
-  D4PG_REQUIRE(cfg->precision >= 0 && cfg->precision <= 2, D4PG_ENOTSUP,
-               "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma)", cfg->precision);
+  D4PG_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, D4PG_ENOTSUP,
+               "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma, 3 bf16 wgmma)", cfg->precision);
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
   D4PG_REQUIRE(!(cfg->loss_flags & 4) || (step_plan(*cfg) == PLAN_TC_CHAIN && cfg->world_size <= 1), D4PG_ENOTSUP,
-               "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1/2, chain 1, "
+               "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1 or 2 (not 0 or 3), chain 1, "
                "batch <= 512, obs_dim <= 32, act_dim <= 32, on one GPU");
   D4PG_REQUIRE(buf->actor && buf->actor_target && buf->critic && buf->critic_target && buf->grad_actor && buf->grad_critic &&
                buf->adam_m_actor && buf->adam_v_actor && buf->adam_m_critic && buf->adam_v_critic &&
@@ -1132,6 +1133,9 @@ extern "C" int32_t d4pg_learner_tensor(d4pg_learner_t* L, const char* name, void
       {"h1_c", w.h1[2], B * 256, 256}, {"h2_c", w.h2[2], B * 256, 256}, {"h3_c", w.h3[2], B * 256, 256},
       {"h1_a", w.h1[3], B * 256, 256}, {"h2_a", w.h2[3], B * 256, 256}, {"h3_a", w.h3[3], B * 256, 256},
       {"h2_p", w.h2[4], B * 256, 256}, {"h3_p", w.h3[4], B * 256, 256},
+      {"h1_at", w.h1[0], B * 256, 256}, {"h2_at", w.h2[0], B * 256, 256}, {"h3_at", w.h3[0], B * 256, 256},
+      {"h1_ct", w.h1[1], B * 256, 256}, {"h2_ct", w.h2[1], B * 256, 256}, {"h3_ct", w.h3[1], B * 256, 256},
+      {"p_dz22", w.p_dz22, B * 256, 256}, {"p_dz2", w.p_dz2, B * 256, 256},
       {"c_dz22", w.c_dz22, B * 256, 256}, {"c_dz2", w.c_dz2, B * 256, 256}, {"c_dz1", w.c_dz1, B * 256, 256},
       {"a_dz3", w.a_dz3, B * Ap, Ap}, {"a_dz22", w.a_dz22, B * 256, 256}, {"a_dh2", w.a_dh2, B * 256, 256},
       {"a_dz1", w.a_dz1, B * 256, 256}};

@@ -53,7 +53,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
 //   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4 (unused by swizzled K-major: 1)
 //   [32,46) stride-dim byte offset >> 4 = 1024 B between 8-row groups      [49,52) base offset = 0 (tiles are
 //   1024-B aligned)      [62,64) layout type: 1 = SWIZZLE_128B
-// A 128-B row holds 32 tf32 along K; the k8 step of one wgmma advances the start address by 32 B.
+// A 128-B row holds 32 tf32 (or 64 bf16) along K; the k8 (bf16: k16) step of one wgmma advances the start address by 32 B.
 constexpr uint32_t WG_DESC_HI = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
   return uint64_t(((saddr >> 4) & 0x3FFFu) | (1u << 16)) | (uint64_t(WG_DESC_HI) << 32);
@@ -87,11 +87,32 @@ __device__ __forceinline__ void wg_mma_n64(float (&d)[32], uint64_t a, uint64_t 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(a), "l"(b) : "memory");
 }
+// D[64 x 32] += A[64 x 16] . B[32 x 16]^T, bf16 operands (both K-major: transpose flags 0) from shared memory, fp32
+// accumulators in registers with the same d[] layout as wg_mma_n32.  A 128-B row holds 64 bf16, so the k16 step also
+// advances the descriptor's start address by 32 B.
+__device__ __forceinline__ void wg_mma_n32_bf16(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b) : "memory");
+}
 
 // ---- SWIZZLE_128B addressing (generic-proxy staging into the canonical wgmma layouts) ------------
 // K-major tile: element (r, k32) of a [rows x 32 fp32] block (128 B per row, 8-row groups 1024 B)
 __device__ __forceinline__ uint32_t sw128_kmajor_off(int r, int k) {
   return uint32_t((r >> 3) * 1024 + (r & 7) * 128 + ((((k >> 2) ^ (r & 7)) & 7) << 4) + ((k & 3) << 2));
+}
+// the same layout for 2-byte elements: element (r, k64) of a [rows x 64 bf16] block, 8 elements per 16-B chunk
+__device__ __forceinline__ uint32_t sw128_kmajor_off_b16(int r, int k) {
+  return uint32_t((r >> 3) * 1024 + (r & 7) * 128 + ((((k >> 3) ^ (r & 7)) & 7) << 4) + ((k & 7) << 1));
+}
+// two fp32 -> one bf16x2 word, each rounded to nearest even; `lo` lands in the low half (the lower k / address)
+__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
 }
 // tf32 split: hi = x with the low 13 mantissa bits cleared (exactly representable in tf32),
 // lo = tf32(x - hi).  x ~= hi + lo to 2^-22 relative; A*B ~= Ah*Bh + Ah*Bl + Al*Bh.

@@ -65,7 +65,7 @@ class _Learner(object):
             cfg.prio_eps = ddpg.prioritized_replay_eps
         else:
             cfg.per_beta0, cfg.per_beta_final, cfg.per_beta_iters, cfg.prio_eps = 1.0, 1.0, 1, 1e-6
-        cfg.precision = {"fp32": 0, "tf32x3": 1, "tf32": 2}[ddpg.precision]
+        cfg.precision = {"fp32": 0, "tf32x3": 1, "tf32": 2, "bf16": 3}[ddpg.precision]
         cfg.sample_mode = 0 if ddpg.sampling == "reference" else 1
         cfg.philox_seed = int(ddpg.philox_seed)
         cfg.world_size = ddpg.comm.world_size if ddpg.comm is not None else 1
@@ -73,6 +73,7 @@ class _Learner(object):
         cfg.loss_flags = ((1 if ddpg.importance_weighted else 0) | (2 if ddpg.priority == "ce" else 0) |
                           (4 if ddpg.actor_critic == "post_update" else 0))
         # plan 1: fp32 = FFMA chain tiles; tf32x3 / tf32 = wgmma chain tiles (mlp_tc_chain.cu); plan 0: one launch per level
+        # (bf16 always runs plan 0)
         cfg.chain = {"levels": 0, "cluster": 1, False: 0, True: 1, 0: 0, 1: 1}[ddpg.chain]
         # device sampling: step t samples batch t+1 on a side branch; reference sampling (host-drawn uniforms): the host
         # pipeline -- train() samples batch k on the learner's ingest stream, behind the add()s issued there, while step
@@ -183,7 +184,8 @@ class DDPG:
         self.env = env
         self.device = torch.device(device) if device is not None else default_device()
         assert sampling in ("reference", "device") and projection in ("reference", "nstep")
-        assert precision in ("fp32", "tf32x3", "tf32")
+        # "bf16": every MLP GEMM operand rounded to bf16, fp32 accumulate; runs the "levels" plan whatever `chain` says
+        assert precision in ("fp32", "tf32x3", "tf32", "bf16")
         self.sampling, self.projection, self.precision = sampling, projection, precision
         self.use_graph, self.philox_seed, self.comm = use_graph, philox_seed, comm
         # step plan of the MLP passes: "cluster" (default) cluster-fused layer chains (exact FFMA tiles for fp32,

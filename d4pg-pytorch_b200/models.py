@@ -51,7 +51,7 @@ class _LinearView(nn.Module):
 
 
 class _FlatNet(nn.Module):
-    precision = 0        # 0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma (set per instance to switch forward())
+    precision = 0        # 0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma, 3 bf16 wgmma (set per instance to switch forward())
 
     def __init__(self, dims, device=None):
         super().__init__()

@@ -203,7 +203,9 @@ int32_t d4pg_replay_set_len(d4pg_replay_t* h, int64_t len, int64_t next_idx, int
 /* ---------------------------------------------------------------------------------------
  * Actor / critic forward (inference entry points).  Replace actor.forward (models.py:32-41)
  * and critic.forward (models.py:76-88).  `params` = flat buffer in d4pg_*_layout order.
- * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 wgmma (fp32-accurate), 2 one TF32 wgmma pass.
+ * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 wgmma (fp32-accurate), 2 one TF32 wgmma pass,
+ * 3 one bf16 wgmma pass (each GEMM operand rounded to bf16, round to nearest even; fp32 accumulate, fp32 bias and
+ * activation; inputs, weights and outputs stay fp32).  Any other value fails with D4PG_ENOTSUP.
  * ------------------------------------------------------------------------------------- */
 int32_t d4pg_actor_forward(const float* params, int32_t obs_dim, int32_t act_dim,
                            const float* s, int32_t B, float* action, float* workspace,
@@ -242,7 +244,10 @@ typedef struct {
   double  per_beta0, per_beta_final; int64_t per_beta_iters;   /* LinearSchedule, ddpg.py:81-86 */
   double  prio_eps;           /* ddpg.py:87 */
   int32_t precision;          /* 0 exact fp32 FFMA, 1 3xTF32 wgmma (hi/lo split, fp32-accurate: meets the 1e-5 parity bar),
-                                 2 one TF32 wgmma pass (not parity-grade) */
+                                 2 one TF32 wgmma pass (not parity-grade), 3 one bf16 wgmma pass: the operands of every
+                                 MLP GEMM (X and W forward, dZ and W for dX, dZ and X for dW) are rounded to bf16 (nearest
+                                 even) as they are staged, products accumulate in fp32; activations, deltas, bias terms,
+                                 bias gradients, the loss heads, Adam and the weights stay fp32 (not parity-grade) */
   int32_t sample_mode;        /* 0 = caller uniforms/positions (parity), 1 = device Philox */
   uint64_t philox_seed;
   int32_t world_size;         /* >1: gradients are averaged over ranks before Adam */
@@ -256,7 +261,8 @@ typedef struct {
   int32_t chain;              /* step plan of the MLP passes (batches above 512 rows always use plan 0): 0 = one grouped launch per dependency
                                  level (18 kernels/step); 1 = cluster-fused layer chains: forward passes, dX passes
                                  and all dW are ONE launch each (7 kernels/step; precision 0: FFMA tiles, bit-identical
-                                 to plan 0; precision 1/2: wgmma tiles, 64-row clusters, pre-packed hi/lo weight images) */
+                                 to plan 0; precision 1/2: wgmma tiles, 64-row clusters, pre-packed hi/lo weight images).
+                                 Precision 3 always runs plan 0 */
   int32_t prefetch;           /* 1 (sample_mode 1 only): step t samples batch t+1 on a side branch, right after its own
                                  priorities are in the trees, while its backward pass and Adam still run.  Same
                                  Philox counters and the same trees as sampling at the start of step t+1, so results
