@@ -92,6 +92,9 @@ _PROTOS = {
     "d4pg_replay_set_len": (C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int32, _P]),
     "d4pg_actor_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, _P]),
     "d4pg_critic_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, C.c_int32, _P]),
+    "d4pg_actor_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
+    "d4pg_critic_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P,
+                                         _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_adam_polyak": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
                                      C.c_int64, C.c_double, C.c_float, _P]),
     "d4pg_polyak": (C.c_int32, [_P, _P, C.c_int64, C.c_double, _P]),

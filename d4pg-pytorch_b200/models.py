@@ -12,6 +12,7 @@ but `forward` raises.
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .utils import default_device
@@ -52,6 +53,10 @@ class _LinearView(nn.Module):
 
 class _FlatNet(nn.Module):
     precision = 0        # 0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma, 3 bf16 wgmma (set per instance to switch forward())
+    # True: with grad mode on and a parameter or input requiring grad, forward() records an autograd node whose backward
+    # runs d4pg_*_backward (loss.backward() fills .grad -- kept in the flat gradient buffer -- and d input).
+    # False: forward() returns a plain tensor.
+    differentiable = False
 
     def __init__(self, dims, device=None):
         super().__init__()
@@ -100,11 +105,31 @@ class _FlatNet(nn.Module):
         return out
 
     def flat_grads(self):
-        """Flat gradient buffer (allocated on first use); `.grad` of every parameter views it."""
+        """Flat gradient buffer (allocated on first use); `.grad` of every parameter views it.  A `.grad` that autograd
+        put elsewhere (a parameter used outside this module's forward, or one reset to None) is taken over: its values
+        are copied into the buffer (None counts as zero) and `.grad` views the buffer again."""
         if self._flat_grad is None:
             self._flat_grad = torch.zeros_like(self._flat)
-            self._bind_grads()
+        self._adopt_grads()
         return self._flat_grad
+
+    def _grad_in_flat(self, g):
+        f = self._flat_grad
+        return (f is not None and g is not None and g.device == f.device
+                and f.data_ptr() <= g.data_ptr() < f.data_ptr() + f.numel() * f.element_size())
+
+    def _adopt_grads(self):
+        for name, (w, b) in zip(_LAYER_NAMES, self._views(self._flat_grad)):
+            layer = getattr(self, name)
+            for p, view in ((layer.weight, w), (layer.bias, b)):
+                if self._grad_in_flat(p.grad):
+                    continue
+                with torch.no_grad():
+                    if p.grad is None:
+                        view.zero_()
+                    else:
+                        view.copy_(p.grad)
+                p.grad = view
 
     def adopt_flat(self, flat):
         """Alias another network's flat parameter storage (local == global model,
@@ -132,6 +157,13 @@ class _FlatNet(nn.Module):
     def zero_grad(self, set_to_none=False):
         if self._flat_grad is not None:
             self._flat_grad.zero_()
+        for p in self._param_list():          # a .grad outside the flat buffer (see flat_grads)
+            if p.grad is not None and not self._grad_in_flat(p.grad):
+                if set_to_none:
+                    p.grad = None
+                else:
+                    with torch.no_grad():
+                        p.grad.zero_()
 
     def _workspace(self, B):
         need = 3 * B * HIDDEN
@@ -150,14 +182,50 @@ class _FlatNet(nn.Module):
         assert x.shape[1] == width, "expected input width %d, got %s" % (width, tuple(x.shape))
         return x.contiguous()
 
+    # ---- autograd path (differentiable=True) ----------------------------------------------
+    def _param_list(self):
+        out = []
+        for name in _LAYER_NAMES:
+            layer = getattr(self, name)
+            out += [layer.weight, layer.bias]
+        return out
+
+    def _use_autograd(self, inputs):
+        if not (self.differentiable and torch.is_grad_enabled()):
+            return False
+        return (any(torch.is_tensor(x) and x.requires_grad for x in inputs)
+                or any(p.requires_grad for p in self._param_list()))
+
+    def _grad_params(self):
+        """The parameters as autograd inputs.  Their .grad is bound to the flat gradient buffer first, so backward
+        accumulates there, where zero_grad(), SharedAdam.step() and the learner read the gradients."""
+        params = self._param_list()
+        if any(p.requires_grad for p in params):
+            self.flat_grads()
+        return params
+
+    def _as_grad_input(self, x, width):
+        """_as_input without the detach: the device / dtype conversion stays on the autograd graph."""
+        if self._flat.device.type != "cuda":
+            raise _lib.D4PGError("the D4PG kernels run only on a CUDA device (sm_90a); this module lives on %s"
+                                 % self._flat.device)
+        if not torch.is_tensor(x):
+            x = torch.as_tensor(np.asarray(x))
+        x = x.to(device=self._flat.device, dtype=torch.float32)
+        if x.dim() == 1:
+            x = x.view(1, -1)
+        assert x.shape[1] == width, "expected input width %d, got %s" % (width, tuple(x.shape))
+        return x.contiguous()
+
 
 class actor(_FlatNet):
     """models.py:15-41.  fc1 -> ReLU -> fc2 -> fc2_2 -> ReLU -> fc3 -> tanh
     (no ReLU between fc2 and fc2_2, SURVEY.md H9)."""
 
-    def __init__(self, input_size, output_size, device=None):
+    def __init__(self, input_size, output_size, device=None, differentiable=False):
         self.input_size, self.output_size = input_size, output_size
         super().__init__([(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)], device)
+        self.differentiable = bool(differentiable)
         self.init_weights()
 
     def init_weights(self, init_w=10e-3):
@@ -167,6 +235,9 @@ class actor(_FlatNet):
 
     def forward(self, state):
         _lib.require_cuda()
+        if self._use_autograd((state,)):
+            x = self._as_grad_input(state, self.input_size)
+            return _ActorFn.apply(self, int(self.precision), x, *self._grad_params())
         x = self._as_input(state, self.input_size)
         B = x.shape[0]
         out = torch.empty(B, self.output_size, dtype=torch.float32, device=x.device)
@@ -179,7 +250,7 @@ class actor(_FlatNet):
 class critic(_FlatNet):
     """models.py:51-88.  fc1 -> ReLU -> cat(., action) -> fc2 -> ReLU -> fc2_2 -> ReLU -> fc3 -> softmax."""
 
-    def __init__(self, state_size, action_size, dist_info, device=None):
+    def __init__(self, state_size, action_size, dist_info, device=None, differentiable=False):
         self.dist_info = dist_info
         if dist_info["type"] != "categorical":
             raise NotImplementedError("only the categorical head exists (mixture_of_gaussian is a TODO stub "
@@ -187,6 +258,7 @@ class critic(_FlatNet):
         self.state_size, self.action_size, self.n_atoms = state_size, action_size, int(dist_info["n_atoms"])
         super().__init__([(state_size, HIDDEN), (HIDDEN + action_size, HIDDEN), (HIDDEN, HIDDEN),
                           (HIDDEN, self.n_atoms)], device)
+        self.differentiable = bool(differentiable)
         self.init_weights()
 
     def init_weights(self, init_w=10e-3):
@@ -195,6 +267,11 @@ class critic(_FlatNet):
 
     def forward(self, state, action, return_logits=False):
         _lib.require_cuda()
+        if self._use_autograd((state, action)):
+            x = self._as_grad_input(state, self.state_size)
+            a = self._as_grad_input(action, self.action_size)
+            probs, logits = _CriticFn.apply(self, int(self.precision), x, a, *self._grad_params())
+            return (probs, logits) if return_logits else probs
         x = self._as_input(state, self.state_size)
         a = self._as_input(action, self.action_size)
         B = x.shape[0]
@@ -205,6 +282,102 @@ class critic(_FlatNet):
                                                   _lib.ptr(self._workspace(B)), int(self.precision), _lib.stream_ptr()),
                    "d4pg_critic_forward")
         return (probs, logits) if return_logits else probs
+
+
+def _backward_scratch(B, out_dim, device):
+    """d4pg_*_backward scratch: two [B,256] delta planes and one output-head plane of row pitch pitch4(out_dim), at
+    least [B,256] (include/d4pg_b200.h)."""
+    head = max(HIDDEN, (out_dim + 3) & ~3)
+    return torch.empty(B * (2 * HIDDEN + head), dtype=torch.float32, device=device)
+
+
+def _param_grads(ctx, net, grad_flat, first):
+    """Per-parameter gradients as views of `grad_flat` (None where autograd did not ask), in _param_list order."""
+    out = []
+    for i, (w, b) in enumerate(net._views(grad_flat) if grad_flat is not None else [(None, None)] * 4):
+        out += [w if ctx.needs_input_grad[first + 2 * i] else None,
+                b if ctx.needs_input_grad[first + 2 * i + 1] else None]
+    return out
+
+
+class _ActorFn(torch.autograd.Function):
+    """action = actor(state) through d4pg_actor_forward; backward = d4pg_actor_backward.  Inputs: the module,
+    the precision, the state and the 8 parameter views (so autograd routes their gradients and their version
+    counters catch an in-place weight write between forward and backward)."""
+
+    @staticmethod
+    def forward(ctx, net, precision, x, *params):
+        B = x.shape[0]
+        out = torch.empty(B, net.output_size, dtype=torch.float32, device=x.device)
+        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)      # h1..h3, kept for backward
+        flat = net._flat
+        _lib.check(_lib.lib().d4pg_actor_forward(_lib.ptr(flat), net.input_size, net.output_size, _lib.ptr(x), B,
+                                                 _lib.ptr(out), _lib.ptr(ws), precision, _lib.stream_ptr()),
+                   "d4pg_actor_forward")
+        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, out, *params)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, out = ctx.saved_tensors[:2]          # unpacking checks the version counters (parameters included)
+        net = ctx.net
+        if g is None:
+            return (None,) * (3 + 8)
+        B = x.shape[0]
+        g = g.to(dtype=torch.float32).contiguous()
+        want_p = any(ctx.needs_input_grad[3:])
+        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
+        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
+        scratch = _backward_scratch(B, net.output_size, x.device)
+        _lib.check(_lib.lib().d4pg_actor_backward(_lib.ptr(ctx.flat), net.input_size, net.output_size, _lib.ptr(x), B,
+                                                  _lib.ptr(out), _lib.ptr(ctx.ws), _lib.ptr(g), _lib.ptr(grad_flat),
+                                                  _lib.ptr(grad_x), _lib.ptr(scratch), ctx.precision,
+                                                  _lib.stream_ptr()), "d4pg_actor_backward")
+        return (None, None, grad_x, *_param_grads(ctx, net, grad_flat, 3))
+
+
+class _CriticFn(torch.autograd.Function):
+    """(probs, logits) = critic(state, action) through d4pg_critic_forward; backward = d4pg_critic_backward."""
+
+    @staticmethod
+    def forward(ctx, net, precision, x, a, *params):
+        B = x.shape[0]
+        probs = torch.empty(B, net.n_atoms, dtype=torch.float32, device=x.device)
+        logits = torch.empty_like(probs)        # always given: without it the forward reuses h1 as logits scratch
+        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)
+        flat = net._flat
+        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(flat), net.state_size, net.action_size, net.n_atoms,
+                                                  _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(probs), _lib.ptr(logits),
+                                                  _lib.ptr(ws), precision, _lib.stream_ptr()), "d4pg_critic_forward")
+        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, a, probs, *params)
+        return probs, logits
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_probs, g_logits):
+        x, a, probs = ctx.saved_tensors[:3]
+        net = ctx.net
+        if g_probs is None and g_logits is None:
+            return (None,) * (4 + 8)
+        B = x.shape[0]
+        g_probs = g_probs.to(dtype=torch.float32).contiguous() if g_probs is not None else None
+        g_logits = g_logits.to(dtype=torch.float32).contiguous() if g_logits is not None else None
+        want_p = any(ctx.needs_input_grad[4:])
+        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
+        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
+        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
+        scratch = _backward_scratch(B, net.n_atoms, x.device)
+        _lib.check(_lib.lib().d4pg_critic_backward(_lib.ptr(ctx.flat), net.state_size, net.action_size, net.n_atoms,
+                                                   _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(probs), _lib.ptr(ctx.ws),
+                                                   _lib.ptr(g_probs), _lib.ptr(g_logits), _lib.ptr(grad_flat),
+                                                   _lib.ptr(grad_x), _lib.ptr(grad_a), _lib.ptr(scratch), ctx.precision,
+                                                   _lib.stream_ptr()), "d4pg_critic_backward")
+        return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
 
 
 def _write_init(net, cpu_linears, fc3_std):

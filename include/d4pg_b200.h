@@ -215,6 +215,37 @@ int32_t d4pg_critic_forward(const float* params, int32_t obs_dim, int32_t act_di
                             float* workspace, int32_t precision, d4pg_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Actor / critic backward: the autograd backward of the two forward calls above, for callers that own
+ * the loss (ddpg.py:229-244 written against the modules, other losses, gradient checks).  Runs the same
+ * per-layer GEMM kernels as the learner's one-launch-per-level plan at the same `precision` (3 rounds dZ and W
+ * for dX, dZ and X for dW to bf16), one launch per layer after a small kernel for the output head.
+ *   params, s (, a), B, precision  exactly as given to the forward call;
+ *   action / probs      the forward's output (tanh output [B,act_dim]; softmax probabilities [B,n_atoms]);
+ *   workspace           h1..h3 exactly as the matching forward call left them.  d4pg_critic_forward reuses h1
+ *                       as logits scratch when `logits` is NULL: a critic forward meant for this backward must
+ *                       be given a logits buffer;
+ *   grad_action         d loss / d action [B,act_dim];
+ *   grad_probs, grad_logits  d loss / d probs and d loss / d logits [B,n_atoms]; either may be NULL (counts as
+ *                       zero), not both; grad_probs needs probs;
+ * outputs (each may be NULL, which skips its launches):
+ *   grad_params         flat buffer in d4pg_*_layout order, overwritten (the call clears it first: the dW of a
+ *                       batch of 1024 rows or more runs split-K with fp32 atomics); pad columns stay zero;
+ *   grad_s [B,obs_dim], grad_a [B,act_dim]  d loss / d input, overwritten;
+ *   scratch             f32 [B*(512 + max(256, pitch4(out)))], out = act_dim (actor) or n_atoms (critic), pitch4(x) =
+ *                       x rounded up to a multiple of 4: two [B,256] delta planes, then the output head's dZ plane
+ *                       [B, pitch4(out)].  For n_atoms <= 128 and act_dim <= 256 that is f32 [3*B*256].
+ * Bad arguments fail with D4PG_EINVAL, an unknown precision with D4PG_ENOTSUP.
+ * ------------------------------------------------------------------------------------- */
+int32_t d4pg_actor_backward(const float* params, int32_t obs_dim, int32_t act_dim, const float* s, int32_t B,
+                            const float* action, const float* workspace, const float* grad_action,
+                            float* grad_params, float* grad_s, float* scratch, int32_t precision, d4pg_stream_t stream);
+int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, int32_t act_dim, int32_t n_atoms,
+                             const float* s, const float* a, int32_t B, const float* probs, const float* workspace,
+                             const float* grad_probs, const float* grad_logits,
+                             float* grad_params, float* grad_s, float* grad_a, float* scratch,
+                             int32_t precision, d4pg_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Fused Adam + Polyak.  Replaces SharedAdam / torch.optim.Adam.step (shared_adam.py:3-17,
  * called at ddpg.py:232,244; torch-2.11 single-tensor formula), sync_local_global
  * (ddpg.py:118-120, identity on shared storage) and update_target_parameters (ddpg.py:110-116).
