@@ -9,7 +9,8 @@
 // layer-to-layer dependency is an all-gather of the 64x256 activation plane inside the cluster.
 //
 // Precision.  3xTF32: x = hi + lo, hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi);
-// D += Al*Bh + Ah*Bl + Ah*Bh with fp32 accumulation (~2^-21 relative, meets the 1e-5 parity bar).
+// D += Al*Bh + Ah*Bl + Ah*Bh with fp32 accumulation (~2^-21 relative, meets the 1e-5 parity bar).  One TF32 pass
+// (TccArgs::passes = 1, precision 2) is D += Ah*Bh alone: both operands truncated to TF32 (round toward zero).
 // Nothing is split on the critical path:
 //   * weights: hi/lo parts are PRE-PACKED once per step (tcc_pack_kernel, right after Adam changed them) into the
 //     exact shared-memory image the MMA reads (K-major SWIZZLE_128B, 32x32 blocks) -- for the backward pass the
@@ -129,8 +130,12 @@ __device__ __forceinline__ void tcc_issue_weights(const TccSlot& S, int rank, in
     if (tcc_group_active(S, g, n0)) tcc_bulk_load(Wb + g * gbytes, S.g[g].wimg + size_t(rank) * gbytes, gbytes, wfull);
 }
 
+// PASSES = 3: 3xTF32 (Ah.Bh + Ah.Bl + Al.Bh); PASSES = 1: one TF32 pass Ah.Bh on the hi images alone (the lo images are
+// still written and copied, but never read).  The hi images truncate (tf32_hi), so one pass is round-toward-zero TF32.
+template <int PASSES>
 __global__ void __cluster_dims__(TCC_CLUSTER, 1, 1) __launch_bounds__(TCC_THREADS, 1)
 mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
+  static_assert(PASSES == 1 || PASSES == 3, "the chain kernel runs one TF32 pass or 3xTF32");
   extern __shared__ uint8_t tcc_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tcc_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* Ab = smem + TCC_OFF_A;        // [TCC_ABUFS] A-chunk buffers; buffer 8 doubles as the resident X chunk
@@ -221,12 +226,16 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
         const TccGroup& G = S.g[g];
         // 3xTF32 in two wgmmas per 8-deep k-step: the weight chunk holds the hi image (32 rows) directly followed by
         // the lo image (32 rows) = a 64-row B operand, so d1[64 x 64] = Ah . [Bh; Bl]^T (columns 0-31 Ah.Bh, 32-63
-        // Ah.Bl) and d2[64 x 32] = Al . Bh^T (Al.Bl, ~2^-22 relative, is not formed).
-        float d1[32], d2[16];
+        // Ah.Bl) and d2[64 x 32] = Al . Bh^T (Al.Bl, ~2^-22 relative, is not formed).  One pass: d1[64 x 32] = Ah . Bh^T
+        // from the first 32 rows of the chunk, and no d2.
+        constexpr int N1 = PASSES == 3 ? 32 : 16;
+        float d1[N1], d2[PASSES == 3 ? 16 : 1];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) d1[i] = 0.f;
+        for (int i = 0; i < N1; ++i) d1[i] = 0.f;
+        if constexpr (PASSES == 3) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) d2[i] = 0.f;
+          for (int i = 0; i < 16; ++i) d2[i] = 0.f;
+        }
         // this thread's epilogue operands do not depend on the chain: fetch them before the accumulator is ready
         float eop[2][8];
         const int npad = mine ? (G.N + 3) & ~3 : 0;
@@ -253,7 +262,8 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
           if (tr && tid == 0) tr[2] = tcc_gtime();
           const uint32_t w_base = smem_u32(Wb) + uint32_t(g * nch) * TCC_W_CHUNK;
           const uint32_t a_base = smem_u32(Ab) + uint32_t(boff) * TCC_A_CHUNK;
-          wg_fence_regs(d1); wg_fence_regs(d2);
+          wg_fence_regs(d1);
+          if constexpr (PASSES == 3) wg_fence_regs(d2);
           // Chunk c of the slot's K lives in A buffer c + boff (checked at launch)
           for (int c = 0; c < nch; ++c) {
             if ((wait_mask >> c) & 1u) {                  // first chunk of a bulk copy / a pre-converted chunk
@@ -267,13 +277,18 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
               const uint64_t bd = wg_desc(w + 32 * ks);
-              wg_mma_n64(d1, wg_desc(a_hi + 32 * ks), bd);
-              wg_mma_n32(d2, wg_desc(a_lo + 32 * ks), bd);
+              if constexpr (PASSES == 3) {
+                wg_mma_n64(d1, wg_desc(a_hi + 32 * ks), bd);
+                wg_mma_n32(d2, wg_desc(a_lo + 32 * ks), bd);
+              } else {
+                wg_mma_n32(d1, wg_desc(a_hi + 32 * ks), bd);
+              }
             }
             wg_commit();
           }
           wg_wait<0>();
-          wg_fence_regs(d1); wg_fence_regs(d2);
+          wg_fence_regs(d1);
+          if constexpr (PASSES == 3) wg_fence_regs(d2);
           if (tr && tid == 0) tr[4] = tcc_gtime();
         }
         // both warpgroups' MMAs are done: the A buffers may be overwritten and the weight buffer refilled
@@ -289,11 +304,16 @@ mlp_tc_chain_kernel(const __grid_constant__ TccArgs args) {
           fence_proxy_async();                             // shared-memory writes -> the tensor core's async-proxy reads
         }
         if (mine) {
-          // ---- Ah.Bh + Ah.Bl + Al.Bh, epilogue ---------------------------------------------------------------
+          // ---- Ah.Bh + Ah.Bl + Al.Bh (one pass: Ah.Bh), epilogue ------------------------------------------------
           const int epi = G.epi;
           float x[16];                                     // x[4 j + 2 rr + e] = (row rl + 8 rr, column cl + 8 j + e)
+          if constexpr (PASSES == 3) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) x[i] = (d1[i + 16] + d2[i]) + d1[i];   // the two small cross terms first
+            for (int i = 0; i < 16; ++i) x[i] = (d1[i + 16] + d2[i]) + d1[i];   // the two small cross terms first
+          } else {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) x[i] = d1[i];
+          }
           // the epilogue kind is decided ONCE per group, around whole loops (a per-element switch compiles to an
           // indirect branch per element)
 #pragma unroll
@@ -576,11 +596,13 @@ int launch_mlp_tc_chain(TccArgs& a, cudaStream_t st) {
       if (l == 0 && ch.pre) D4PG_REQUIRE(s.g[0].N > (TCC_CLUSTER - 1) * TCC_BN, D4PG_ENOTSUP, "launch_mlp_tc_chain: the first slot must span the cluster");
     }
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    D4PG_CUDA_OK(cudaFuncSetAttribute(mlp_tc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(TCC_SMEM)));
-    D4PG_CUDA_OK(cudaFuncSetAttribute(mlp_tc_chain_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared)));
-    attr_set = true;
+  void (*kern)(TccArgs) = a.passes == 3 ? mlp_tc_chain_kernel<3> : mlp_tc_chain_kernel<1>;
+  static bool attr_set[2] = {false, false};          // per instantiation
+  const int ai = a.passes == 3 ? 1 : 0;
+  if (!attr_set[ai]) {
+    D4PG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(TCC_SMEM)));
+    D4PG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared)));
+    attr_set[ai] = true;
   }
   a.watchdog = tcc_watchdog_device();
   unsigned long long* dbg = debug_trace_buffer();
@@ -591,7 +613,7 @@ int launch_mlp_tc_chain(TccArgs& a, cudaStream_t st) {
   cfg.gridDim = dim3(a.nchains * a.row_blocks * TCC_CLUSTER); cfg.blockDim = dim3(TCC_THREADS);
   cfg.dynamicSmemBytes = TCC_SMEM; cfg.stream = st;
   cfg.attrs = nullptr; cfg.numAttrs = 0;              // cluster shape is compiled in (__cluster_dims__)
-  D4PG_CUDA_OK(cudaLaunchKernelEx(&cfg, mlp_tc_chain_kernel, a));
+  D4PG_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, a));
   return D4PG_OK;
 }
 

@@ -48,7 +48,7 @@ struct TccChain {
 struct TccArgs {
   TccChain chain[TCC_MAX_CHAINS];
   int nchains, B, row_blocks;
-  int passes;                     // 3 = 3xTF32 (fp32-accurate), 1 = one TF32 pass
+  int passes;                     // 3 = 3xTF32 (fp32-accurate), 1 = one TF32 pass on the hi images (truncated operands)
   // host pipeline: the batch is sampled on another stream; every CTA first waits until wait_epoch[0..wait_n) >= *wait_clock + 1
   const unsigned long long* wait_epoch; const long long* wait_clock; int wait_n;
   uint8_t* xchg;                  // [nchains][row_blocks][TCC_PLANES][TCC_PLANE_BYTES]

@@ -203,8 +203,8 @@ int32_t d4pg_replay_set_len(d4pg_replay_t* h, int64_t len, int64_t next_idx, int
 /* ---------------------------------------------------------------------------------------
  * Actor / critic forward (inference entry points).  Replace actor.forward (models.py:32-41)
  * and critic.forward (models.py:76-88).  `params` = flat buffer in d4pg_*_layout order.
- * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 wgmma (fp32-accurate), 2 one TF32 wgmma pass,
- * 3 one bf16 wgmma pass (each GEMM operand rounded to bf16, round to nearest even; fp32 accumulate, fp32 bias and
+ * `workspace` f32 [3*B*256] scratch.  precision: 0 fp32 (FFMA), 1 3xTF32 wgmma (fp32-accurate), 2 one TF32 wgmma pass
+ * (operands truncated to TF32, round toward zero), 3 one bf16 wgmma pass (each GEMM operand rounded to bf16, round to nearest even; fp32 accumulate, fp32 bias and
  * activation; inputs, weights and outputs stay fp32).  Any other value fails with D4PG_ENOTSUP.
  * ------------------------------------------------------------------------------------- */
 int32_t d4pg_actor_forward(const float* params, int32_t obs_dim, int32_t act_dim,
@@ -275,7 +275,11 @@ typedef struct {
   double  per_beta0, per_beta_final; int64_t per_beta_iters;   /* LinearSchedule, ddpg.py:81-86 */
   double  prio_eps;           /* ddpg.py:87 */
   int32_t precision;          /* 0 exact fp32 FFMA, 1 3xTF32 wgmma (hi/lo split, fp32-accurate: meets the 1e-5 parity bar),
-                                 2 one TF32 wgmma pass (not parity-grade), 3 one bf16 wgmma pass: the operands of every
+                                 2 one TF32 pass (not parity-grade) whose rounding follows the step plan: the wgmma
+                                 chains and plan 0 truncate each operand to TF32 (round toward zero), the mma.sync
+                                 chain tiles (|s| or |a| > 32, or > 256 atoms) round to nearest, ties away from zero;
+                                 dW is exact fp32 FFMA on both chain plans and TF32 (truncated) on plan 0,
+                                 3 one bf16 wgmma pass: the operands of every
                                  MLP GEMM (X and W forward, dZ and W for dX, dZ and X for dW) are rounded to bf16 (nearest
                                  even) as they are staged, products accumulate in fp32; activations, deltas, bias terms,
                                  bias gradients, the loss heads, Adam and the weights stay fp32 (not parity-grade) */

@@ -1,7 +1,8 @@
 """`actor(..., differentiable=True)` / `critic(..., differentiable=True)`: an opt-in autograd path whose backward runs
 d4pg_actor_backward / d4pg_critic_backward (csrc/mlp_backward.cu: an output-head kernel, then the level GEMMs).
 
-Yardsticks: a float64 torch autograd restatement of models.py:32-41,76-88 (precisions 0-2), the bf16 linear of
+Yardsticks: a float64 torch autograd restatement of models.py:32-41,76-88 (precisions 0-1), the TF32 linear of
+tests/tf32_oracle.py with truncated operands (precision 2: the level GEMMs' rounding), the bf16 linear of
 tests/bf16_oracle.py (precision 3: that oracle already defines the bf16 backward), and the learner's own gradient
 buffer after one DDPG.train() step, recomputed here through the reference's learner body (ddpg.py:229-244)."""
 import ctypes as C
@@ -14,11 +15,16 @@ import torch.nn.functional as F
 
 from oracle import d4pg_oracle as O
 from tests import bf16_oracle as BO
+from tests import tf32_oracle as TO
 
 NAMES = ("fc1.weight", "fc1.bias", "fc2.weight", "fc2.bias", "fc2_2.weight", "fc2_2.bias", "fc3.weight", "fc3.bias")
 # (S, A, N, B); A = 300 makes the actor's head plane wider than the 256-wide delta planes
 SHAPES = [(17, 6, 51, 256), (3, 1, 51, 64), (5, 2, 7, 37), (17, 6, 51, 1), (376, 17, 51, 1024), (17, 6, 101, 4096),
           (5, 300, 7, 33)]
+# precision 2 against the rz linear of tests/tf32_oracle.py: the reference chain computes its own forward, and an
+# activation whose fp32 value differs in the last bit from the device's may truncate to the neighbouring TF32 value.
+# Worst measured on one H100: 1.3e-4 (actor fc3.weight); against the unrounded float64 chain this bound was 5e-3.
+TF32_REL_L2 = 3e-4
 
 
 def _info(N):
@@ -178,7 +184,7 @@ def _check(name, mine, ref, precision):
     if precision in (0, 1):
         _close(name, mine, ref, 1e-5)
     elif precision == 2:
-        _rel_l2(name, mine, ref, 5e-3)
+        _rel_l2(name, mine, ref, TF32_REL_L2)
     else:
         _rel_l2(name, mine, ref, 1e-3)
 
@@ -188,15 +194,16 @@ def _check(name, mine, ref, precision):
 @pytest.mark.parametrize("precision", [0, 1, 2, 3])
 def test_gradients_vs_float64_autograd(precision, S, A, N, B):
     """Random upstream gradients on the output; every parameter gradient, d state and d action against torch autograd on
-    the float64 restatement (precision 3: the bf16 linear of tests/bf16_oracle.py).  B >= 1024 runs split-K dW.  The
+    the float64 restatement (precision 2: the rz TF32 linear of tests/tf32_oracle.py; precision 3: the bf16 linear of
+    tests/bf16_oracle.py).  B >= 1024 runs split-K dW.  The
     upstream gradients are N(0, 1) / B, what a batch-mean loss (ddpg.py:217,238) hands the output layer."""
     import d4pg_b200 as d4pg
     a, c = _nets(d4pg, S, A, N, precision)
     g = torch.Generator().manual_seed(7)
     s0 = torch.randn(B, S, generator=g); act0 = torch.rand(B, A, generator=g) * 2 - 1
     ga, gp, gz = (torch.randn(B, n, generator=g) / B for n in (A, N, N))
-    dt = torch.float32 if precision == 3 else torch.float64
-    lin = BO.linear("bf16") if precision == 3 else F.linear
+    dt = torch.float32 if precision in (2, 3) else torch.float64
+    lin = {2: TO.linear("rz"), 3: BO.linear("bf16")}.get(precision, F.linear)
 
     # actor
     s = s0.cuda().requires_grad_(True)
