@@ -14,6 +14,7 @@ OK, EINVAL, ECUDA, ENOTSUP, ENCCL, ESTATE = 0, -1, -2, -3, -4, -5
 PROJ_TARGET_IS_PROBS, PROJ_Q_IS_PROBS = 1, 2
 HIDDEN = 256
 MAX_ATOMS = 128
+MAX_COMPONENTS = 32
 
 c_float_p = C.POINTER(C.c_float)
 c_double_p = C.POINTER(C.c_double)
@@ -44,6 +45,7 @@ class LearnerConfig(C.Structure):
         ("philox_seed", C.c_uint64),
         ("world_size", C.c_int32), ("use_graph", C.c_int32),
         ("loss_flags", C.c_int32), ("chain", C.c_int32), ("prefetch", C.c_int32),
+        ("dist_type", C.c_int32), ("n_components", C.c_int32),
     ]
 
 
@@ -69,6 +71,9 @@ _PROTOS = {
     "d4pg_proj_loss": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double,
                                    C.c_int32, C.c_int32, C.c_double, C.c_float,
                                    _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "d4pg_mog_loss": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_float,
+                                  _P, _P, _P, _P, _P, _P, _P]),
+    "d4pg_mog_quadrature": (C.c_int32, [_P, _P]),
     "d4pg_replay_capacity": (C.c_int32, [C.c_int64, C.POINTER(C.c_int64)]),
     "d4pg_replay_create": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32, C.c_double, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                        _P, C.POINTER(_P)]),
@@ -95,6 +100,10 @@ _PROTOS = {
     "d4pg_actor_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_critic_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P,
                                          _P, _P, _P, _P, C.c_int32, _P]),
+    "d4pg_critic_forward_mog": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P, _P,
+                                            C.c_int32, _P]),
+    "d4pg_critic_backward_mog": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P, _P,
+                                             _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_adam_polyak": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
                                      C.c_int64, C.c_double, C.c_float, _P]),
     "d4pg_polyak": (C.c_int32, [_P, _P, C.c_int64, C.c_double, _P]),
@@ -200,6 +209,13 @@ def actor_layout(obs_dim, act_dim):
     out = NetLayout()
     check(lib().d4pg_actor_layout(obs_dim, act_dim, C.byref(out)), "d4pg_actor_layout")
     return list(out.offsets), list(out.sizes), int(out.total), list(out.pitch)
+
+
+def mog_quadrature():
+    """The library's 8-node Gauss-Hermite table (x, h) of the mixture critic's loss (host only, no GPU needed)."""
+    x, h = (C.c_double * 8)(), (C.c_double * 8)()
+    check(lib().d4pg_mog_quadrature(x, h), "d4pg_mog_quadrature")
+    return list(x), list(h)
 
 
 def critic_layout(obs_dim, act_dim, n_atoms):

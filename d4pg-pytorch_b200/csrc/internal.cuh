@@ -27,6 +27,25 @@ struct HeadsArgs {
 };
 int launch_heads(const HeadsArgs& a, int mode, cudaStream_t st);
 
+// mixture-of-Gaussians head (mog_heads.cu): every [B, 3K] raw plane has row pitch `ld`
+struct MogArgs {
+  const float* target_raw; const float* q_raw; const float* pi_raw;
+  const double* rewards; const uint8_t* dones;
+  int B, K, ld;
+  double discount, prio_eps;
+  float grad_scale;
+  float* loss_rows; float* td; float* prio; float* dq_raw; float* pi_rows; float* dpi_raw;
+  const float* is_weights;       // non-null: critic loss row i is scaled by the PER importance weight w_i
+  int pdl;
+  unsigned long long* trace;
+  int only_policy;               // as HeadsArgs::only_policy
+  LearnerClock* sampler_clock;   // as HeadsArgs::sampler_clock
+};
+int launch_mog_heads(const MogArgs& a, cudaStream_t st);
+int launch_mog_transform(const float* raw, int ldr, int B, int K, float* w, float* mu, float* sigma, cudaStream_t st);
+int launch_mog_head_backward(const float* raw, int ldr, const float* gw, const float* gmu, const float* gsig, int B, int K,
+                             float* dz, int ldz, cudaStream_t st);
+
 constexpr int SAMPLE_ROWS = 32;      // batch rows per CTA of the sample + gather kernel (replay_dev.cuh)
 
 // sample for the learner: per-step scalars come from device memory (graph replay safe)

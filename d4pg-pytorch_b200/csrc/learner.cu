@@ -61,6 +61,13 @@ static StepPlan step_plan(const d4pg_learner_config_t& c) {
   if (c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256) return PLAN_TC_CHAIN;
   return PLAN_CHAIN;
 }
+// The mixture-of-Gaussians critic (dist_type 1) has a raw head of 3K columns: it takes the place of n_atoms wherever a
+// plane or a layer is sized (carve, critic_dims, step_plan, tcc_setup), so the learner keeps the config with n_atoms = 3K
+static d4pg_learner_config_t with_head_width(const d4pg_learner_config_t& c) {
+  d4pg_learner_config_t e = c;
+  if (c.dist_type == 1) e.n_atoms = 3 * c.n_components;
+  return e;
+}
 // The warm host-pipeline graph of the wgmma plan waits for the sampler by polling its per-CTA epochs from the forward
 // chains' threads (one epoch per thread)
 static_assert((CHAIN_MAX_BATCH + SAMPLE_ROWS - 1) / SAMPLE_ROWS <= TCC_THREADS, "sampler epochs exceed the chain CTA's threads");
@@ -343,7 +350,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     if (L->profiling) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);    \
       std::string nm0(#expr);                                                              \
       /* the loss kernel also advances the sampler clock under the prefetch pipeline: not idempotent there */ \
-      const bool rep = nm0.rfind("gemm_launch", 0) == 0 || (nm0.rfind("launch_heads", 0) == 0 && !pf) || \
+      const bool rep = nm0.rfind("gemm_launch", 0) == 0 || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0) && !pf) || \
                        nm0.rfind("launch_mlp_chain", 0) == 0 || nm0.rfind("launch_mlp_tc_chain", 0) == 0; \
       cudaEventRecord(e0, st); rc = (expr);                                                \
       for (int _r = 1; rep && _r < PROFILE_REPS && rc == 0; ++_r) rc = (expr);             \
@@ -491,6 +498,17 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   }
 
   // 3. heads: softmaxes, projection, CE loss, td, priorities, logit gradients (ddpg.py:214-222,236-238)
+  //    (mixture critic: the quadrature cross-entropy, td, priorities and raw-head gradients of mog_heads.cu)
+  const bool mog = c.dist_type == 1;
+  MogArgs ma{};
+  ma.target_raw = w.out[1]; ma.q_raw = w.out[2]; ma.pi_raw = h7 ? nullptr : w.out[4];
+  ma.rewards = w.r; ma.dones = w.done; ma.B = B; ma.K = c.n_components; ma.ld = Np;
+  ma.discount = (c.proj_mode == 1) ? pow(c.gamma, double(c.n_steps)) : c.gamma; ma.prio_eps = c.prio_eps;
+  ma.grad_scale = 1.0f / (float(B) * float(c.world_size > 1 ? c.world_size : 1));
+  ma.loss_rows = w.loss_rows; ma.td = b.td; ma.prio = b.prio; ma.dq_raw = w.dlogits_q;
+  ma.pi_rows = w.pi_rows; ma.dpi_raw = w.dlogits_pi;
+  ma.is_weights = ((c.loss_flags & 1) && c.prioritized) ? bwts : nullptr;
+  ma.sampler_clock = pf ? w.clock : nullptr;
   HeadsArgs ha{};
   ha.target_logits = w.out[1]; ha.q_logits = w.out[2]; ha.pi_logits = h7 ? nullptr : w.out[4];
   ha.rewards = w.r; ha.dones = w.done; ha.B = B; ha.N = N; ha.flags = 0; ha.ld = Np;
@@ -504,7 +522,8 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   ha.is_weights = ((c.loss_flags & 1) && c.prioritized) ? bwts : nullptr;
   ha.sampler_clock = pf ? w.clock : nullptr;          // sample(t) is done, sample(t+1) not yet launched
   ha.ce_priority = (c.loss_flags & 2) ? 1 : 0;
-  RUN(launch_heads(ha, c.proj_mode, st));
+  if (mog) RUN(launch_mog_heads(ma, st));
+  else RUN(launch_heads(ha, c.proj_mode, st));
 
   // 4. priorities into the trees (ddpg.py:252-255): independent of the backward pass, so it runs
   //    on a forked branch (side stream -> parallel graph branch) and joins before the step ends
@@ -722,7 +741,10 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     RUN(launch_mlp_tc_chain(fb, st));
     HeadsArgs hp = ha;
     hp.pi_logits = w.out[4]; hp.only_policy = 1; hp.sampler_clock = nullptr;
-    RUN(launch_heads(hp, c.proj_mode, st));
+    MogArgs mp = ma;
+    mp.pi_raw = w.out[4]; mp.only_policy = 1; mp.sampler_clock = nullptr;
+    if (mog) RUN(launch_mog_heads(mp, st));
+    else RUN(launch_heads(hp, c.proj_mode, st));
     TccArgs& bb = L->tcc_bwd_args;
     tcc_args_begin(bb, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); bb.step_slot = 5;
     tcc_build_bwd_P(bb, 0, cx);
@@ -747,21 +769,31 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
 
 extern "C" int64_t d4pg_learner_workspace_floats(const d4pg_learner_config_t* cfg) {
   if (!cfg) return -1;
-  return carve(nullptr, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, step_plan(*cfg), piped(*cfg)).total;
+  const d4pg_learner_config_t ec = with_head_width(*cfg);
+  return carve(nullptr, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, step_plan(ec), piped(ec)).total;
 }
 
 extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d4pg_learner_buffers_t* buf,
                                        d4pg_replay_t* replay, d4pg_comm_t* comm, d4pg_learner_t** out) {
   D4PG_REQUIRE(cfg && buf && replay && out, D4PG_EINVAL, "d4pg_learner_create: null argument");
   D4PG_REQUIRE(cfg->batch > 0 && cfg->obs_dim > 0 && cfg->act_dim > 0, D4PG_EINVAL, "d4pg_learner_create: bad dims");
-  D4PG_REQUIRE(cfg->n_atoms >= 2 && cfg->n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_learner_create: n_atoms must be in [2,%d]", D4PG_MAX_ATOMS);
-  D4PG_REQUIRE(cfg->v_max > cfg->v_min, D4PG_EINVAL, "d4pg_learner_create: v_max <= v_min");
+  D4PG_REQUIRE(cfg->dist_type == 0 || cfg->dist_type == 1, D4PG_EINVAL, "d4pg_learner_create: dist_type must be 0 (categorical) or 1 (mixture of Gaussians)");
+  if (cfg->dist_type == 1) {
+    D4PG_REQUIRE(cfg->n_components >= 1 && cfg->n_components <= D4PG_MAX_COMPONENTS, D4PG_EINVAL,
+                 "d4pg_learner_create: n_components must be in [1,%d]", D4PG_MAX_COMPONENTS);
+    D4PG_REQUIRE(!(cfg->loss_flags & 2), D4PG_ENOTSUP,
+                 "d4pg_learner_create: loss_flags & 2 (cross-entropy priority) is not supported by the mixture critic: the cross-entropy of a density can be negative");
+  } else {
+    D4PG_REQUIRE(cfg->n_atoms >= 2 && cfg->n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_learner_create: n_atoms must be in [2,%d]", D4PG_MAX_ATOMS);
+    D4PG_REQUIRE(cfg->v_max > cfg->v_min, D4PG_EINVAL, "d4pg_learner_create: v_max <= v_min");
+  }
+  const d4pg_learner_config_t ec = with_head_width(*cfg);
   D4PG_REQUIRE(cfg->proj_mode == 0 || cfg->proj_mode == 1, D4PG_EINVAL, "d4pg_learner_create: proj_mode must be 0/1");
   D4PG_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, D4PG_ENOTSUP,
                "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma, 3 bf16 wgmma)", cfg->precision);
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
-  D4PG_REQUIRE(!(cfg->loss_flags & 4) || (step_plan(*cfg) == PLAN_TC_CHAIN && cfg->world_size <= 1), D4PG_ENOTSUP,
+  D4PG_REQUIRE(!(cfg->loss_flags & 4) || (step_plan(ec) == PLAN_TC_CHAIN && cfg->world_size <= 1), D4PG_ENOTSUP,
                "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1 or 2 (not 0 or 3), chain 1, "
                "batch <= 512, obs_dim <= 32, act_dim <= 32, on one GPU");
   D4PG_REQUIRE(buf->actor && buf->actor_target && buf->critic && buf->critic_target && buf->grad_actor && buf->grad_critic &&
@@ -770,14 +802,14 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
                "d4pg_learner_create: null device buffer");
   d4pg_learner* L = new (std::nothrow) d4pg_learner();
   D4PG_REQUIRE(L, D4PG_EINVAL, "d4pg_learner_create: out of host memory");
-  L->cfg = *cfg; L->buf = *buf; L->replay = replay; L->comm = comm; L->plan = step_plan(*cfg);
+  L->cfg = ec; L->buf = *buf; L->replay = replay; L->comm = comm; L->plan = step_plan(ec);
   L->da = actor_dims(cfg->obs_dim, cfg->act_dim);
-  L->dc = critic_dims(cfg->obs_dim, cfg->act_dim, cfg->n_atoms);
+  L->dc = critic_dims(ec.obs_dim, ec.act_dim, ec.n_atoms);
   if (buf->grad_critic != buf->grad_actor + L->da.total) {
     set_error("d4pg_learner_create: grad_critic must equal grad_actor + P_a (one flat gradient buffer)");
     delete L; return D4PG_EINVAL;
   }
-  L->ws = carve(buf->workspace, cfg->batch, cfg->obs_dim, cfg->act_dim, cfg->n_atoms, L->plan, piped(*cfg));
+  L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec));
   for (int i = 0; i < 4; ++i) { L->graph_exec[i] = nullptr; L->graph_ready[i] = false; }
   for (int i = 0; i < 2; ++i) { L->multi_exec[i] = nullptr; L->multi_ready[i] = false; }
   L->pipe_par = 0; L->last_par = 0; L->prefetch_valid = false; L->seen_gen = -1;

@@ -46,6 +46,9 @@ __global__ void head_backward_kernel(const float* __restrict__ y, const float* _
   }
 }
 
+int launch_mog_head_backward(const float* raw, int ldr, const float* gw, const float* gmu, const float* gsig, int B, int K,
+                             float* dz, int ldz, cudaStream_t st);      // mog_heads.cu
+
 static int launch_level(GemmBatch& b, int precision, cudaStream_t st) {
   return b.n ? gemm_launch(b, precision, st) : D4PG_OK;
 }
@@ -104,32 +107,20 @@ extern "C" int32_t d4pg_actor_backward(const float* params, int32_t obs_dim, int
   return D4PG_OK;
 }
 
-// critic: fc1 -> relu -> cat(., a) -> fc2 -> relu -> fc2_2 -> relu -> fc3 -> softmax.  Levels fc3 -> fc2_2 -> fc2 -> fc1;
-// fc2 splits into its h1 columns (dX masked by h1 > 0, dW with the bias gradient) and its action columns W2[:, H:]
-// (dX = d action, dW without bias).
-extern "C" int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, int32_t act_dim, int32_t n_atoms,
-                                        const float* s, const float* a, int32_t B, const float* probs,
-                                        const float* workspace, const float* grad_probs, const float* grad_logits,
-                                        float* grad_params, float* grad_s, float* grad_a, float* scratch,
-                                        int32_t precision, d4pg_stream_t stream) {
-  D4PG_REQUIRE(params && s && a && workspace && scratch && B > 0 && obs_dim > 0 && act_dim > 0, D4PG_EINVAL,
-               "d4pg_critic_backward: null/empty argument");
-  D4PG_REQUIRE(grad_probs || grad_logits, D4PG_EINVAL, "d4pg_critic_backward: grad_probs and grad_logits are both NULL");
-  D4PG_REQUIRE(probs || !grad_probs, D4PG_EINVAL, "d4pg_critic_backward: grad_probs needs probs");
-  D4PG_REQUIRE(n_atoms >= 2 && n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_critic_backward: n_atoms out of range");
-  D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_critic_backward: unknown precision %d", precision);
+// the critic's levels fc3 -> fc2_2 -> fc2 -> fc1 from the output layer's dZ plane `dz` [B, pitch4(N)] (held in scratch
+// behind the two delta planes); the caller checked the arguments
+static int critic_levels(const float* params, int obs_dim, int act_dim, int n_atoms, const float* s, const float* a, int B,
+                         const float* workspace, const float* dz, float* grad_params, float* grad_s, float* grad_a,
+                         float* scratch, int precision, cudaStream_t st) {
   const NetDims d = critic_dims(obs_dim, act_dim, n_atoms);
   const int H = D4PG_HIDDEN, S = obs_dim, A = act_dim, N = n_atoms, Np = pitch4(n_atoms);
   const float* h1 = workspace; const float* h2 = h1 + size_t(B) * H; const float* h3 = h2 + size_t(B) * H;
-  float* p0 = scratch; float* p1 = p0 + size_t(B) * H; float* dz = p1 + size_t(B) * H;
+  float* p0 = scratch; float* p1 = p0 + size_t(B) * H;
   const float* W = params; float* G = grad_params;
-  cudaStream_t st = as_stream(stream);
   if (!G && !grad_s && !grad_a) return D4PG_OK;
   if (G) D4PG_CUDA_OK(cudaMemsetAsync(G, 0, size_t(d.total) * sizeof(float), st));
   const bool need_dz1 = G || grad_s;
 
-  head_backward_kernel<<<cdiv(B * 32, 256), 256, 0, st>>>(probs, grad_probs, grad_logits, dz, B, N, Np, 1);
-  D4PG_LAUNCH_OK();
   GemmBatch g;
   // fc3
   gemm_batch_begin(g);
@@ -156,4 +147,47 @@ extern "C" int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, in
     RUN_LEVEL(g);
   }
   return D4PG_OK;
+}
+
+// critic: fc1 -> relu -> cat(., a) -> fc2 -> relu -> fc2_2 -> relu -> fc3 -> softmax.  Levels fc3 -> fc2_2 -> fc2 -> fc1;
+// fc2 splits into its h1 columns (dX masked by h1 > 0, dW with the bias gradient) and its action columns W2[:, H:]
+// (dX = d action, dW without bias).
+extern "C" int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, int32_t act_dim, int32_t n_atoms,
+                                        const float* s, const float* a, int32_t B, const float* probs,
+                                        const float* workspace, const float* grad_probs, const float* grad_logits,
+                                        float* grad_params, float* grad_s, float* grad_a, float* scratch,
+                                        int32_t precision, d4pg_stream_t stream) {
+  D4PG_REQUIRE(params && s && a && workspace && scratch && B > 0 && obs_dim > 0 && act_dim > 0, D4PG_EINVAL,
+               "d4pg_critic_backward: null/empty argument");
+  D4PG_REQUIRE(grad_probs || grad_logits, D4PG_EINVAL, "d4pg_critic_backward: grad_probs and grad_logits are both NULL");
+  D4PG_REQUIRE(probs || !grad_probs, D4PG_EINVAL, "d4pg_critic_backward: grad_probs needs probs");
+  D4PG_REQUIRE(n_atoms >= 2 && n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_critic_backward: n_atoms out of range");
+  D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_critic_backward: unknown precision %d", precision);
+  const int Np = pitch4(n_atoms);
+  float* dz = scratch + size_t(B) * 2 * D4PG_HIDDEN;
+  if (!grad_params && !grad_s && !grad_a) return D4PG_OK;
+  head_backward_kernel<<<cdiv(B * 32, 256), 256, 0, as_stream(stream)>>>(probs, grad_probs, grad_logits, dz, B, n_atoms, Np, 1);
+  D4PG_LAUNCH_OK();
+  return critic_levels(params, obs_dim, act_dim, n_atoms, s, a, B, workspace, dz, grad_params, grad_s, grad_a, scratch,
+                       precision, as_stream(stream));
+}
+
+// mixture-of-Gaussians critic (mog_heads.cu): the raw head's dZ from (g_w, g_mu, g_sigma), then the same levels
+extern "C" int32_t d4pg_critic_backward_mog(const float* params, int32_t obs_dim, int32_t act_dim, int32_t K,
+                                            const float* s, const float* a, int32_t B, const float* raw,
+                                            const float* workspace, const float* grad_w, const float* grad_mu,
+                                            const float* grad_sigma, float* grad_params, float* grad_s, float* grad_a,
+                                            float* scratch, int32_t precision, d4pg_stream_t stream) {
+  D4PG_REQUIRE(params && s && a && raw && workspace && scratch && B > 0 && obs_dim > 0 && act_dim > 0, D4PG_EINVAL,
+               "d4pg_critic_backward_mog: null/empty argument");
+  D4PG_REQUIRE(grad_w || grad_mu || grad_sigma, D4PG_EINVAL, "d4pg_critic_backward_mog: grad_w, grad_mu and grad_sigma are all NULL");
+  D4PG_REQUIRE(K >= 1 && K <= D4PG_MAX_COMPONENTS, D4PG_EINVAL, "d4pg_critic_backward_mog: K=%d outside [1,%d]", K, D4PG_MAX_COMPONENTS);
+  D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_critic_backward_mog: unknown precision %d", precision);
+  if (!grad_params && !grad_s && !grad_a) return D4PG_OK;
+  const int N = 3 * K;
+  float* dz = scratch + size_t(B) * 2 * D4PG_HIDDEN;
+  const int rc = launch_mog_head_backward(raw, N, grad_w, grad_mu, grad_sigma, B, K, dz, pitch4(N), as_stream(stream));
+  if (rc) return rc;
+  return critic_levels(params, obs_dim, act_dim, N, s, a, B, workspace, dz, grad_params, grad_s, grad_a, scratch,
+                       precision, as_stream(stream));
 }

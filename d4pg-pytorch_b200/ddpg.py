@@ -53,7 +53,11 @@ class _Learner(object):
         B = ddpg.batch_size
         cfg = _lib.LearnerConfig()
         cfg.obs_dim, cfg.act_dim, cfg.n_atoms, cfg.batch = ddpg.obs_dim, ddpg.act_dim, ddpg.n_atoms, B
-        cfg.v_min, cfg.v_max, cfg.gamma = float(ddpg.v_min), float(ddpg.v_max), float(ddpg.gamma)
+        if ddpg.n_components is not None:       # mixture critic: n_atoms / v_min / v_max are ignored by the library
+            cfg.dist_type, cfg.n_components, cfg.v_min, cfg.v_max = 1, ddpg.n_components, 0.0, 0.0
+        else:
+            cfg.v_min, cfg.v_max = float(ddpg.v_min), float(ddpg.v_max)
+        cfg.gamma = float(ddpg.gamma)
         cfg.n_steps = int(ddpg.n_steps)
         cfg.proj_mode = 1 if ddpg.projection == "nstep" else 0
         cfg.tau = float(ddpg.tau)
@@ -202,14 +206,26 @@ class DDPG:
         self.actor_critic = actor_critic
 
         self.dist_type = critic_dist_info["type"]
-        if self.dist_type != "categorical":
-            raise NotImplementedError("only the categorical critic exists (the reference's "
-                                      "mixture_of_gaussian branch is a TODO stub, ddpg.py:48-50)")
-        self.v_min = critic_dist_info["v_min"]
-        self.v_max = critic_dist_info["v_max"]
-        self.n_atoms = critic_dist_info["n_atoms"]
-        self.delta = (self.v_max - self.v_min) / float(self.n_atoms - 1)
-        self.bin_centers = np.array([self.v_min + i * self.delta for i in range(self.n_atoms)]).reshape(-1, 1)
+        if self.dist_type == "mixture_of_gaussian":
+            # {"type": "mixture_of_gaussian", "n_components": K}: the reference stubs this branch (ddpg.py:48-50).  The
+            # critic loss is the cross-entropy of the online mixture under the target mixture, integrated with 8
+            # Gauss-Hermite nodes per target component (csrc/mog_heads.cu); td = E[Q] - (r + c E[Q']).
+            if priority == "ce":
+                raise _lib.D4PGError('priority="ce" is not supported with a mixture_of_gaussian critic: the '
+                                     'cross-entropy of a density can be negative')
+            self.n_components = int(critic_dist_info["n_components"])
+            self.v_min = self.v_max = self.delta = self.bin_centers = None
+            self.n_atoms = 3 * self.n_components        # raw head width of the critic's fc3
+        elif self.dist_type == "categorical":
+            self.n_components = None
+            self.v_min = critic_dist_info["v_min"]
+            self.v_max = critic_dist_info["v_max"]
+            self.n_atoms = critic_dist_info["n_atoms"]
+            self.delta = (self.v_max - self.v_min) / float(self.n_atoms - 1)
+            self.bin_centers = np.array([self.v_min + i * self.delta for i in range(self.n_atoms)]).reshape(-1, 1)
+        else:
+            raise NotImplementedError("critic_dist_info['type'] must be 'categorical' or 'mixture_of_gaussian', got %r"
+                                      % (self.dist_type,))
 
         # networks, built in the reference's order so a seeded RNG yields the same weights (ddpg.py:56-64)
         self.actor = actor(input_size=obs_dim, output_size=act_dim, device=self.device)
@@ -279,6 +295,9 @@ class DDPG:
 
     # ---- projections as standalone methods (numpy in / numpy out, computed on the GPU) --------
     def _project(self, target_z_dist, rewards, terminates, mode):
+        if self.n_components is not None:
+            raise _lib.D4PGError("reproject2 / reproj_categorical_dist project onto the categorical atoms; this DDPG has "
+                                 "a mixture_of_gaussian critic")
         _lib.require_cuda()
         p = torch.as_tensor(np.ascontiguousarray(target_z_dist, dtype=np.float32)).to(self.device)
         B, N = p.shape

@@ -248,14 +248,27 @@ class actor(_FlatNet):
 
 
 class critic(_FlatNet):
-    """models.py:51-88.  fc1 -> ReLU -> cat(., action) -> fc2 -> ReLU -> fc2_2 -> ReLU -> fc3 -> softmax."""
+    """models.py:51-88.  fc1 -> ReLU -> cat(., action) -> fc2 -> ReLU -> fc2_2 -> ReLU -> fc3 -> softmax.
+
+    dist_info {"type": "mixture_of_gaussian", "n_components": K} (1 <= K <= 32; the reference stubs this branch,
+    models.py:63-65): fc3 is Linear(256, 3K) and forward returns (w, mu, sigma), each [B, K]: w = softmax(raw[:, :K]),
+    mu = raw[:, K:2K], sigma = softplus(raw[:, 2K:]) + 1e-3.  `n_atoms` is then the raw head width 3K."""
 
     def __init__(self, state_size, action_size, dist_info, device=None, differentiable=False):
         self.dist_info = dist_info
-        if dist_info["type"] != "categorical":
-            raise NotImplementedError("only the categorical head exists (mixture_of_gaussian is a TODO stub "
-                                      "in the reference too, models.py:63-65)")
-        self.state_size, self.action_size, self.n_atoms = state_size, action_size, int(dist_info["n_atoms"])
+        self.dist_type = dist_info["type"]
+        if self.dist_type == "mixture_of_gaussian":
+            self.n_components = int(dist_info["n_components"])
+            if not 1 <= self.n_components <= _lib.MAX_COMPONENTS:
+                raise _lib.D4PGError("n_components must be in [1, %d], got %d" % (_lib.MAX_COMPONENTS, self.n_components))
+            head = 3 * self.n_components
+        elif self.dist_type == "categorical":
+            self.n_components = None
+            head = int(dist_info["n_atoms"])
+        else:
+            raise NotImplementedError("critic_dist_info['type'] must be 'categorical' or 'mixture_of_gaussian', got %r"
+                                      % (self.dist_type,))
+        self.state_size, self.action_size, self.n_atoms = state_size, action_size, head
         super().__init__([(state_size, HIDDEN), (HIDDEN + action_size, HIDDEN), (HIDDEN, HIDDEN),
                           (HIDDEN, self.n_atoms)], device)
         self.differentiable = bool(differentiable)
@@ -266,7 +279,11 @@ class critic(_FlatNet):
         _write_init(self, ls, 3e-4)
 
     def forward(self, state, action, return_logits=False):
+        """Categorical: probs (and logits with return_logits).  Mixture: (w, mu, sigma) (and the raw fc3 output
+        [B, 3K] as a fourth element with return_logits)."""
         _lib.require_cuda()
+        if self.n_components is not None:
+            return self._forward_mog(state, action, return_logits)
         if self._use_autograd((state, action)):
             x = self._as_grad_input(state, self.state_size)
             a = self._as_grad_input(action, self.action_size)
@@ -282,6 +299,23 @@ class critic(_FlatNet):
                                                   _lib.ptr(self._workspace(B)), int(self.precision), _lib.stream_ptr()),
                    "d4pg_critic_forward")
         return (probs, logits) if return_logits else probs
+
+    def _forward_mog(self, state, action, return_raw):
+        if self._use_autograd((state, action)):
+            x = self._as_grad_input(state, self.state_size)
+            a = self._as_grad_input(action, self.action_size)
+            w, mu, sigma, raw = _CriticMogFn.apply(self, int(self.precision), x, a, *self._grad_params())
+            return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
+        x = self._as_input(state, self.state_size)
+        a = self._as_input(action, self.action_size)
+        B, K = x.shape[0], self.n_components
+        w, mu, sigma = (torch.empty(B, K, dtype=torch.float32, device=x.device) for _ in range(3))
+        raw = torch.empty(B, 3 * K, dtype=torch.float32, device=x.device) if return_raw else None
+        _lib.check(_lib.lib().d4pg_critic_forward_mog(_lib.ptr(self._flat), self.state_size, self.action_size, K,
+                                                      _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(w), _lib.ptr(mu),
+                                                      _lib.ptr(sigma), _lib.ptr(raw), _lib.ptr(self._workspace(B)),
+                                                      int(self.precision), _lib.stream_ptr()), "d4pg_critic_forward_mog")
+        return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
 
 
 def _backward_scratch(B, out_dim, device):
@@ -377,6 +411,50 @@ class _CriticFn(torch.autograd.Function):
                                                    _lib.ptr(g_probs), _lib.ptr(g_logits), _lib.ptr(grad_flat),
                                                    _lib.ptr(grad_x), _lib.ptr(grad_a), _lib.ptr(scratch), ctx.precision,
                                                    _lib.stream_ptr()), "d4pg_critic_backward")
+        return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
+
+
+class _CriticMogFn(torch.autograd.Function):
+    """(w, mu, sigma, raw) = mixture critic(state, action) through d4pg_critic_forward_mog; backward =
+    d4pg_critic_backward_mog.  raw is returned for inspection only: its gradient is not propagated."""
+
+    @staticmethod
+    def forward(ctx, net, precision, x, a, *params):
+        B, K = x.shape[0], net.n_components
+        w, mu, sigma = (torch.empty(B, K, dtype=torch.float32, device=x.device) for _ in range(3))
+        raw = torch.empty(B, 3 * K, dtype=torch.float32, device=x.device)   # kept for backward (softmax / softplus')
+        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)
+        flat = net._flat
+        _lib.check(_lib.lib().d4pg_critic_forward_mog(_lib.ptr(flat), net.state_size, net.action_size, K, _lib.ptr(x),
+                                                      _lib.ptr(a), B, _lib.ptr(w), _lib.ptr(mu), _lib.ptr(sigma),
+                                                      _lib.ptr(raw), _lib.ptr(ws), precision, _lib.stream_ptr()),
+                   "d4pg_critic_forward_mog")
+        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(raw)
+        ctx.save_for_backward(x, a, raw, *params)
+        return w, mu, sigma, raw
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_w, g_mu, g_sigma, g_raw):
+        x, a, raw = ctx.saved_tensors[:3]
+        net = ctx.net
+        if g_w is None and g_mu is None and g_sigma is None:
+            return (None,) * (4 + 8)
+        B = x.shape[0]
+        g_w, g_mu, g_sigma = (g.to(dtype=torch.float32).contiguous() if g is not None else None for g in (g_w, g_mu, g_sigma))
+        want_p = any(ctx.needs_input_grad[4:])
+        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
+        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
+        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
+        scratch = _backward_scratch(B, net.n_atoms, x.device)
+        _lib.check(_lib.lib().d4pg_critic_backward_mog(_lib.ptr(ctx.flat), net.state_size, net.action_size,
+                                                       net.n_components, _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(raw),
+                                                       _lib.ptr(ctx.ws), _lib.ptr(g_w), _lib.ptr(g_mu), _lib.ptr(g_sigma),
+                                                       _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(grad_a),
+                                                       _lib.ptr(scratch), ctx.precision, _lib.stream_ptr()),
+                   "d4pg_critic_backward_mog")
         return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
 
 

@@ -35,6 +35,7 @@ extern "C" {
 
 #define D4PG_HIDDEN      256   /* models.py:18-23,56-62 hard-code 256 hidden units */
 #define D4PG_MAX_ATOMS   128
+#define D4PG_MAX_COMPONENTS 32  /* mixture-of-Gaussians critic: at most 32 components (one warp lane each) */
 
 typedef void* d4pg_stream_t;   /* cudaStream_t */
 
@@ -94,6 +95,29 @@ int32_t d4pg_proj_loss(const float* target_logits, const float* q_logits, const 
                        float* target_probs, float* q_probs,
                        float* loss_rows, float* td, float* prio, float* dlogits_q,
                        float* pi_rows, float* dlogits_pi, d4pg_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Mixture-of-Gaussians critic head (critic_dist_info['type'] == 'mixture_of_gaussian', K = n_components in
+ * [1, D4PG_MAX_COMPONENTS]).  The reference stubs this branch (ddpg.py:48-50, models.py:63-65); these semantics are
+ * the library's own.  A raw head row o has 3K columns:
+ *   w = softmax(o[0:K]),  mu = o[K:2K],  sigma = softplus(o[2K:3K]) + 1e-3   (softplus(x) = x for x > 20)
+ * Target mixture of row i (from target_raw): weights w'_k, means r_i + c mu'_k, std devs c sigma'_k, with
+ * c = discount * (1 - done_i) -- a terminal row is a Dirac at r_i.
+ *   loss_rows [B]  L_i = -sum_{k,q} w'_k h_q / sqrt(pi) * log p(r_i + c (mu'_k + sqrt(2) sigma'_k x_q)), the
+ *                  cross-entropy of the online mixture p (from q_raw) under the target mixture, integrated with the
+ *                  8 Gauss-Hermite nodes (x_q, h_q) of d4pg_mog_quadrature (deterministic: no sampling)
+ *   td [B]         sum_j w_j mu_j - (r_i + c sum_k w'_k mu'_k);  prio [B] = |td| + prio_eps
+ *   dq_raw [B,3K]  d(mean loss)/d q_raw;  pi_rows [B] = -sum_j w_j mu_j of pi_raw;  dpi_raw [B,3K] its gradient
+ * Both gradients are multiplied by `grad_scale`.  Raw planes are dense [B,3K]; every output may be NULL, and so may
+ * pi_raw.  The row is evaluated in fp64, one warp per row.
+ * d4pg_mog_quadrature writes the 8 nodes x[8] and weights h[8] (numpy.polynomial.hermite.hermgauss(8)); host only.
+ * ------------------------------------------------------------------------------------- */
+int32_t d4pg_mog_loss(const float* target_raw, const float* q_raw, const float* pi_raw,
+                      const double* rewards, const uint8_t* dones, int32_t B, int32_t K,
+                      double discount, double prio_eps, float grad_scale,
+                      float* loss_rows, float* td, float* prio, float* dq_raw,
+                      float* pi_rows, float* dpi_raw, d4pg_stream_t stream);
+int32_t d4pg_mog_quadrature(double* x, double* h);
 
 /* ---------------------------------------------------------------------------------------
  * Prioritized replay: GPU-resident sum/min segment trees + SoA transition storage.
@@ -245,6 +269,22 @@ int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, int32_t act_d
                              float* grad_params, float* grad_s, float* grad_a, float* scratch,
                              int32_t precision, d4pg_stream_t stream);
 
+/* Mixture-of-Gaussians critic (K components, see d4pg_mog_loss): the critic MLP with a 3K-wide fc3 (parameters in
+ * d4pg_critic_layout(obs_dim, act_dim, 3K) order), then the head transform.
+ *   d4pg_critic_forward_mog   w, mu, sigma [B,K] f32 (required); raw [B,3K] the fc3 output (may be NULL: then h1 of the
+ *                             workspace is used as scratch, so a forward meant for the backward below must be given raw)
+ *   d4pg_critic_backward_mog  raw = the forward's raw output; grad_w, grad_mu, grad_sigma [B,K] (each may be NULL,
+ *                             counting as zero, not all three); everything else as d4pg_critic_backward with
+ *                             n_atoms = 3K (scratch f32 [B*(512 + 256)] since 3K <= 96). */
+int32_t d4pg_critic_forward_mog(const float* params, int32_t obs_dim, int32_t act_dim, int32_t K,
+                                const float* s, const float* a, int32_t B, float* w, float* mu, float* sigma,
+                                float* raw, float* workspace, int32_t precision, d4pg_stream_t stream);
+int32_t d4pg_critic_backward_mog(const float* params, int32_t obs_dim, int32_t act_dim, int32_t K,
+                                 const float* s, const float* a, int32_t B, const float* raw, const float* workspace,
+                                 const float* grad_w, const float* grad_mu, const float* grad_sigma,
+                                 float* grad_params, float* grad_s, float* grad_a, float* scratch,
+                                 int32_t precision, d4pg_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * Fused Adam + Polyak.  Replaces SharedAdam / torch.optim.Adam.step (shared_adam.py:3-17,
  * called at ddpg.py:232,244; torch-2.11 single-tensor formula), sync_local_global
@@ -309,6 +349,11 @@ typedef struct {
                                  gated on step k-1's priority write-back, while step k-1's backward pass, dW and Adam
                                  still run.  Tree operations keep the reference's order update(k-1) -> add(k) ->
                                  sample(k) (ddpg.py:200-255 + main.py's add loop): results are identical */
+  int32_t dist_type;          /* critic head: 0 = categorical (n_atoms, v_min, v_max), 1 = mixture of Gaussians with
+                                 n_components = K in [1, 32] (d4pg_mog_loss): n_atoms / v_min / v_max are ignored and the
+                                 critic's fc3 and every raw-head plane are 3K wide.  loss_flags & 2 is not supported with
+                                 the mixture (the cross-entropy of a density can be negative) */
+  int32_t n_components;
 } d4pg_learner_config_t;
 
 /* Caller-owned device buffers.  P_a / P_c = d4pg_*_layout().total. */
