@@ -30,7 +30,7 @@ Actor, Critic = actor, critic
 ReplayMemory = Replay
 PrioritizedReplayMemory = PrioritizedReplayBuffer
 
-__version__ = "0.4.0"
+__version__ = "0.5.0"
 
 
 def install_reference_aliases():

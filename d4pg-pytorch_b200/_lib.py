@@ -46,6 +46,7 @@ class LearnerConfig(C.Structure):
         ("world_size", C.c_int32), ("use_graph", C.c_int32),
         ("loss_flags", C.c_int32), ("chain", C.c_int32), ("prefetch", C.c_int32),
         ("dist_type", C.c_int32), ("n_components", C.c_int32),
+        ("qr_kappa", C.c_double),
     ]
 
 
@@ -74,6 +75,8 @@ _PROTOS = {
     "d4pg_mog_loss": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_float,
                                   _P, _P, _P, _P, _P, _P, _P]),
     "d4pg_mog_quadrature": (C.c_int32, [_P, _P]),
+    "d4pg_qr_loss": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_float,
+                                 C.c_int32, _P, _P, _P, _P, _P, _P, _P]),
     "d4pg_replay_capacity": (C.c_int32, [C.c_int64, C.POINTER(C.c_int64)]),
     "d4pg_replay_create": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32, C.c_double, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                        _P, C.POINTER(_P)]),

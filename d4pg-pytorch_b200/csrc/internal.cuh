@@ -46,6 +46,23 @@ int launch_mog_transform(const float* raw, int ldr, int B, int K, float* w, floa
 int launch_mog_head_backward(const float* raw, int ldr, const float* gw, const float* gmu, const float* gsig, int B, int K,
                              float* dz, int ldz, cudaStream_t st);
 
+// quantile-regression head (qr_heads.cu): every [B, N] quantile plane has row pitch `ld`
+struct QrArgs {
+  const float* target_q; const float* q; const float* pi_q;
+  const double* rewards; const uint8_t* dones;
+  int B, N, ld;
+  double discount, kappa, prio_eps;
+  float grad_scale;
+  float* loss_rows; float* td; float* prio; float* dq; float* pi_rows; float* dpi;
+  const float* is_weights;       // non-null: critic loss row i is scaled by the PER importance weight w_i
+  int ce_priority;               // 1: priority = L_i + eps (unweighted) instead of |td_i| + eps
+  int pdl;
+  unsigned long long* trace;
+  int only_policy;               // as HeadsArgs::only_policy
+  LearnerClock* sampler_clock;   // as HeadsArgs::sampler_clock
+};
+int launch_qr_heads(const QrArgs& a, cudaStream_t st);
+
 constexpr int SAMPLE_ROWS = 32;      // batch rows per CTA of the sample + gather kernel (replay_dev.cuh)
 
 // sample for the learner: per-step scalars come from device memory (graph replay safe)

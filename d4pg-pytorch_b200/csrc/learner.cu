@@ -350,7 +350,8 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     if (L->profiling) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);    \
       std::string nm0(#expr);                                                              \
       /* the loss kernel also advances the sampler clock under the prefetch pipeline: not idempotent there */ \
-      const bool rep = nm0.rfind("gemm_launch", 0) == 0 || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0) && !pf) || \
+      const bool rep = nm0.rfind("gemm_launch", 0) == 0 || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0 || \
+                                                            nm0.rfind("launch_qr_heads", 0) == 0) && !pf) || \
                        nm0.rfind("launch_mlp_chain", 0) == 0 || nm0.rfind("launch_mlp_tc_chain", 0) == 0; \
       cudaEventRecord(e0, st); rc = (expr);                                                \
       for (int _r = 1; rep && _r < PROFILE_REPS && rc == 0; ++_r) rc = (expr);             \
@@ -509,6 +510,16 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   ma.pi_rows = w.pi_rows; ma.dpi_raw = w.dlogits_pi;
   ma.is_weights = ((c.loss_flags & 1) && c.prioritized) ? bwts : nullptr;
   ma.sampler_clock = pf ? w.clock : nullptr;
+  //    (quantile critic: the quantile-Huber loss, td, priorities and quantile gradients of qr_heads.cu)
+  const bool qr = c.dist_type == 2;
+  QrArgs qa{};
+  qa.target_q = w.out[1]; qa.q = w.out[2]; qa.pi_q = h7 ? nullptr : w.out[4];
+  qa.rewards = w.r; qa.dones = w.done; qa.B = B; qa.N = N; qa.ld = Np;
+  qa.discount = ma.discount; qa.kappa = c.qr_kappa; qa.prio_eps = c.prio_eps; qa.grad_scale = ma.grad_scale;
+  qa.loss_rows = w.loss_rows; qa.td = b.td; qa.prio = b.prio; qa.dq = w.dlogits_q;
+  qa.pi_rows = w.pi_rows; qa.dpi = w.dlogits_pi;
+  qa.is_weights = ma.is_weights; qa.ce_priority = (c.loss_flags & 2) ? 1 : 0;
+  qa.sampler_clock = ma.sampler_clock;
   HeadsArgs ha{};
   ha.target_logits = w.out[1]; ha.q_logits = w.out[2]; ha.pi_logits = h7 ? nullptr : w.out[4];
   ha.rewards = w.r; ha.dones = w.done; ha.B = B; ha.N = N; ha.flags = 0; ha.ld = Np;
@@ -523,6 +534,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   ha.sampler_clock = pf ? w.clock : nullptr;          // sample(t) is done, sample(t+1) not yet launched
   ha.ce_priority = (c.loss_flags & 2) ? 1 : 0;
   if (mog) RUN(launch_mog_heads(ma, st));
+  else if (qr) RUN(launch_qr_heads(qa, st));
   else RUN(launch_heads(ha, c.proj_mode, st));
 
   // 4. priorities into the trees (ddpg.py:252-255): independent of the backward pass, so it runs
@@ -743,7 +755,10 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
     hp.pi_logits = w.out[4]; hp.only_policy = 1; hp.sampler_clock = nullptr;
     MogArgs mp = ma;
     mp.pi_raw = w.out[4]; mp.only_policy = 1; mp.sampler_clock = nullptr;
+    QrArgs qp = qa;
+    qp.pi_q = w.out[4]; qp.only_policy = 1; qp.sampler_clock = nullptr;
     if (mog) RUN(launch_mog_heads(mp, st));
+    else if (qr) RUN(launch_qr_heads(qp, st));
     else RUN(launch_heads(hp, c.proj_mode, st));
     TccArgs& bb = L->tcc_bwd_args;
     tcc_args_begin(bb, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); bb.step_slot = 5;
@@ -777,8 +792,14 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
                                        d4pg_replay_t* replay, d4pg_comm_t* comm, d4pg_learner_t** out) {
   D4PG_REQUIRE(cfg && buf && replay && out, D4PG_EINVAL, "d4pg_learner_create: null argument");
   D4PG_REQUIRE(cfg->batch > 0 && cfg->obs_dim > 0 && cfg->act_dim > 0, D4PG_EINVAL, "d4pg_learner_create: bad dims");
-  D4PG_REQUIRE(cfg->dist_type == 0 || cfg->dist_type == 1, D4PG_EINVAL, "d4pg_learner_create: dist_type must be 0 (categorical) or 1 (mixture of Gaussians)");
-  if (cfg->dist_type == 1) {
+  D4PG_REQUIRE(cfg->dist_type >= 0 && cfg->dist_type <= 2, D4PG_EINVAL,
+               "d4pg_learner_create: dist_type must be 0 (categorical), 1 (mixture of Gaussians) or 2 (quantile regression)");
+  if (cfg->dist_type == 2) {
+    D4PG_REQUIRE(cfg->n_atoms >= 2 && cfg->n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL,
+                 "d4pg_learner_create: the quantile critic's n_atoms (its N quantiles) must be in [2,%d]", D4PG_MAX_ATOMS);
+    D4PG_REQUIRE(std::isfinite(cfg->qr_kappa) && cfg->qr_kappa > 0.0, D4PG_EINVAL,
+                 "d4pg_learner_create: qr_kappa must be finite and > 0 (got %g)", cfg->qr_kappa);
+  } else if (cfg->dist_type == 1) {
     D4PG_REQUIRE(cfg->n_components >= 1 && cfg->n_components <= D4PG_MAX_COMPONENTS, D4PG_EINVAL,
                  "d4pg_learner_create: n_components must be in [1,%d]", D4PG_MAX_COMPONENTS);
     D4PG_REQUIRE(!(cfg->loss_flags & 2), D4PG_ENOTSUP,

@@ -55,6 +55,8 @@ class _Learner(object):
         cfg.obs_dim, cfg.act_dim, cfg.n_atoms, cfg.batch = ddpg.obs_dim, ddpg.act_dim, ddpg.n_atoms, B
         if ddpg.n_components is not None:       # mixture critic: n_atoms / v_min / v_max are ignored by the library
             cfg.dist_type, cfg.n_components, cfg.v_min, cfg.v_max = 1, ddpg.n_components, 0.0, 0.0
+        elif ddpg.n_quantiles is not None:      # quantile critic: n_atoms = N quantiles, v_min / v_max are ignored
+            cfg.dist_type, cfg.qr_kappa, cfg.v_min, cfg.v_max = 2, ddpg.qr_kappa, 0.0, 0.0
         else:
             cfg.v_min, cfg.v_max = float(ddpg.v_min), float(ddpg.v_max)
         cfg.gamma = float(ddpg.gamma)
@@ -206,7 +208,17 @@ class DDPG:
         self.actor_critic = actor_critic
 
         self.dist_type = critic_dist_info["type"]
-        if self.dist_type == "mixture_of_gaussian":
+        self.n_quantiles = self.qr_kappa = None
+        if self.dist_type == "quantile":
+            # {"type": "quantile", "n_quantiles": N, "kappa": 1.0}: quantile regression (QR-DQN).  The critic's fc3 gives
+            # N quantiles at tau_k = (2k+1) / (2N); the critic loss is the quantile-Huber loss against the N bootstrapped
+            # target quantiles (csrc/qr_heads.cu); td = mean(theta) - (r + c mean(theta')).  Validated by the critic.
+            self.n_components = None
+            self.n_quantiles = int(critic_dist_info["n_quantiles"])
+            self.qr_kappa = float(critic_dist_info.get("kappa", 1.0))
+            self.v_min = self.v_max = self.delta = self.bin_centers = None
+            self.n_atoms = self.n_quantiles
+        elif self.dist_type == "mixture_of_gaussian":
             # {"type": "mixture_of_gaussian", "n_components": K}: the reference stubs this branch (ddpg.py:48-50).  The
             # critic loss is the cross-entropy of the online mixture under the target mixture, integrated with 8
             # Gauss-Hermite nodes per target component (csrc/mog_heads.cu); td = E[Q] - (r + c E[Q']).
@@ -224,8 +236,8 @@ class DDPG:
             self.delta = (self.v_max - self.v_min) / float(self.n_atoms - 1)
             self.bin_centers = np.array([self.v_min + i * self.delta for i in range(self.n_atoms)]).reshape(-1, 1)
         else:
-            raise NotImplementedError("critic_dist_info['type'] must be 'categorical' or 'mixture_of_gaussian', got %r"
-                                      % (self.dist_type,))
+            raise NotImplementedError("critic_dist_info['type'] must be 'categorical', 'mixture_of_gaussian' or "
+                                      "'quantile', got %r" % (self.dist_type,))
 
         # networks, built in the reference's order so a seeded RNG yields the same weights (ddpg.py:56-64)
         self.actor = actor(input_size=obs_dim, output_size=act_dim, device=self.device)
@@ -295,9 +307,9 @@ class DDPG:
 
     # ---- projections as standalone methods (numpy in / numpy out, computed on the GPU) --------
     def _project(self, target_z_dist, rewards, terminates, mode):
-        if self.n_components is not None:
+        if self.dist_type != "categorical":
             raise _lib.D4PGError("reproject2 / reproj_categorical_dist project onto the categorical atoms; this DDPG has "
-                                 "a mixture_of_gaussian critic")
+                                 "a %s critic" % self.dist_type)
         _lib.require_cuda()
         p = torch.as_tensor(np.ascontiguousarray(target_z_dist, dtype=np.float32)).to(self.device)
         B, N = p.shape

@@ -9,6 +9,8 @@ learner, the fused Adam/Polyak kernel and the gradient all-reduce operate on; th
 eager/CPU fallback -- on a box without a GPU the modules can be built and (de)serialised
 but `forward` raises.
 """
+import math
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -252,12 +254,27 @@ class critic(_FlatNet):
 
     dist_info {"type": "mixture_of_gaussian", "n_components": K} (1 <= K <= 32; the reference stubs this branch,
     models.py:63-65): fc3 is Linear(256, 3K) and forward returns (w, mu, sigma), each [B, K]: w = softmax(raw[:, :K]),
-    mu = raw[:, K:2K], sigma = softplus(raw[:, 2K:]) + 1e-3.  `n_atoms` is then the raw head width 3K."""
+    mu = raw[:, K:2K], sigma = softplus(raw[:, 2K:]) + 1e-3.  `n_atoms` is then the raw head width 3K.
+
+    dist_info {"type": "quantile", "n_quantiles": N, "kappa": 1.0} (2 <= N <= 128, kappa finite and > 0, default 1.0):
+    fc3 is Linear(256, N), built like a categorical fc3 with N atoms, and forward returns the quantiles theta [B, N],
+    the raw fc3 output (quantile k at tau_k = (2k+1) / (2N)).  `n_atoms` is N; `kappa` is the Huber threshold of the
+    learner's quantile-Huber loss (it does not enter the module)."""
 
     def __init__(self, state_size, action_size, dist_info, device=None, differentiable=False):
         self.dist_info = dist_info
         self.dist_type = dist_info["type"]
-        if self.dist_type == "mixture_of_gaussian":
+        self.n_quantiles = self.kappa = None
+        if self.dist_type == "quantile":
+            self.n_components = None
+            self.n_quantiles = int(dist_info["n_quantiles"])
+            if not 2 <= self.n_quantiles <= _lib.MAX_ATOMS:
+                raise _lib.D4PGError("n_quantiles must be in [2, %d], got %d" % (_lib.MAX_ATOMS, self.n_quantiles))
+            self.kappa = float(dist_info.get("kappa", 1.0))
+            if not (math.isfinite(self.kappa) and self.kappa > 0.0):
+                raise _lib.D4PGError("kappa must be finite and > 0, got %r" % (self.kappa,))
+            head = self.n_quantiles
+        elif self.dist_type == "mixture_of_gaussian":
             self.n_components = int(dist_info["n_components"])
             if not 1 <= self.n_components <= _lib.MAX_COMPONENTS:
                 raise _lib.D4PGError("n_components must be in [1, %d], got %d" % (_lib.MAX_COMPONENTS, self.n_components))
@@ -266,8 +283,8 @@ class critic(_FlatNet):
             self.n_components = None
             head = int(dist_info["n_atoms"])
         else:
-            raise NotImplementedError("critic_dist_info['type'] must be 'categorical' or 'mixture_of_gaussian', got %r"
-                                      % (self.dist_type,))
+            raise NotImplementedError("critic_dist_info['type'] must be 'categorical', 'mixture_of_gaussian' or "
+                                      "'quantile', got %r" % (self.dist_type,))
         self.state_size, self.action_size, self.n_atoms = state_size, action_size, head
         super().__init__([(state_size, HIDDEN), (HIDDEN + action_size, HIDDEN), (HIDDEN, HIDDEN),
                           (HIDDEN, self.n_atoms)], device)
@@ -280,10 +297,13 @@ class critic(_FlatNet):
 
     def forward(self, state, action, return_logits=False):
         """Categorical: probs (and logits with return_logits).  Mixture: (w, mu, sigma) (and the raw fc3 output
-        [B, 3K] as a fourth element with return_logits)."""
+        [B, 3K] as a fourth element with return_logits).  Quantile: theta [B, N], which already is the raw fc3 output
+        (return_logits is ignored)."""
         _lib.require_cuda()
         if self.n_components is not None:
             return self._forward_mog(state, action, return_logits)
+        if self.n_quantiles is not None:
+            return self._forward_qr(state, action)
         if self._use_autograd((state, action)):
             x = self._as_grad_input(state, self.state_size)
             a = self._as_grad_input(action, self.action_size)
@@ -316,6 +336,21 @@ class critic(_FlatNet):
                                                       _lib.ptr(sigma), _lib.ptr(raw), _lib.ptr(self._workspace(B)),
                                                       int(self.precision), _lib.stream_ptr()), "d4pg_critic_forward_mog")
         return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
+
+    def _forward_qr(self, state, action):
+        if self._use_autograd((state, action)):
+            x = self._as_grad_input(state, self.state_size)
+            a = self._as_grad_input(action, self.action_size)
+            return _CriticQrFn.apply(self, int(self.precision), x, a, *self._grad_params())
+        x = self._as_input(state, self.state_size)
+        a = self._as_input(action, self.action_size)
+        B = x.shape[0]
+        theta = torch.empty(B, self.n_atoms, dtype=torch.float32, device=x.device)
+        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(self._flat), self.state_size, self.action_size, self.n_atoms,
+                                                  _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(theta),
+                                                  _lib.ptr(self._workspace(B)), int(self.precision), _lib.stream_ptr()),
+                   "d4pg_critic_forward")
+        return theta
 
 
 def _backward_scratch(B, out_dim, device):
@@ -455,6 +490,46 @@ class _CriticMogFn(torch.autograd.Function):
                                                        _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(grad_a),
                                                        _lib.ptr(scratch), ctx.precision, _lib.stream_ptr()),
                    "d4pg_critic_backward_mog")
+        return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
+
+
+class _CriticQrFn(torch.autograd.Function):
+    """theta = quantile critic(state, action) through d4pg_critic_forward without the softmax (probs = NULL); backward =
+    d4pg_critic_backward with grad_logits = d loss / d theta (no head Jacobian)."""
+
+    @staticmethod
+    def forward(ctx, net, precision, x, a, *params):
+        B = x.shape[0]
+        theta = torch.empty(B, net.n_atoms, dtype=torch.float32, device=x.device)
+        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)      # h1..h3, kept for backward
+        flat = net._flat
+        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(flat), net.state_size, net.action_size, net.n_atoms,
+                                                  _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(theta), _lib.ptr(ws),
+                                                  precision, _lib.stream_ptr()), "d4pg_critic_forward")
+        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(x, a, *params)
+        return theta
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, a = ctx.saved_tensors[:2]
+        net = ctx.net
+        if g is None:
+            return (None,) * (4 + 8)
+        B = x.shape[0]
+        g = g.to(dtype=torch.float32).contiguous()
+        want_p = any(ctx.needs_input_grad[4:])
+        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
+        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
+        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
+        scratch = _backward_scratch(B, net.n_atoms, x.device)
+        _lib.check(_lib.lib().d4pg_critic_backward(_lib.ptr(ctx.flat), net.state_size, net.action_size, net.n_atoms,
+                                                   _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(ctx.ws), None,
+                                                   _lib.ptr(g), _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(grad_a),
+                                                   _lib.ptr(scratch), ctx.precision, _lib.stream_ptr()),
+                   "d4pg_critic_backward")
         return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
 
 

@@ -120,6 +120,30 @@ int32_t d4pg_mog_loss(const float* target_raw, const float* q_raw, const float* 
 int32_t d4pg_mog_quadrature(double* x, double* h);
 
 /* ---------------------------------------------------------------------------------------
+ * Quantile-regression critic head (critic_dist_info['type'] == 'quantile', N = n_quantiles in [2, D4PG_MAX_ATOMS]):
+ * the quantile-Huber loss of QR-DQN (Dabney et al. 2018).  The reference has no quantile code; these semantics are the
+ * library's own.  A row theta [N] is the critic's raw fc3 output (no head transform); quantile k sits at the midpoint
+ * tau_k = (2k+1) / (2N).  With c = discount * (1 - done_i), targets y_j = r_i + c theta'_j (theta' from target_q; a
+ * terminal row's targets are all r_i), u_jk = y_j - theta_k,
+ *   H(u) = u^2/2 if |u| <= kappa, else kappa (|u| - kappa/2);   rho_jk = |tau_k - 1{u_jk < 0}| H(u_jk) / kappa
+ *   loss_rows [B]  L_i = (1/N) sum_j sum_k rho_jk   (>= 0; no gradient into the target)
+ *   dq [B,N]       grad_scale * dL_i/dtheta_k = -grad_scale/N sum_j |tau_k - 1{u_jk < 0}| clamp(u_jk, -kappa, kappa) / kappa
+ *   td [B]         mean_k theta_k - (r_i + c mean_j theta'_j);  prio [B] = |td| + prio_eps, or L_i + prio_eps when
+ *                  ce_priority != 0
+ *   pi_rows [B]    -mean_k theta_k of pi_q;  dpi [B,N] = -grad_scale / N
+ * kappa must be finite and > 0.  Planes are dense [B,N]; every output may be NULL, and so may pi_q.  One warp per row,
+ * the N^2 pair terms in fp64; no atomics (run-to-run identical).  In the learner (dist_type 2) the loss row is also
+ * multiplied by the PER importance weight with loss_flags & 1, and so is dq.
+ * The critic module of a quantile critic is d4pg_critic_forward with probs = NULL (logits = theta) and
+ * d4pg_critic_backward with probs = grad_probs = NULL (grad_logits = d loss / d theta).
+ * ------------------------------------------------------------------------------------- */
+int32_t d4pg_qr_loss(const float* target_q, const float* q, const float* pi_q,
+                     const double* rewards, const uint8_t* dones, int32_t B, int32_t N,
+                     double discount, double kappa, double prio_eps, float grad_scale, int32_t ce_priority,
+                     float* loss_rows, float* td, float* prio, float* dq,
+                     float* pi_rows, float* dpi, d4pg_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Prioritized replay: GPU-resident sum/min segment trees + SoA transition storage.
  * Replaces SegmentTree / SumSegmentTree / MinSegmentTree (prioritized_replay_memory.py:33-162),
  * ReplayBuffer (:164-222) and PrioritizedReplayBuffer (:224-335).
@@ -352,8 +376,12 @@ typedef struct {
   int32_t dist_type;          /* critic head: 0 = categorical (n_atoms, v_min, v_max), 1 = mixture of Gaussians with
                                  n_components = K in [1, 32] (d4pg_mog_loss): n_atoms / v_min / v_max are ignored and the
                                  critic's fc3 and every raw-head plane are 3K wide.  loss_flags & 2 is not supported with
-                                 the mixture (the cross-entropy of a density can be negative) */
+                                 the mixture (the cross-entropy of a density can be negative).  2 = quantile regression
+                                 (d4pg_qr_loss): n_atoms carries the number of quantiles N in [2, D4PG_MAX_ATOMS], v_min /
+                                 v_max are ignored, qr_kappa is the Huber threshold; loss_flags & 2 gives
+                                 priority = L_i + eps (the quantile-Huber loss is non-negative) */
   int32_t n_components;
+  double  qr_kappa;           /* dist_type 2: Huber threshold kappa, finite and > 0 (1.0 is the usual choice) */
 } d4pg_learner_config_t;
 
 /* Caller-owned device buffers.  P_a / P_c = d4pg_*_layout().total. */
