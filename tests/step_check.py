@@ -1,0 +1,322 @@
+"""One learner step, layer by layer: every forward layer, dX layer, weight gradient and bias gradient of one eager
+DDPG.train() recomputed in float64 from the DEVICE's own input to that layer (teacher forcing), and held to a
+componentwise bound.
+
+Teacher forcing.  Each layer is fed the device's input plane, the device's ReLU mask (h > 0) and the device's upstream
+delta, and the tanh' factor is 1 - y^2 of the device's own actor output.  A pre-activation within rounding of zero then
+masks the same element on both sides, so no delta element can flip and a tight bound survives any batch size.
+
+Rounding.  `rho` is the operand rounding the plan's kernels apply before the products: None for fp32 and 3xTF32
+(tf32x3), "rz" / "rna" for one TF32 pass (tests/tf32_oracle.py), "bf16" for the bf16 kernels (tests/bf16_oracle.py).
+Which kernel computes dW, and so whether dW is rounded, follows the plan table of test_gpu_tf32.py (`MODES` below).
+
+Bound.  An element computed as sum_k a_k b_k (+ bias) from K products, with S = |rho(A)| |rho(B)|^T (+ |bias|):
+
+    |dev - ref| <= (ALPHA * 2^-24 * sqrt(K) + beta + TRUNC * Kc * 2^-24) * S
+
+Kc is the number of rows one tensor-core accumulator sums (0 for the FFMA kernels; see TRUNC).  beta = 0 where the oracle reproduces the operand rounding (fp32, tf32, bf16), BETA_3XTF32 for the 3xTF32 split, which
+the oracle does not reproduce (it takes the fp32 operands as exact).  A bias gradient is sum_k delta_k: S = sum |delta|.
+ReLU and tanh are 1-Lipschitz and keep the pre-activation bound; tanh adds 4 ulp of its output, and the tanh' factor of
+d action (computed in fp32 from y) adds 4 ulp of its input sum.  On the CPU (test_gpu_step_edges.py), fp32 matmul,
+8-way split-K and sequential fp32 accumulation reach at most 0.99 x 2^-24 sqrt(K) S (at K = 1), the 3xTF32 split
+with rz hi/lo 1.23 x 2^-20 S; dropping one row's contribution exceeds the bound by > 100x.
+
+Power.  A bound is only worth what it rejects: for every weight and bias gradient, the reference with the contribution
+of the last batch row that contributes anything removed must be at least POWER_MIN x the bound away from the device.
+
+Layers the wgmma chains keep inside the cluster (the target chains' hidden planes, p_dz22 and p_dz2) are not written
+row-major, so actor_target_out, target_logits and a_dz3 are checked through the float64 chain (each layer cast to fp32
+as the device stores it) at relative L2 (`CHAINED_TOL`).  actor_critic="post_update" sends the policy pass through the
+critic AFTER its Adam step, whose h1 the device recomputes without storing: h2_p is checked through that chain too.
+"""
+import math
+
+import torch
+
+from tests import bf16_oracle as BO
+from tests import tf32_oracle as TO
+
+H_ = 256
+U = 2.0 ** -24                     # unit roundoff of fp32
+ALPHA = 4.0
+BETA_3XTF32 = 4 * 2.0 ** -20
+# The tensor cores' fp32 accumulator rounds its adds toward zero, so over a sum whose terms share a sign the errors do
+# not cancel: each add loses up to 2^-23 of a partial sum that grows toward S, ~2^-24 S per row on average.  Sequential
+# round-toward-zero accumulation of same-sign terms reaches 0.35-0.46 x K 2^-24 S on the CPU (test_gpu_step_edges.py),
+# and 3xTF32 dW on wgmma reached 1.9x the sqrt(K) bound alone at 1023 unsplit rows (~2.1e-5 S, the same as that
+# emulation's 2.3e-5 S).
+TRUNC = 1.0
+POWER_MIN = 10.0
+
+# (plan, precision) -> (rho, beta, tensor-core accumulation) of forward / dX, then the same of dW
+#   tc_chain  mlp_tc_chain.cu wgmma chains; dW with exact fp32 FFMA (gemm_wide_kernel)
+#   chain     mlp_chain.cu cluster chains: FFMA tiles at fp32, mma.sync tiles otherwise; dW as above
+#   levels    one launch per level: gemm_ffma (fp32), gemm_tc (wgmma tf32x3 / tf32), gemm_bf16 -- dW included
+MODES = {("tc_chain", "tf32x3"): (None, BETA_3XTF32, True, None, 0.0, False),
+         ("tc_chain", "tf32"): ("rz", 0.0, True, None, 0.0, False),
+         ("chain", "fp32"): (None, 0.0, False, None, 0.0, False),
+         ("chain", "tf32x3"): (None, BETA_3XTF32, True, None, 0.0, False),
+         ("chain", "tf32"): ("rna", 0.0, True, None, 0.0, False),
+         ("levels", "fp32"): (None, 0.0, False, None, 0.0, False),
+         ("levels", "tf32x3"): (None, BETA_3XTF32, True, None, BETA_3XTF32, True),
+         ("levels", "tf32"): ("rz", 0.0, True, "rz", 0.0, True),
+         ("levels", "bf16"): ("bf16", 0.0, True, "bf16", 0.0, True)}
+
+
+def kslice(K):
+    """Rows one dW accumulator sums on the level plan: split-K from 1024 rows (csrc/gemm_ffma.cu prepare_problem)."""
+    if K < 1024:
+        return K
+    ksplit = min(8, -(-K // 512))
+    return -(-(-(-K // ksplit)) // 64) * 64
+# kernels of one eager step, by plan (no post-update critic)
+KERNELS = {"tc_chain": 9, "chain": 7, "levels": 18}
+# relative L2 of the chained checks: a one-pass TF32 chain may truncate a chained operand whose fp32 value differs in
+# the last bit to the neighbouring TF32 value (test_gpu_tf32.py); an unrounded chain differs by fp32 casts only
+CHAINED_TOL = {None: {"actor_target_out*": 1e-5, "target_logits*": 1e-5, "a_dz3*": 1e-5, "h2_p*": 1e-5},
+               "rz": {"actor_target_out*": 5e-5, "target_logits*": 5e-6, "a_dz3*": 1e-4, "h2_p*": 5e-5}}
+
+
+def rnd(t, rho):
+    """The operand a kernel with rounding `rho` multiplies, held exactly in float64."""
+    if rho is None:
+        return t.double()
+    if rho == "bf16":
+        return BO.rb(t)
+    return TO.rt(t, rho)
+
+
+def bound(S, K, beta=0.0, alpha=ALPHA, kc=0):
+    """kc: rows summed by one tensor-core accumulator (0: none), whose fp32 adds truncate (TRUNC below)."""
+    return (alpha * U * math.sqrt(K) + beta + TRUNC * kc * U) * S
+
+
+def ratio(dev, ref, tol):
+    """max |dev - ref| / tol; an element with tol == 0 (every product zero) must match exactly."""
+    err = (dev.double() - ref).abs()
+    zero = tol == 0
+    r = torch.where(zero, torch.zeros_like(err), err / torch.where(zero, torch.ones_like(tol), tol))
+    if bool((zero & (err != 0)).any()):
+        return math.inf
+    return float(r.max()) if r.numel() else 0.0
+
+
+def matmul_bound(a, b, rho, beta=0.0, kc=0):
+    """a [M, K] @ b [K, N] on rho-rounded operands: (float64 reference, componentwise bound)."""
+    ra, rb_ = rnd(a, rho), rnd(b, rho)
+    return ra @ rb_, bound(ra.abs() @ rb_.abs(), a.shape[1], beta, kc=kc)
+
+
+def drop_row_ratio(dev, ref, tol, a, b, rho):
+    """For ref = a^T b (a [K, M], b [K, N] or None for a column sum): the ratio to the bound of the reference with the
+    contribution of the last row k whose contribution is nonzero removed; None when no row contributes."""
+    ra = rnd(a, rho)
+    rb_ = rnd(b, rho) if b is not None else None
+    nz = (ra != 0).any(1) if rb_ is None else ((ra != 0).any(1) & (rb_ != 0).any(1))
+    rows = torch.nonzero(nz).flatten()
+    if rows.numel() == 0:
+        return None
+    k = int(rows[-1])
+    contrib = ra[k] if rb_ is None else torch.outer(ra[k], rb_[k])
+    return ratio(dev, ref - contrib.reshape(ref.shape), tol)
+
+
+class Report:
+    """(name, ratio to the bound) of every check and the power ratios; all printed before the first failure."""
+
+    def __init__(self, label):
+        self.label, self.rows, self.power, self.chained = label, [], [], []
+
+    def add(self, name, r):
+        self.rows.append((name, r))
+
+    def finish(self):
+        for name, r in self.rows:
+            print("%s %-20s %.3f of bound" % (self.label, name, r))
+        for name, r, tol in self.chained:
+            print("%s %-20s rel L2 %.3e (bound %.1e)" % (self.label, name, r, tol))
+        for name, r in self.power:
+            print("%s %-20s last contributing row dropped: %.3g x bound" % (self.label, name, r))
+        worst = max((r for _, r in self.rows), default=0.0)
+        pmin = min((r for _, r in self.power if r is not None), default=math.inf)
+        print("%s worst %.3f of bound, smallest power ratio %.3g" % (self.label, worst, pmin))
+        bad = ["%s %.3g" % (n, r) for n, r in self.rows if not r <= 1.0]
+        bad += ["%s rel L2 %.3e > %.1e" % (n, r, tol) for n, r, tol in self.chained if not r <= tol]
+        bad += ["%s power %s" % (n, r) for n, r in self.power if r is None or not r >= POWER_MIN]
+        assert not bad, "%s: %s" % (self.label, ", ".join(bad))
+        return worst, pmin
+
+
+def snapshot(dd):
+    """The four networks' weights before a step (float32, on the CPU)."""
+    return {k: {n_: v.detach().cpu().clone() for n_, v in net.state_dict().items()}
+            for k, net in (("a", dd.actor), ("at", dd.actor_target), ("c", dd.critic), ("ct", dd.critic_target))}
+
+
+class StepCheck:
+    """The teacher-forced restatement of the step `dd` just ran from the weights `W` (a `snapshot` taken before it)."""
+
+    def __init__(self, dd, W, plan, precision, post_update=False, label=None):
+        self.rho, self.beta, self.tc_fwd, self.rho_dw, self.beta_dw, self.tc_dw = MODES[plan, precision]
+        self.tc, self.post_update = plan == "tc_chain", post_update
+        dev = dd.critic.fc3.weight.device
+        self.W = {k: {n_: v.to(dev) for n_, v in w.items()} for k, w in W.items()}
+        # the policy pass's critic: the critic after its Adam step under actor_critic="post_update"
+        self.W["p"] = ({n_: v.detach().clone() for n_, v in dd.critic.state_dict().items()} if post_update
+                       else self.W["c"])
+        self.N = W["c"]["fc3.weight"].shape[0]
+        self.S, self.A = W["a"]["fc1.weight"].shape[1], W["a"]["fc3.weight"].shape[0]
+        self.dd = dd
+        B = dd.batch_size
+        self.B = B
+        self.t = lambda name, w=None: dd.debug_tensor(name, (B, w) if w else None)
+        self.rep = Report(label or "%s/%s(%d,%d,%d,%d)" % (plan, precision, B, self.S, self.A, self.N))
+
+    def _width(self, name):
+        if name in ("actor_out", "actor_target_out", "a_dz3"):
+            return self.A
+        if "logits" in name:
+            return self.N
+        return H_
+
+    def dev(self, name):
+        return self.t(name, self._width(name))
+
+    # ---- one layer ------------------------------------------------------------------------------------------------
+    def forward(self, name, x, w, layer, act):
+        """y = act(x @ W^T + b) against the device plane `name`."""
+        W, b = w[layer + ".weight"], w[layer + ".bias"]
+        kc = x.shape[1] if self.tc_fwd else 0
+        ref, tol = matmul_bound(x, W.T, self.rho, self.beta, kc)
+        ref = ref + b.double()
+        tol = tol + bound(b.double().abs(), x.shape[1], self.beta, kc=kc)
+        if act == "relu":
+            ref = torch.relu(ref)
+        elif act == "tanh":
+            ref = torch.tanh(ref)
+            tol = tol + 4 * 2.0 ** -23 * ref.abs()
+        self.rep.add(name, ratio(self.dev(name), ref, tol))
+
+    def backward(self, name, g, w, mask=None, tanh_y=None):
+        """dX = (g @ W) * mask (or * (1 - y^2)) against the device plane `name`."""
+        ref, tol = matmul_bound(g, w, self.rho, self.beta, g.shape[1] if self.tc_fwd else 0)
+        if mask is not None:
+            ref, tol = ref * mask, tol * mask
+        if tanh_y is not None:
+            f = 1 - tanh_y.double() ** 2
+            S = rnd(g, self.rho).abs() @ rnd(w, self.rho).abs()
+            ref, tol = ref * f, tol * f.abs() + 4 * U * S
+        self.rep.add(name, ratio(self.dev(name), ref, tol))
+
+    def grad(self, name, dev, delta, x):
+        """dW = delta^T x (x None: the bias gradient, sum of the fp32 delta) against the device gradient `dev`, and the
+        power of the bound against a dropped row."""
+        if x is None:
+            ref, tol = delta.double().sum(0), bound(delta.double().abs().sum(0), delta.shape[0])
+            rho = None
+        else:
+            kc = kslice(delta.shape[0]) if self.tc_dw else 0
+            ref, tol = matmul_bound(delta.T, x, self.rho_dw, self.beta_dw, kc)
+            rho = self.rho_dw
+        dev = dev.to(ref.device).reshape(ref.shape)
+        self.rep.add(name, ratio(dev, ref, tol))
+        self.rep.power.append((name, drop_row_ratio(dev, ref, tol, delta, x, rho)))
+
+    def chained(self, name, dev, ref):
+        r = float((dev.double() - ref).norm()) / max(float(ref.norm()), 1e-30)
+        self.rep.chained.append((name, r, CHAINED_TOL["rz" if self.rho else None][name]))
+
+    def chain(self, x, w, layers):
+        """Layers in float64 on rho-rounded operands, each cast to fp32 as the device stores it."""
+        for l, act in layers:
+            y = rnd(x, self.rho) @ rnd(w[l + ".weight"], self.rho).T + w[l + ".bias"].double()
+            x = (torch.relu(y) if act == "relu" else torch.tanh(y) if act == "tanh" else y).float()
+        return x
+
+    # ---- the step ---------------------------------------------------------------------------------------------------
+    def run(self):
+        t, dev, W = self.t, self.dev, self.W
+        S, A, N = self.S, self.A, self.N
+        Wa, Wat, Wc, Wct, Wp = W["a"], W["at"], W["c"], W["ct"], W["p"]
+        s, a, s2 = t("s", S), t("a", A), t("s2", S)
+        f = self.forward
+        ah1, ah2, ah3, aout = dev("h1_a"), dev("h2_a"), dev("h3_a"), dev("actor_out")
+        f("h1_a", s, Wa, "fc1", "relu")
+        f("h2_a", ah1, Wa, "fc2", None)
+        f("h3_a", ah2, Wa, "fc2_2", "relu")
+        f("actor_out", ah3, Wa, "fc3", "tanh")
+        ch1, ch2, ch3 = dev("h1_c"), dev("h2_c"), dev("h3_c")
+        f("h1_c", s, Wc, "fc1", "relu")
+        f("h2_c", torch.cat([ch1, a], 1), Wc, "fc2", "relu")
+        f("h3_c", ch2, Wc, "fc2_2", "relu")
+        f("q_logits", ch3, Wc, "fc3", None)
+        ph2, ph3 = dev("h2_p"), dev("h3_p")
+        if self.post_update:      # h1 of the updated critic is recomputed on the device, not stored
+            self.chained("h2_p*", ph2, self.chain(torch.cat([self.chain(s, Wp, (("fc1", "relu"),)), aout], 1), Wp,
+                                                  (("fc2", "relu"),)).double())
+        else:                     # the policy pass's critic h1 is h1_c
+            f("h2_p", torch.cat([ch1, aout], 1), Wp, "fc2", "relu")
+        f("h3_p", ph2, Wp, "fc2_2", "relu")
+        f("pi_logits", ph3, Wp, "fc3", None)
+        at_out = dev("actor_target_out")
+        if not self.tc:
+            th1, th2, th3 = dev("h1_at"), dev("h2_at"), dev("h3_at")
+            f("h1_at", s2, Wat, "fc1", "relu")
+            f("h2_at", th1, Wat, "fc2", None)
+            f("h3_at", th2, Wat, "fc2_2", "relu")
+            f("actor_target_out", th3, Wat, "fc3", "tanh")
+            ct1, ct2, ct3 = dev("h1_ct"), dev("h2_ct"), dev("h3_ct")
+            f("h1_ct", s2, Wct, "fc1", "relu")
+            f("h2_ct", torch.cat([ct1, at_out], 1), Wct, "fc2", "relu")
+            f("h3_ct", ct2, Wct, "fc2_2", "relu")
+            f("target_logits", ct3, Wct, "fc3", None)
+        else:
+            self.chained("actor_target_out*", at_out,
+                         self.chain(s2, Wat, (("fc1", "relu"), ("fc2", None), ("fc2_2", "relu"), ("fc3", "tanh"))).double())
+            ct1 = self.chain(s2, Wct, (("fc1", "relu"),))
+            self.chained("target_logits*", dev("target_logits"),
+                         self.chain(torch.cat([ct1, at_out], 1), Wct, (("fc2", "relu"), ("fc2_2", "relu"), ("fc3", None))).double())
+
+        # backward: from the device's logit gradients, deltas and masks
+        dq, dpi = dev("dlogits_q"), dev("dlogits_pi")
+        m = lambda h: (h > 0).double()
+        bw = self.backward
+        c_dz22, c_dz2, c_dz1 = dev("c_dz22"), dev("c_dz2"), dev("c_dz1")
+        bw("c_dz22", dq, Wc["fc3.weight"], m(ch3))
+        bw("c_dz2", c_dz22, Wc["fc2_2.weight"], m(ch2))
+        bw("c_dz1", c_dz2, Wc["fc2.weight"][:, :H_], m(ch1))
+        a_dz3 = dev("a_dz3")
+        if self.tc:               # p_dz22 / p_dz2 stay in the cluster
+            p22 = (rnd(dpi, self.rho) @ rnd(Wp["fc3.weight"], self.rho) * m(ph3)).float()
+            p2 = (rnd(p22, self.rho) @ rnd(Wp["fc2_2.weight"], self.rho) * m(ph2)).float()
+            ref = rnd(p2, self.rho) @ rnd(Wp["fc2.weight"][:, H_:], self.rho) * (1 - aout.double() ** 2)
+            self.chained("a_dz3*", a_dz3, ref)
+        else:
+            p_dz22, p_dz2 = dev("p_dz22"), dev("p_dz2")
+            bw("p_dz22", dpi, Wp["fc3.weight"], m(ph3))
+            bw("p_dz2", p_dz22, Wp["fc2_2.weight"], m(ph2))
+            bw("a_dz3", p_dz2, Wp["fc2.weight"][:, H_:], tanh_y=aout)
+        a_dz22, a_dh2, a_dz1 = dev("a_dz22"), dev("a_dh2"), dev("a_dz1")
+        bw("a_dz22", a_dz3, Wa["fc3.weight"], m(ah3))
+        bw("a_dh2", a_dz22, Wa["fc2_2.weight"])
+        bw("a_dz1", a_dh2, Wa["fc2.weight"], m(ah1))
+
+        # weight and bias gradients from the device's deltas and activations
+        deltas = {"c": {"fc3": (dq, ch3), "fc2_2": (c_dz22, ch2), "fc2": (c_dz2, torch.cat([ch1, a], 1)), "fc1": (c_dz1, s)},
+                  "a": {"fc3": (a_dz3, ah3), "fc2_2": (a_dz22, ah2), "fc2": (a_dh2, ah1), "fc1": (a_dz1, s)}}
+        self.grads(deltas)
+        return self.rep.finish()
+
+    def grads(self, deltas):
+        """deltas: {"c" / "a": {layer: (delta, input)}} -> every weight and bias gradient of both networks."""
+        for key, net in (("c", self.dd.critic), ("a", self.dd.actor)):
+            views = net.named_grad_views()
+            for layer, (g, x) in deltas[key].items():
+                self.grad("%s.%s.weight" % (key, layer), views[layer + ".weight"], g, x)
+                self.grad("%s.%s.bias" % (key, layer), views[layer + ".bias"], g, None)
+
+
+def check_step(dd, W, plan, precision, post_update=False, label=None):
+    """Every layer of the step `dd` just ran (from the weights `W`) against its bound; returns (worst ratio to the
+    bound, smallest power ratio) after printing one line per check."""
+    return StepCheck(dd, W, plan, precision, post_update=post_update, label=label).run()

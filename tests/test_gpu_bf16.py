@@ -15,6 +15,7 @@ import torch
 from oracle import d4pg_oracle as O
 from tests import bf16_oracle as BO
 from tests import helpers as H
+from tests import step_check as SC
 
 H_ = 256
 rb = BO.rb
@@ -151,7 +152,8 @@ def _ddpg(d4pg, B, S, A, N, n=None, graph=False, chain="cluster", projection="re
 def test_bf16_every_intermediate_vs_rounded_restatement(B, S, A, N, graph, chain, projection):
     """Every activation, logit, delta and parameter gradient of one eager DDPG.train() at precision="bf16" against the
     float64 restatement on bf16-rounded operands.  Each layer is fed the device's own inputs and ReLU masks (the same
-    fp32 value rounds to the same bf16 on both sides); bound 1e-5 x max(1, |ref|max)."""
+    fp32 value rounds to the same bf16 on both sides); bound 1e-5 x max(1, |ref|max), for the parameter gradients (~1e-6)
+    the componentwise bound of tests/step_check.py."""
     import d4pg_b200 as d4pg
     dd = _ddpg(d4pg, B, S, A, N, graph=graph, chain=chain, projection=projection, n_steps=5 if projection == "nstep" else 1)
     with torch.no_grad():
@@ -219,20 +221,13 @@ def test_bf16_every_intermediate_vs_rounded_restatement(B, S, A, N, graph, chain
         err = float((dev[name].double() - ref).abs().max())
         assert err <= 1e-5 * max(gs, float(ref.abs().max())), "%s: %.3e vs scale %.3e" % (name, err, gs)
 
-    # dW from the device's deltas and activations; bias gradients are sums of the unrounded fp32 deltas
-    dw = lambda g, x: rb(g).T @ rb(x)
-    grads = {"c": {"fc3.weight": dw(dq, ch3), "fc3.bias": dq.double().sum(0),
-                   "fc2_2.weight": dw(dev["c_dz22"], ch2), "fc2_2.bias": dev["c_dz22"].double().sum(0),
-                   "fc2.weight": dw(dev["c_dz2"], torch.cat([ch1, a], 1)), "fc2.bias": dev["c_dz2"].double().sum(0),
-                   "fc1.weight": dw(dev["c_dz1"], s), "fc1.bias": dev["c_dz1"].double().sum(0)},
-             "a": {"fc3.weight": dw(dev["a_dz3"], ah3), "fc3.bias": dev["a_dz3"].double().sum(0),
-                   "fc2_2.weight": dw(dev["a_dz22"], ah2), "fc2_2.bias": dev["a_dz22"].double().sum(0),
-                   "fc2.weight": dw(dev["a_dh2"], ah1), "fc2.bias": dev["a_dh2"].double().sum(0),
-                   "fc1.weight": dw(dev["a_dz1"], s), "fc1.bias": dev["a_dz1"].double().sum(0)}}
-    for key, net in (("c", dd.critic), ("a", dd.actor)):
-        views = net.named_grad_views()
-        for k, ref in grads[key].items():
-            _close("%s.%s" % (key, k), views[k].cpu().reshape(ref.shape), ref)
+    # dW from the device's deltas and activations on bf16-rounded operands, bias gradients as sums of the unrounded
+    # fp32 deltas: against the componentwise bound of tests/step_check.py, with its power check
+    sc = SC.StepCheck(dd, W, "levels", "bf16", label="bf16(%d,%d,%d,%d)" % (B, S, A, N))
+    sc.grads({"c": {"fc3": (dq, ch3), "fc2_2": (dev["c_dz22"], ch2), "fc2": (dev["c_dz2"], torch.cat([ch1, a], 1)),
+                    "fc1": (dev["c_dz1"], s)},
+              "a": {"fc3": (dev["a_dz3"], ah3), "fc2_2": (dev["a_dz22"], ah2), "fc2": (dev["a_dh2"], ah1), "fc1": (dev["a_dz1"], s)}})
+    sc.rep.finish()
 
 
 def _rel(x, ref):

@@ -20,6 +20,7 @@ from oracle import d4pg_oracle as O
 from tests import bf16_oracle as BO
 from tests import helpers as H
 from tests import qr_oracle as QO
+from tests import step_check as SC
 from tests import tf32_oracle as TO
 
 H_ = 256
@@ -263,6 +264,8 @@ def _snapshot(dd):
 
 PLANS = {"wgmma": ("tf32x3", 256, "cluster"), "mma_ffma": ("fp32", 256, "cluster"), "levels_b1024": ("fp32", 1024, "cluster"),
          "levels": ("tf32x3", 256, "levels")}
+STEP_PLANS = {"wgmma": ("tc_chain", "tf32x3"), "mma_ffma": ("chain", "fp32"), "levels_b1024": ("levels", "fp32"),
+              "levels": ("levels", "tf32x3")}       # (step plan, precision) of tests/step_check.py
 
 
 @pytest.mark.gpu
@@ -290,6 +293,7 @@ def test_qr_learner_step_vs_oracle(N, plan, variant):
         pr = (np.random.RandomState(3).rand(len(S)).astype(np.float32) + np.float32(1e-3))
         dd.replayBuffer.update_priorities(np.arange(len(S)), pr)
     W = _snapshot(dd)
+    W_step = SC.snapshot(dd)                          # the oracle's Adam and Polyak update W in place
     lo = QO.QrLearnerOracle(17, 6, N, n_steps=kw.get("n_steps", 1), projection="nstep" if variant == "nstep" else "live",
                             actor_w=W["a"], critic_w=W["c"])
     lo.actor_target, lo.critic_target = W["at"], W["ct"]
@@ -316,10 +320,8 @@ def test_qr_learner_step_vs_oracle(N, plan, variant):
     for name, ref in (("dlogits_q", out["dq"]), ("dlogits_pi", out["dpi"])):
         err = float((t(name, N).double() - ref.double()).abs().max())
         assert err <= 1e-5 * gs, (name, err, gs)
-    for key, net, grads in (("critic", dd.critic, out["grads_critic"]), ("actor", dd.actor, out["grads_actor"])):
-        views = net.named_grad_views()
-        for k in H.NAMES:
-            _close("%s grad %s" % (key, k), views[k].cpu(), grads[k])
+    # every layer and parameter gradient from the device's own quantile gradients (held to the oracle above)
+    SC.check_step(dd, W_step, *STEP_PLANS[plan], post_update=variant == "post_update", label="qr %s/%s N=%d" % (plan, variant, N))
 
 
 @pytest.mark.gpu

@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import step_check as SC
 from tests import tf32_oracle as TO
 
 H_ = 256
@@ -210,7 +211,8 @@ TOL_CHAINED = {"actor_target_out*": 5e-5, "target_logits*": 5e-6, "a_dz3*": 1e-4
 def test_tf32_every_intermediate_vs_rounded_restatement(plan, B, S, A, N, graph, chain, projection):
     """Every activation, logit, delta and parameter gradient of one eager DDPG.train() at precision="tf32" against the
     float64 restatement on operands rounded the way the plan's kernels round them.  Each layer is fed the device's own
-    inputs, ReLU masks and upstream deltas; bound 1e-5 x max(1, |ref|max), for the deltas (O(1/B)) 1e-5 x |ref|max."""
+    inputs, ReLU masks and upstream deltas; bound 1e-5 x max(1, |ref|max), for the deltas (O(1/B)) 1e-5 x |ref|max, for
+    the parameter gradients (~1e-6) the componentwise bound of tests/step_check.py."""
     import d4pg_b200 as d4pg
     mode, round_dw, nk = PLANS[plan]
     tc = plan == "tc_chain"
@@ -309,24 +311,15 @@ def test_tf32_every_intermediate_vs_rounded_restatement(plan, B, S, A, N, graph,
             ref, unr = ref * msk, unr * msk
         rep.check(name, dev[name], ref, scale=max(float(ref.abs().max()), 1e-30), unrounded=unr, kind="dX")
 
-    # dW from the device's deltas and activations (rounded on the level plan only); bias gradients are sums of the
-    # unrounded fp32 deltas
-    dwm = mode if round_dw else None
-    dw = lambda g, x: (rt(g, dwm).T @ rt(x, dwm)) if dwm else (g.double().T @ x.double())
+    # dW from the device's deltas and activations (rounded on the level plan only), bias gradients as sums of the
+    # unrounded fp32 deltas: against the componentwise bound of tests/step_check.py, with its power check
     ah1, ah2, ah3 = t("h1_a", H_), t("h2_a", H_), t("h3_a", H_)
-    grads = {"c": {"fc3.weight": dw(dq, ch3), "fc3.bias": dq.double().sum(0),
-                   "fc2_2.weight": dw(dev["c_dz22"], ch2), "fc2_2.bias": dev["c_dz22"].double().sum(0),
-                   "fc2.weight": dw(dev["c_dz2"], torch.cat([ch1, a], 1)), "fc2.bias": dev["c_dz2"].double().sum(0),
-                   "fc1.weight": dw(dev["c_dz1"], s), "fc1.bias": dev["c_dz1"].double().sum(0)},
-             "a": {"fc3.weight": dw(dev["a_dz3"], ah3), "fc3.bias": dev["a_dz3"].double().sum(0),
-                   "fc2_2.weight": dw(dev["a_dz22"], ah2), "fc2_2.bias": dev["a_dz22"].double().sum(0),
-                   "fc2.weight": dw(dev["a_dh2"], ah1), "fc2.bias": dev["a_dh2"].double().sum(0),
-                   "fc1.weight": dw(dev["a_dz1"], s), "fc1.bias": dev["a_dz1"].double().sum(0)}}
-    for key, net in (("c", dd.critic), ("a", dd.actor)):
-        views = net.named_grad_views()
-        for k, ref in grads[key].items():
-            rep.check("%s.%s" % (key, k), views[k].cpu().reshape(ref.shape), ref)
+    sc = SC.StepCheck(dd, W, plan, "tf32", label=rep.label)
+    sc.grads({"c": {"fc3": (dq, ch3), "fc2_2": (dev["c_dz22"], ch2), "fc2": (dev["c_dz2"], torch.cat([ch1, a], 1)),
+                    "fc1": (dev["c_dz1"], s)},
+              "a": {"fc3": (dev["a_dz3"], ah3), "fc2_2": (dev["a_dz22"], ah2), "fc2": (dev["a_dh2"], ah1), "fc1": (dev["a_dz1"], s)}})
     rep.finish()
+    sc.rep.finish()
 
     # the rounding is there, once: one forward layer and one dX layer land far outside the bound of the unrounded layer
     assert max(_seps(rep, "fwd")) > 10, ("forward", rep.sep)
