@@ -344,13 +344,15 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
   const int Sp = pitch4(S), Ap = pitch4(A), Np = pitch4(N);          // activation row pitches
   const int* la = da.ld; const int* lc = dc.ld;                        // weight row pitches per layer
   int rc; int nk = 0;
-#define LEVEL(gb) RUN(gemm_launch(gb, c.precision, st))
+  bool splitk = false;               // the level being launched accumulates split-K slices with atomics
+#define LEVEL(gb) do { splitk = gemm_batch_has_splitk(gb); RUN(gemm_launch(gb, c.precision, st)); } while (0)
 #define RUN(expr)                                                                          \
   do {                                                                                     \
     if (L->profiling) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);    \
       std::string nm0(#expr);                                                              \
-      /* the loss kernel also advances the sampler clock under the prefetch pipeline: not idempotent there */ \
-      const bool rep = nm0.rfind("gemm_launch", 0) == 0 || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0 || \
+      /* the loss kernel also advances the sampler clock under the prefetch pipeline: not idempotent there; a split-K */ \
+      /* dW level adds into the step's zeroed gradient buffer, so a repeat would multiply the gradient */                \
+      const bool rep = (nm0.rfind("gemm_launch", 0) == 0 && !splitk) || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0 || \
                                                             nm0.rfind("launch_qr_heads", 0) == 0) && !pf) || \
                        nm0.rfind("launch_mlp_chain", 0) == 0 || nm0.rfind("launch_mlp_tc_chain", 0) == 0; \
       cudaEventRecord(e0, st); rc = (expr);                                                \

@@ -129,8 +129,8 @@ class _Learner(object):
         self.losses_out = (C.c_float * 4)()
         self.fresh_host_step = False          # the most recent step was a train() (its losses are in the pinned ring)
         self._store = store
-        # parameter writes torch can see (load_state_dict, hard_update, optimizer steps: in-place ops bump the version counter
-        # the views share with the flat buffer) are reported to the library by train(); see DDPG.weights_changed
+        # parameter writes that advance a flat buffer's version counter (in-place ops on the flat buffer, load_state_dict,
+        # hard_update, SharedAdam.step) are reported to the library by train(); see DDPG.weights_changed
         self._flats = (g.actor.flat_params(), g.critic.flat_params(), ddpg.actor_target.flat_params(), ddpg.critic_target.flat_params())
         self.seen_versions = None
         self.weights_changed = L.d4pg_learner_weights_changed
@@ -287,10 +287,12 @@ class DDPG:
         model_global._bind_grads()
 
     def weights_changed(self):
-        """Report a parameter write the learner cannot see.  train() notices every in-place torch operation on actor /
-        critic / target parameters (load_state_dict, hard_update, sync_local_global, `with torch.no_grad(): p.copy_(..)`)
-        through the tensors' version counters; writes through `p.data` or raw pointers bypass those counters -- call this
-        after them (or construct with track_weights=False: the weight images are then rebuilt on every step)."""
+        """Report a parameter write the learner cannot see.  train() notices writes that advance the version counter of
+        an actor / critic / target flat buffer: in-place torch operations on `flat_params()`, load_state_dict (so
+        hard_update and sync_local_global) and SharedAdam.step.  A parameter's own version counter is not the flat
+        buffer's, so in-place writes to single parameters (`with torch.no_grad(): p.copy_(..)`, `p.data`) and writes
+        through raw pointers bypass it -- call this after them (or construct with track_weights=False: the weight images
+        are then rebuilt on every step)."""
         if self._learner is not None and self._learner.handle is not None:
             self._learner.seen_versions = None
 

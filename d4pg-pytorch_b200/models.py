@@ -151,6 +151,14 @@ class _FlatNet(nn.Module):
         self._bind()
         return self
 
+    def load_state_dict(self, state_dict, strict=True, assign=False):
+        # the copies go through the parameters, whose version counters are their own (a `.data` assignment does not
+        # share the flat buffer's), so the flat buffer's counter -- which DDPG.train() watches to re-pack the learner's
+        # weight images -- is advanced here
+        out = super().load_state_dict(state_dict, strict=strict, assign=assign)
+        torch.autograd.graph.increment_version(self._flat)
+        return out
+
     def share_memory(self):
         # CUDA storage is already visible to every stream of the process; the reference's
         # cross-process sharing (ddpg.py:96-98) is replaced by NCCL data parallelism.

@@ -65,5 +65,6 @@ class SharedAdam(torch.optim.Optimizer):
             _lib.check(_lib.lib().d4pg_adam_polyak(_lib.ptr(p), _lib.ptr(g), _lib.ptr(m), _lib.ptr(v), None,
                                                    p.numel(), lr, b1, b2, eps, self.step_count, 0.0, 1.0,
                                                    _lib.stream_ptr()), "d4pg_adam_polyak")
+            torch.autograd.graph.increment_version(p)      # written through a raw pointer: let version watchers see it
         for st in self.state.values():
             st["step"] = self.step_count

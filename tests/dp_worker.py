@@ -39,7 +39,7 @@ def main():
     dd.replayBuffer.add_batch(*shard(rank))
 
     if os.environ.get("D4PG_DP_MODE") == "device":
-        # the benchmark's configuration: device-side sampling, prefetch pipeline, 4-step graphs, gradient exchange fused
+        # the benchmark's configuration: device-side sampling, prefetch pipeline, 8-step graphs, gradient exchange fused
         # into the dW / Adam kernels.  Replicas must stay bit-identical through replays, adds and single steps.
         torch.manual_seed(0)
         dv = d4pg.DDPG(17, 6, memory_size=n, batch_size=B, critic_dist_info=info, comm=comm, precision=precision,

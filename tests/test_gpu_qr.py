@@ -388,12 +388,13 @@ def test_qr_graph_steps_with_reference_sampling_and_adds():
 
 @pytest.mark.gpu
 def test_qr_train_n_equals_single_steps():
-    """train_n(8) with device sampling (one 8-step graph, prefetch pipeline) is bit-identical to 8 single steps: the
-    quantile head kernel advances the sampler clock."""
+    """One cold step, then train_n(8) with device sampling (one 8-step graph, prefetch pipeline) is bit-identical to 9
+    single steps: the quantile head kernel advances the sampler clock."""
     import d4pg_b200 as d4pg
     res = []
     for multi in (True, False):
         dd, _ = _qr_ddpg(d4pg, 51, 256, "tf32x3", sampling="device", philox_seed=9)
+        dd.train()                      # the prefetched batch makes the next step warm: train_n(8) replays the graph
         if multi:
             dd.train_n(8)
         else:
