@@ -82,17 +82,17 @@ struct HeadsWarpSmem {
 template <int MODE, int NT>
 __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane, HeadsWarpSmem& ws, int parts = 3) {
   const int N = a.N;
-  const size_t ro = size_t(row) * a.ld;
+  const size_t ro = size_t(row) * a.h.ld;
   if (parts & 1) {
 
   // ---- target distribution ------------------------------------------------------------
   float p[NT], xt[NT], xq[NT];
   const bool t_probs = (a.flags & D4PG_PROJ_TARGET_IS_PROBS) != 0, q_probs = (a.flags & D4PG_PROJ_Q_IS_PROBS) != 0;
-  row_load(a.target_logits + ro, N, lane, xt, t_probs);
-  row_load(a.q_logits + ro, N, lane, xq, q_probs);
-  const double r = a.rewards[row];
-  const bool done = a.dones[row] != 0;
-  const float isw = a.is_weights ? __ldg(a.is_weights + row) : 1.f;
+  row_load(a.h.target + ro, N, lane, xt, t_probs);
+  row_load(a.h.q + ro, N, lane, xq, q_probs);
+  const double r = a.h.rewards[row];
+  const bool done = a.h.dones[row] != 0;
+  const float isw = a.h.is_weights ? __ldg(a.h.is_weights + row) : 1.f;
   row_softmax_x(xt, N, lane, p, t_probs);
 
   float mk[NT];
@@ -124,8 +124,8 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
       if (j < N) {
         double zj = __dadd_rn(a.v_min, __dmul_rn(double(j), a.delta));
         double c;
-        if (MODE == 0) c = __dmul_rn(zj, a.discount);                        // (v_min+j*delta)*gamma
-        else c = __dmul_rn(__dmul_rn(a.discount, done ? 0.0 : 1.0), zj);      // gamma^n*(1-d)*z_j
+        if (MODE == 0) c = __dmul_rn(zj, a.h.discount);                        // (v_min+j*delta)*gamma
+        else c = __dmul_rn(__dmul_rn(a.h.discount, done ? 0.0 : 1.0), zj);      // gamma^n*(1-d)*z_j
         double tz = fmin(a.v_max, fmax(a.v_min, __dadd_rn(r, c)));
         double b = __ddiv_rn(__dsub_rn(tz, a.v_min), a.delta);
         double lf = floor(b), uf = ceil(b);
@@ -193,7 +193,7 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
   row_softmax_x(xq, N, lane, q, q_probs);
   float ce = 0.f, mq = 0.f, sq = 0.f;
   float gq[NT];
-  const float gscale = a.grad_scale * isw;
+  const float gscale = a.h.grad_scale * isw;
 #pragma unroll
   for (int t = 0; t < NT; ++t) {
     int k = lane + 32 * t;
@@ -214,22 +214,22 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
       if (a.m) a.m[ro + k] = mk[t];
       if (a.target_probs) a.target_probs[ro + k] = p[t];
       if (a.q_probs) a.q_probs[ro + k] = q[t];
-      if (a.dlogits_q) a.dlogits_q[ro + k] = q[t] * (gq[t] - sq);   // softmax backward
+      if (a.h.dq) a.h.dq[ro + k] = q[t] * (gq[t] - sq);   // softmax backward
     }
   }
   if (lane == 0) {
     float tdv = -mq;
-    if (a.loss_rows) a.loss_rows[row] = -ce * isw;
-    if (a.td) a.td[row] = tdv;
-    if (a.prio) a.prio[row] = (a.ce_priority ? -ce : fabsf(tdv)) + float(a.prio_eps);   // np.abs(f32) + 1e-6 (f32)
+    if (a.h.loss_rows) a.h.loss_rows[row] = -ce * isw;
+    if (a.h.td) a.h.td[row] = tdv;
+    if (a.h.prio) a.h.prio[row] = (a.ce_priority ? -ce : fabsf(tdv)) + float(a.h.prio_eps);   // np.abs(f32) + 1e-6 (f32)
   }
 
   }   // parts & 1
 
   // ---- policy head: -E_q[z] and its logit gradient --------------------------------------
-  if ((parts & 2) && a.pi_logits) {
+  if ((parts & 2) && a.h.pi) {
     float qp[NT];
-    row_softmax(a.pi_logits + ro, N, lane, qp);
+    row_softmax(a.h.pi + ro, N, lane, qp);
     float ez = 0.f;
     float z[NT];
 #pragma unroll
@@ -242,9 +242,9 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
       int k = lane + 32 * t;
-      if (k < N && a.dlogits_pi) a.dlogits_pi[ro + k] = -a.grad_scale * qp[t] * (z[t] - ez);
+      if (k < N && a.h.dpi) a.h.dpi[ro + k] = -a.h.grad_scale * qp[t] * (z[t] - ez);
     }
-    if (lane == 0 && a.pi_rows) a.pi_rows[row] = -ez;
+    if (lane == 0 && a.h.pi_rows) a.h.pi_rows[row] = -ez;
   }
 }
 
@@ -252,19 +252,19 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
 template <int MODE, int NT>
 __global__ void __launch_bounds__(HEAD_WARPS * 32) heads_kernel(const HeadsArgs a) {
   __shared__ HeadsWarpSmem ws[HEAD_WARPS];
-  pdl_trigger(a.pdl);
+  pdl_trigger(a.h.pdl);
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = blockIdx.x * HEAD_WARPS + warp;            // warps [0, B): critic part of row g; [B, 2B): policy head of row g - B
-  step_stamp(a.trace, 2);
-  if (a.only_policy) { if (g < a.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 2); }
-  else if (g < a.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 1);
-  else if (g < 2 * a.B) heads_row<MODE, NT>(a, g - a.B, lane, ws[warp], 2);
-  step_stamp(a.trace, 2 + 16);
-  if (a.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
-    a.sampler_clock->s_adam_step += 1; a.sampler_clock->s_beta_t += 1; a.sampler_clock->s_steps_done += 1;
+  step_stamp(a.h.trace, 2);
+  if (a.h.only_policy) { if (g < a.h.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 2); }
+  else if (g < a.h.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 1);
+  else if (g < 2 * a.h.B) heads_row<MODE, NT>(a, g - a.h.B, lane, ws[warp], 2);
+  step_stamp(a.h.trace, 2 + 16);
+  if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
+    a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;
   }
-  pdl_trigger_end(a.pdl);
+  pdl_trigger_end(a.h.pdl);
 }
 
 }  // namespace d4pg

@@ -8,58 +8,48 @@ struct d4pg_comm;
 
 namespace d4pg {
 
-struct HeadsArgs {
-  const float* target_logits; const float* q_logits; const float* pi_logits;
+// What the three loss heads of the learner step share.  `target`, `q`, `pi` are the raw fc3 rows of critic_target(s', .),
+// critic(s, a) and critic(s, actor(s)) (logits, raw mixture heads or quantiles); every such plane has row pitch `ld`.
+struct HeadCommon {
+  const float* target; const float* q; const float* pi;
   const double* rewards; const uint8_t* dones;
-  int B, N; int flags;
-  int ld;                 // row pitch (floats) of every [B,N] array (>= N)
-  double v_min, v_max, delta, discount, prio_eps;
+  int B, ld;
+  double discount, prio_eps;
   float grad_scale;
-  float* m; int32_t* bins_l; int32_t* bins_u; float* target_probs; float* q_probs;
-  float* loss_rows; float* td; float* prio; float* dlogits_q; float* pi_rows; float* dlogits_pi;
-  // corrected-semantics switches (SURVEY.md section 8f.4; the reference does neither, H3 / H4):
-  const float* is_weights;   // non-null: critic CE row i is scaled by the PER importance weight w_i
-  int ce_priority;           // 1: priority = CE_i + eps instead of |sum_j m_ij q_ij| + eps
-  int pdl;                   // programmatic-dependent-launch trigger position (0/1/2)
+  float* loss_rows; float* td; float* prio; float* dq; float* pi_rows; float* dpi;
+  const float* is_weights;       // non-null: critic loss row i is scaled by the PER importance weight w_i (SURVEY.md section 8f.4, H3)
+  int pdl;                       // programmatic-dependent-launch trigger position (0/1/2)
   unsigned long long* trace;
-  int only_policy;               // 1: only the policy head (pi_rows, dlogits_pi) -- the second loss launch of the post-update-critic plan
+  int only_policy;               // 1: only the policy head (pi_rows, dpi) -- the second loss launch of the post-update-critic plan
   LearnerClock* sampler_clock;   // prefetch pipeline: thread 0 advances the sampler's counters (after sample(k), before sample(k+1))
+};
+
+// categorical head (proj_loss.cu): N atoms on [v_min, v_max]
+struct HeadsArgs {
+  HeadCommon h;
+  int N; int flags;
+  double v_min, v_max, delta;
+  float* m; int32_t* bins_l; int32_t* bins_u; float* target_probs; float* q_probs;
+  int ce_priority;               // 1: priority = CE_i + eps instead of |sum_j m_ij q_ij| + eps (the reference does not, H4)
 };
 int launch_heads(const HeadsArgs& a, int mode, cudaStream_t st);
 
-// mixture-of-Gaussians head (mog_heads.cu): every [B, 3K] raw plane has row pitch `ld`
+// mixture-of-Gaussians head (mog_heads.cu): K components, raw planes of 3K columns
 struct MogArgs {
-  const float* target_raw; const float* q_raw; const float* pi_raw;
-  const double* rewards; const uint8_t* dones;
-  int B, K, ld;
-  double discount, prio_eps;
-  float grad_scale;
-  float* loss_rows; float* td; float* prio; float* dq_raw; float* pi_rows; float* dpi_raw;
-  const float* is_weights;       // non-null: critic loss row i is scaled by the PER importance weight w_i
-  int pdl;
-  unsigned long long* trace;
-  int only_policy;               // as HeadsArgs::only_policy
-  LearnerClock* sampler_clock;   // as HeadsArgs::sampler_clock
+  HeadCommon h;
+  int K;
 };
 int launch_mog_heads(const MogArgs& a, cudaStream_t st);
 int launch_mog_transform(const float* raw, int ldr, int B, int K, float* w, float* mu, float* sigma, cudaStream_t st);
 int launch_mog_head_backward(const float* raw, int ldr, const float* gw, const float* gmu, const float* gsig, int B, int K,
                              float* dz, int ldz, cudaStream_t st);
 
-// quantile-regression head (qr_heads.cu): every [B, N] quantile plane has row pitch `ld`
+// quantile-regression head (qr_heads.cu): N quantiles
 struct QrArgs {
-  const float* target_q; const float* q; const float* pi_q;
-  const double* rewards; const uint8_t* dones;
-  int B, N, ld;
-  double discount, kappa, prio_eps;
-  float grad_scale;
-  float* loss_rows; float* td; float* prio; float* dq; float* pi_rows; float* dpi;
-  const float* is_weights;       // non-null: critic loss row i is scaled by the PER importance weight w_i
+  HeadCommon h;
+  int N;
+  double kappa;
   int ce_priority;               // 1: priority = L_i + eps (unweighted) instead of |td_i| + eps
-  int pdl;
-  unsigned long long* trace;
-  int only_policy;               // as HeadsArgs::only_policy
-  LearnerClock* sampler_clock;   // as HeadsArgs::sampler_clock
 };
 int launch_qr_heads(const QrArgs& a, cudaStream_t st);
 

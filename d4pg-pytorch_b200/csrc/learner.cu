@@ -3,21 +3,24 @@
 // per-step scalar (Adam bias corrections, PER beta, Philox counter) lives in device memory and
 // is advanced by a one-thread clock kernel so the captured graph never needs patching.
 //
-// Step order (reference line -> launch):
-//   ddpg.py:202  sample                       -> sample_gather_kernel (tree descent + row gather)
-//   ddpg.py:205-208 target/online forwards    -> 7 grouped-GEMM levels (actor_target, critic_target,
-//                                                critic, actor and critic(s, actor(s)) in lock-step)
-//   ddpg.py:214-222 projection, CE loss, td   -> heads_kernel (also the policy head of ddpg.py:236-238)
-//   ddpg.py:229-231 critic backward           -> grouped dX / dW levels (shared with the policy pass)
+// Step order (reference line -> phase function of enqueue_step: launch):
+//   ddpg.py:202  sample                       -> sample_batch: sample_gather_kernel (tree descent + row gather)
+//   ddpg.py:205-208 target/online forwards    -> forward_levels: 7 grouped-GEMM levels (actor_target, critic_target,
+//                                                critic, actor and critic(s, actor(s)) in lock-step);
+//                                                forward_chain / forward_tc_chain: the same layers as three cluster chains
+//   ddpg.py:214-222 projection, CE loss, td   -> launch_step_heads: heads_kernel (also the policy head of ddpg.py:236-238)
+//   ddpg.py:252-255 update_priorities         -> side_branch: tree_write_kernel<TREE_UPDATE>, beside the backward pass
+//   ddpg.py:229-231 critic backward           -> backward_levels: grouped dX / dW levels (shared with the policy pass);
+//                                                backward_chain / backward_tc_chain: two dX chains, then dw_wide
 //   ddpg.py:236-243 policy backward           -> uses the PRE-update critic weights (SURVEY.md H7):
 //                                                both backward passes run before any Adam update
-//   ddpg.py:232,244,247,250 Adam x2, sync, Polyak -> one fused adam_polyak_kernel (2 segments)
-//   ddpg.py:252-255 update_priorities         -> tree_write_kernel<TREE_UPDATE>
+//   ddpg.py:232,244,247,250 Adam x2, sync, Polyak -> exchange_gradients, then one fused adam_polyak_kernel (2 segments)
 #include "common.cuh"
 #include "gemm_ffma.cuh"
 #include "adam.cuh"
 #include <string.h>
 #include <stdlib.h>
+#include <initializer_list>
 #include <new>
 #include <string>
 #include <vector>
@@ -28,9 +31,13 @@
 
 namespace d4pg {
 
+// One half of the double-buffered batch: the rows the sample kernel gathers, the indices and IS weights it draws
+struct Batch { float *s, *a, *s2; double* r; uint8_t* done; int32_t* idx; float* wts; };
+
 struct Workspace {
-  // batch
-  float *s, *a, *s2; double* r; uint8_t* done;
+  // batch[1] exists under the prefetch / host pipelines only; without them batch[0].idx / .wts are the caller's
+  // buffers (d4pg_learner_create), with them the sampler's own
+  Batch batch[2];
   // activations: [0]=actor_target [1]=critic_target [2]=critic [3]=actor [4]=critic on policy action
   float *h1[5], *h2[5], *h3[5], *out[5];
   // heads
@@ -40,9 +47,6 @@ struct Workspace {
   LearnerClock* clock;
   float* xchg;                     // exchange planes of the cluster-fused chain kernels (chain mode)
   unsigned long long* pipe_epoch;  // host pipeline: per-CTA completion epochs of the presample kernel (polled by the forward chains)
-  // prefetch pipeline: the second half of the double-buffered batch, and the sampler's own index / weight buffers
-  float *s_b, *a_b, *s2_b; double* r_b; uint8_t* done_b;
-  int32_t* idx2[2]; float* wts2[2];
   int64_t total;
 };
 
@@ -79,9 +83,12 @@ static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, b
   int64_t off = 0;
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += align4(n); return p; };
   const int H = D4PG_HIDDEN, Sp = pitch4(S), Ap = pitch4(A), Np = pitch4(N);
-  w.s = take(int64_t(B) * Sp); w.a = take(int64_t(B) * Ap); w.s2 = take(int64_t(B) * Sp);
-  w.r = reinterpret_cast<double*>(take(int64_t(B) * 2));
-  w.done = reinterpret_cast<uint8_t*>(take((B + 3) / 4));
+  auto take_rows = [&](Batch& h) {
+    h.s = take(int64_t(B) * Sp); h.a = take(int64_t(B) * Ap); h.s2 = take(int64_t(B) * Sp);
+    h.r = reinterpret_cast<double*>(take(int64_t(B) * 2));
+    h.done = reinterpret_cast<uint8_t*>(take((B + 3) / 4));
+  };
+  take_rows(w.batch[0]);
   for (int k = 0; k < 5; ++k) {
     if (k != 4) w.h1[k] = take(int64_t(B) * H);
     w.h2[k] = take(int64_t(B) * H); w.h3[k] = take(int64_t(B) * H);
@@ -99,10 +106,8 @@ static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, b
   w.xchg = plan != PLAN_LEVELS ? take(std::max(chain_xchg_floats(B), tcc_xchg_floats(B))) : nullptr;
   w.pipe_epoch = reinterpret_cast<unsigned long long*>(take(2 * int64_t((B + SAMPLE_ROWS - 1) / SAMPLE_ROWS)));
   if (prefetch) {
-    w.s_b = take(int64_t(B) * Sp); w.a_b = take(int64_t(B) * Ap); w.s2_b = take(int64_t(B) * Sp);
-    w.r_b = reinterpret_cast<double*>(take(int64_t(B) * 2));
-    w.done_b = reinterpret_cast<uint8_t*>(take((B + 3) / 4));
-    for (int k = 0; k < 2; ++k) { w.idx2[k] = reinterpret_cast<int32_t*>(take(B)); w.wts2[k] = take(B); }
+    take_rows(w.batch[1]);
+    for (int k = 0; k < 2; ++k) { w.batch[k].idx = reinterpret_cast<int32_t*>(take(B)); w.batch[k].wts = take(B); }
   }
   w.total = off;
   return w;
@@ -119,6 +124,7 @@ struct d4pg_learner {
   StepPlan plan;
   Workspace ws;
   NetDims da, dc;
+  ClockParams clock_params;        // what the sample kernel derives the step's device-side scalars from
   cudaGraphExec_t graph_exec[4];   // [batch parity * 2 + cold]; only [0] without the prefetch pipeline
   bool graph_ready[4];
   cudaGraphExec_t multi_exec[2];   // RUN_UNROLL warm steps in one graph, by starting batch parity (d4pg_learner_run)
@@ -166,46 +172,64 @@ static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0
 static bool host_pipe(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 0 && c.use_graph != 0; }
 static bool piped(const d4pg_learner_config_t& c) { return prefetching(c) || host_pipe(c); }
 
+// ---- the layers ---------------------------------------------------------------------------------------------------
+enum Net { ACTOR, ACTOR_TARGET, CRITIC, CRITIC_TARGET };
+// Layer l (fc1, fc2, fc2_2, fc3) of a network as every plan's forward pass consumes it
+struct Layer { const float* W; int ldw; const float* bias; int n_out, k_in, epi; };
+static Layer layer(const d4pg_learner* L, Net net, int l) {
+  const bool critic = net >= CRITIC;
+  const NetDims& d = critic ? L->dc : L->da;
+  const float* P[4] = {L->buf.actor, L->buf.actor_target, L->buf.critic, L->buf.critic_target};
+  // actor (models.py:33-40): fc2 has no activation, fc3 ends in tanh; critic (models.py:77-83): fc2 contracts
+  // cat(h1, a) (k_in = H + |a|), fc3 gives the raw head
+  const int epi_actor[4] = {EPI_BIAS_RELU, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_TANH};
+  const int epi_critic[4] = {EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS};
+  return Layer{P[net] + d.w_off[l], d.ld[l], P[net] + d.b_off[l], d.out[l], d.in[l], (critic ? epi_critic : epi_actor)[l]};
+}
+// critic fc2's action columns start H floats into each row of its weight (and weight-gradient) matrix
+static int64_t critic_fc2_action_off(const d4pg_learner* L) { return L->dc.w_off[1] + D4PG_HIDDEN; }
+// The same layer as the dX pass of the online nets consumes it: dX[., n_in] = dZ[., k_out] . W.  Critic fc2 is its h1
+// columns here; its action columns are a problem of their own
+struct LayerDx { const float* W; int ldw, n_in, k_out; };
+static LayerDx layer_dx(const d4pg_learner* L, Net net, int l) {
+  const Layer y = layer(L, net, l);
+  return LayerDx{y.W, y.ldw, (net == CRITIC && l == 1) ? D4PG_HIDDEN : y.k_in, y.n_out};
+}
+static LayerDx critic_fc2_action_dx(const d4pg_learner* L) {
+  return LayerDx{L->buf.critic + critic_fc2_action_off(L), L->dc.ld[1], L->cfg.act_dim, D4PG_HIDDEN};
+}
+
 // weight matrices as the tensor-core chains consume them (F = forward image, D = transposed image for dX)
 enum { U_A_F1, U_A_F2, U_A_F22, U_A_F3, U_A_D3, U_A_D22, U_A_D2, U_AT_F1, U_AT_F2, U_AT_F22, U_AT_F3,
        U_C_F1, U_C_F2, U_C_F22, U_C_F3, U_C_D3, U_C_D22, U_C_D2H, U_C_D2A, U_CT_F1, U_CT_F2, U_CT_F22, U_CT_F3, U_COUNT };
+static int fwd_image(Net net, int l) {
+  const int fc1[4] = {U_A_F1, U_AT_F1, U_C_F1, U_CT_F1};
+  return fc1[net] + l;
+}
 
 // the weight images of the wgmma chains (PLAN_TC_CHAIN only)
 static int tcc_setup(d4pg_learner* L) {
-  const d4pg_learner_config_t& c = L->cfg;
-  const d4pg_learner_buffers_t& b = L->buf;
-  const NetDims& da = L->da; const NetDims& dc = L->dc;
-  const int S = c.obs_dim, A = c.act_dim, N = c.n_atoms, H = D4PG_HIDDEN;
   TccPackArgs& pf = L->tcc_pack_fwd; TccPackArgs& pd = L->tcc_pack_dx;
   tcc_pack_begin(pf, nullptr); tcc_pack_begin(pd, nullptr);
   int use_of[U_COUNT]; bool is_dx[U_COUNT];
-  auto add = [&](int id, const float* W, int ldw, int mode, int rows, int K) {
-    is_dx[id] = mode == GEMM_DX;
-    use_of[id] = tcc_pack_add(is_dx[id] ? pd : pf, W, ldw, mode, rows, K);
+  auto add_dx = [&](int id, const LayerDx& d) {
+    is_dx[id] = true;
+    use_of[id] = tcc_pack_add(pd, d.W, d.ldw, GEMM_DX, d.n_in, d.k_out);
   };
-  const float* Wn[2] = {b.actor, b.actor_target};
-  for (int t = 0; t < 2; ++t) {
-    const int base = t ? U_AT_F1 : U_A_F1;
-    add(base + 0, Wn[t] + da.w_off[0], da.ld[0], GEMM_FWD, H, S);
-    add(base + 1, Wn[t] + da.w_off[1], da.ld[1], GEMM_FWD, H, H);
-    add(base + 2, Wn[t] + da.w_off[2], da.ld[2], GEMM_FWD, H, H);
-    add(base + 3, Wn[t] + da.w_off[3], da.ld[3], GEMM_FWD, A, H);
-  }
-  add(U_A_D3, b.actor + da.w_off[3], da.ld[3], GEMM_DX, H, A);
-  add(U_A_D22, b.actor + da.w_off[2], da.ld[2], GEMM_DX, H, H);
-  add(U_A_D2, b.actor + da.w_off[1], da.ld[1], GEMM_DX, H, H);
-  const float* Wm[2] = {b.critic, b.critic_target};
-  for (int t = 0; t < 2; ++t) {
-    const int base = t ? U_CT_F1 : U_C_F1;
-    add(base + 0, Wm[t] + dc.w_off[0], dc.ld[0], GEMM_FWD, H, S);
-    add(base + 1, Wm[t] + dc.w_off[1], dc.ld[1], GEMM_FWD, H, H + A);      // K = [h1 (256) | action]: 8 chunks + a tail chunk
-    add(base + 2, Wm[t] + dc.w_off[2], dc.ld[2], GEMM_FWD, H, H);
-    add(base + 3, Wm[t] + dc.w_off[3], dc.ld[3], GEMM_FWD, N, H);
-  }
-  add(U_C_D3, b.critic + dc.w_off[3], dc.ld[3], GEMM_DX, H, N);
-  add(U_C_D22, b.critic + dc.w_off[2], dc.ld[2], GEMM_DX, H, H);
-  add(U_C_D2H, b.critic + dc.w_off[1], dc.ld[1], GEMM_DX, H, H);
-  add(U_C_D2A, b.critic + dc.w_off[1] + H, dc.ld[1], GEMM_DX, A, H);
+  for (int net = ACTOR; net <= CRITIC_TARGET; ++net)
+    for (int l = 0; l < 4; ++l) {                  // critic fc2: K = [h1 (256) | action]: 8 chunks + a tail chunk
+      const Layer y = layer(L, Net(net), l);
+      const int id = fwd_image(Net(net), l);
+      is_dx[id] = false;
+      use_of[id] = tcc_pack_add(pf, y.W, y.ldw, GEMM_FWD, y.n_out, y.k_in);
+    }
+  add_dx(U_A_D3, layer_dx(L, ACTOR, 3));
+  add_dx(U_A_D22, layer_dx(L, ACTOR, 2));
+  add_dx(U_A_D2, layer_dx(L, ACTOR, 1));
+  add_dx(U_C_D3, layer_dx(L, CRITIC, 3));
+  add_dx(U_C_D22, layer_dx(L, CRITIC, 2));
+  add_dx(U_C_D2H, layer_dx(L, CRITIC, 1));
+  add_dx(U_C_D2A, critic_fc2_action_dx(L));
   for (int i = 0; i < U_COUNT; ++i) D4PG_REQUIRE(use_of[i] >= 0, D4PG_ENOTSUP, "tcc_setup: too many weight images");
   const long long fwd_bytes = tcc_pack_bytes(pf), all_bytes = fwd_bytes + tcc_pack_bytes(pd);
   D4PG_CUDA_OK(cudaMalloc(&L->tcc_images, size_t(all_bytes)));
@@ -217,82 +241,354 @@ static int tcc_setup(d4pg_learner* L) {
   return D4PG_OK;
 }
 
-// ---- tensor-core chain builders (mlp_tc_chain.cu) ------------------------------------------------------------------
-struct TccCtx {
-  d4pg_learner* L; const Workspace* w; const NetDims* da; const NetDims* dc;
-  const float *Wa, *Wat, *Wc, *Wct;
-  int B, S, A, N, Sp, Ap, Np;
+// ---- one step -----------------------------------------------------------------------------------------------------
+// Exchange shapes of the data-parallel gradient (D4PG_COMM_MODE=mc|mc2|pull|rs; default: "mc" from D4PG_COMM_MC_FROM =
+// 3 ranks up when the communicator set up a multicast object, else "pull").  These defaults were chosen on another GPU
+// generation and have NOT been validated on Hopper (no multi-GPU H100 measurement exists yet; tools/ab_mc8.sh compares
+// the modes):
+//   XCHG_ALLREDUCE  no IPC-mapped peers: the communicator's all-reduce over the flat [P_a + P_c] buffer;
+//   XCHG_PULL  one hop, every rank sums all N halves inside Adam (N x 1.15 MB inbound over NVLink);
+//   XCHG_MC    in-switch reduction: ONE hop and 1.15 MB inbound per rank -- the Adam kernel's multimem.ld_reduce over an NVLS
+//              multicast object returns the sum over all ranks, added by the NVSwitch;
+//   XCHG_MC2   its two-phase form: every rank ld_reduces its 1/N slice and multimem.st's it to everyone (2 x 1.15 MB per
+//              GPU whatever N), then a second flag hop;
+//   XCHG_RS    reduce-scatter + all-gather over peer memory: TWO hops of 16-B remote accesses.
+enum Exchange { XCHG_NONE, XCHG_ALLREDUCE, XCHG_PULL, XCHG_MC, XCHG_MC2, XCHG_RS };
+static Exchange exchange_mode(d4pg_learner* L, PeerInfo* peers) {
+  if (L->cfg.world_size <= 1) return XCHG_NONE;
+  if (!comm_peer_info(L->comm, peers)) return XCHG_ALLREDUCE;
+  static const int comm_mode = [] { const char* e = getenv("D4PG_COMM_MODE");
+                                    return !e ? 0 : (e[0] == 'p' ? 1 : (e[0] == 'r' ? 2 : (e[0] == 'm' && e[1] == 'c' && e[2] == '2' ? 4 : 3))); }();
+  static const int mc_from = [] { const char* e = getenv("D4PG_COMM_MC_FROM"); return e ? atoi(e) : 3; }();
+  static const int mc2_from = [] { const char* e = getenv("D4PG_COMM_MC2_FROM"); return e ? atoi(e) : 1000; }();
+  const bool mc_avail = peers->mc != nullptr && L->plan != PLAN_LEVELS;
+  if (mc_avail && (comm_mode == 4 || (comm_mode == 0 && peers->world >= mc2_from))) return XCHG_MC2;
+  if (mc_avail && (comm_mode == 3 || (comm_mode == 0 && peers->world >= mc_from))) return XCHG_MC;
+  return comm_mode == 2 ? XCHG_RS : XCHG_PULL;
+}
+
+// What the phases of one step share
+struct Step {
+  d4pg_learner* L; cudaStream_t st;
+  const d4pg_learner_config_t& c; const d4pg_learner_buffers_t& b; const Workspace& w;
+  Batch bt;                          // the half of the double-buffered batch this step trains on
+  int par; bool cold;                // that half's index; sample it first (no valid prefetch)
+  bool pf;                           // prefetch or host pipeline
+  // corrected-semantics switch (SURVEY.md H7, loss_flags & 4): the actor gradient goes through the critic AFTER this
+  // step's critic update (the reference uses the stale local copy, ddpg.py:229-247).  Two half steps: critic forward /
+  // loss / backward / Adam, then the policy pass through the updated critic, actor backward / Adam.
+  bool h7;                           // PLAN_TC_CHAIN on one GPU (checked at create)
+  int B, S, A, N, Sp, Ap, Np;        // Sp, Ap, Np: activation row pitches
+  Exchange xm; PeerInfo peers; int gpar;   // gradient exchange: its shape, the peers, which half of the exchange buffer
+  float *Ga, *Gc;                    // where this step's gradients go
+  int nk;                            // launches so far
 };
-// T: actor_target(s') -> critic_target(s', .)   (fc1 of both networks share the resident s' chunk)     ddpg.py:205-206
-static void tcc_build_T(TccArgs& fa, int ci, const TccCtx& x) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w; const NetDims& da = *x.da; const NetDims& dc = *x.dc;
-  const int H = D4PG_HIDDEN;
-  int l, p1, p2, pa;
-  tcc_chain_x0(fa, ci, w.s2, x.Sp, x.S);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_x(fa, ci, l);
-  p1 = tcc_slot_group(fa, ci, l, U[U_AT_F1], EPI_BIAS_RELU, x.Wat + da.b_off[0], nullptr, 0, nullptr, H, 1);
-  p2 = tcc_slot_group(fa, ci, l, U[U_CT_F1], EPI_BIAS_RELU, x.Wct + dc.b_off[0], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_AT_F2], EPI_BIAS, x.Wat + da.b_off[1], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_AT_F22], EPI_BIAS_RELU, x.Wat + da.b_off[2], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  pa = tcc_slot_group(fa, ci, l, U[U_AT_F3], EPI_BIAS_TANH, x.Wat + da.b_off[3], nullptr, 0, w.out[0], x.Ap, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p2, 8); tcc_slot_src_plane(fa, ci, l, pa, 1);
-  p1 = tcc_slot_group(fa, ci, l, U[U_CT_F2], EPI_BIAS_RELU, x.Wct + dc.b_off[1], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_CT_F22], EPI_BIAS_RELU, x.Wct + dc.b_off[2], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  tcc_slot_group(fa, ci, l, U[U_CT_F3], EPI_BIAS, x.Wct + dc.b_off[3], nullptr, 0, w.out[1], x.Np, 0);
+static bool peer_exchange(const Step& x) { return x.xm >= XCHG_PULL; }
+
+// idempotent launches (pure functions of their inputs) are repeated in profile mode
+constexpr int PROFILE_REPS = 16;
+// One launch of the step, counted, under the name d4pg_learner_profile_step reports it by.  Profile mode puts a
+// CUDA-event pair around it on the step's stream and repeats it when the call site says it is repeatable.
+template <class F>
+static int run_launch(Step& x, const char* name, bool repeatable, F launch) {
+  d4pg_learner* L = x.L;
+  int rc;
+  if (L->profiling) {
+    cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
+    cudaEventRecord(e0, x.st); rc = launch();
+    for (int r = 1; repeatable && r < PROFILE_REPS && rc == 0; ++r) rc = launch();
+    cudaEventRecord(e1, x.st);
+    L->ev.push_back(e0); L->ev.push_back(e1); L->ev_reps.push_back(repeatable ? PROFILE_REPS : 1);
+    L->ev_name.push_back(name);
+  } else rc = launch();
+  if (rc == 0) ++x.nk;
+  return rc;
 }
-// the actor's four layers on s (outputs kept row-major for its backward pass); returns the plane of its action output
-static int tcc_build_actor(TccArgs& fa, int ci, const TccCtx& x, int* critic_h1_plane) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w; const NetDims& da = *x.da; const NetDims& dc = *x.dc;
-  const int H = D4PG_HIDDEN;
-  int l, p1;
-  tcc_chain_x0(fa, ci, w.s, x.Sp, x.S);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_x(fa, ci, l);
-  p1 = tcc_slot_group(fa, ci, l, U[U_A_F1], EPI_BIAS_RELU, x.Wa + da.b_off[0], nullptr, 0, w.h1[3], H, 1);
-  if (critic_h1_plane)       // critic fc1 on the same resident s chunk (h1 of critic(s, actor(s)); same values as chain Q's)
-    *critic_h1_plane = tcc_slot_group(fa, ci, l, U[U_C_F1], EPI_BIAS_RELU, x.Wc + dc.b_off[0], nullptr, 0, nullptr, H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_A_F2], EPI_BIAS, x.Wa + da.b_off[1], nullptr, 0, w.h2[3], H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_A_F22], EPI_BIAS_RELU, x.Wa + da.b_off[2], nullptr, 0, w.h3[3], H, 1);
-  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  return tcc_slot_group(fa, ci, l, U[U_A_F3], EPI_BIAS_TANH, x.Wa + da.b_off[3], nullptr, 0, w.out[3], x.Ap, 1);
+#define RUN(name, repeatable, call) \
+  do { if (int rc_ = run_launch(x, name, repeatable, [&] { return (call); })) return rc_; } while (0)
+// One dependency level of the level plan: its GEMMs as one grouped launch
+static int run_level(Step& x, std::initializer_list<GemmProblem> problems) {
+  GemmBatch g;
+  gemm_batch_begin(g);
+  for (const GemmProblem& p : problems) gemm_batch_add(g, p);
+  // a split-K dW level adds into the step's zeroed gradient buffer, so a repeat would multiply the gradient
+  RUN("gemm_launch", !gemm_batch_has_splitk(g), gemm_launch(g, x.c.precision, x.st));
+  return D4PG_OK;
 }
-// P: actor(s) -> critic(s, actor(s))                                                                     ddpg.py:236-238
-static void tcc_build_P(TccArgs& fa, int ci, const TccCtx& x) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w; const NetDims& dc = *x.dc;
+
+// 1. sample + gather (ddpg.py:187-197).  The same kernel derives this step's device-side
+//    scalars (Adam bias corrections, PER beta, Philox counter) from the learner clock.
+static int sample_batch(Step& x) {
+  const d4pg_learner_config_t& c = x.c;
+  RUN("learner_sample", false,
+      learner_sample(x.L->replay, x.B, c.prioritized, c.sample_mode == 0 ? x.b.uniforms : nullptr,
+                     (c.sample_mode == 0 && !c.prioritized) ? x.b.positions : nullptr,
+                     c.philox_seed, x.w.clock, x.L->clock_params,
+                     x.bt.idx, x.bt.wts, x.bt.s, x.bt.a, x.bt.r, x.bt.s2, x.bt.done, x.Sp, x.Ap, x.pf ? x.par : -1, x.st));
+  return D4PG_OK;
+}
+
+// ---- forward, PLAN_TC_CHAIN (mlp_tc_chain.cu): clusters of 8 CTAs own 64 rows, every layer a wgmma tile ---------------
+static void tcc_begin(const Step& x, TccArgs& a, int step_slot) {
+  tcc_args_begin(a, x.B, reinterpret_cast<uint8_t*>(x.w.xchg), x.c.precision == 1 ? 3 : 1);
+  a.step_slot = step_slot;
+}
+// output group of layer l of `net` in slot `sl` of chain `ci`
+static int tcc_fwd_group(TccArgs& fa, int ci, int sl, const Step& x, Net net, int l, float* C, int ldc, int publish) {
+  const Layer y = layer(x.L, net, l);
+  return tcc_slot_group(fa, ci, sl, x.L->tcc_img[fwd_image(net, l)], y.epi, y.bias, nullptr, 0, C, ldc, publish);
+}
+// Actor `an` on `s`, then critic `cn` on (s, that action); fc1 of both networks share the resident chunk of s:
+//   T: actor_target(s') -> critic_target(s', .)                                                          ddpg.py:205-206
+//   P: actor(s) -> critic(s, actor(s))                                                                   ddpg.py:236-238
+// keep: the hidden activations are also stored row-major (sets ka / kc), for the backward pass of the online nets.
+// actor_only: the post-update plan's chain 1; its critic pass follows the critic's Adam
+static void tcc_build_actor_critic(TccArgs& fa, int ci, const Step& x, Net an, Net cn, const float* s, int ka, int kc,
+                                   bool keep, bool actor_only = false) {
+  const Workspace& w = x.w;
   const int H = D4PG_HIDDEN;
   int l, p1, p2 = -1;
-  const int pa = tcc_build_actor(fa, ci, x, &p2);
+  tcc_chain_x0(fa, ci, s, x.Sp, x.S);
+  l = tcc_slot_begin(fa, ci); tcc_slot_src_x(fa, ci, l);
+  p1 = tcc_fwd_group(fa, ci, l, x, an, 0, keep ? w.h1[ka] : nullptr, H, 1);
+  if (!actor_only) p2 = tcc_fwd_group(fa, ci, l, x, cn, 0, nullptr, H, 1);   // (P: same values as chain Q's h1)
+  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
+  p1 = tcc_fwd_group(fa, ci, l, x, an, 1, keep ? w.h2[ka] : nullptr, H, 1);
+  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
+  p1 = tcc_fwd_group(fa, ci, l, x, an, 2, keep ? w.h3[ka] : nullptr, H, 1);
+  l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
+  const int pa = tcc_fwd_group(fa, ci, l, x, an, 3, w.out[ka], x.Ap, 1);
+  if (actor_only) return;
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p2, 8); tcc_slot_src_plane(fa, ci, l, pa, 1);
-  p1 = tcc_slot_group(fa, ci, l, U[U_C_F2], EPI_BIAS_RELU, x.Wc + dc.b_off[1], nullptr, 0, w.h2[4], H, 1);
+  p1 = tcc_fwd_group(fa, ci, l, x, cn, 1, keep ? w.h2[kc] : nullptr, H, 1);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_C_F22], EPI_BIAS_RELU, x.Wc + dc.b_off[2], nullptr, 0, w.h3[4], H, 1);
+  p1 = tcc_fwd_group(fa, ci, l, x, cn, 2, keep ? w.h3[kc] : nullptr, H, 1);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  tcc_slot_group(fa, ci, l, U[U_C_F3], EPI_BIAS, x.Wc + dc.b_off[3], nullptr, 0, w.out[4], x.Np, 0);
+  tcc_fwd_group(fa, ci, l, x, cn, 3, w.out[kc], x.Np, 0);
 }
 // critic(s, `act`): the resident chunk holds s for fc1, then the action rows (fc2's K tail)                ddpg.py:208
-static void tcc_build_Q(TccArgs& fa, int ci, const TccCtx& x, const float* act, float* h1, float* h2, float* h3, float* logits) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w; const NetDims& dc = *x.dc;
+static void tcc_build_Q(TccArgs& fa, int ci, const Step& x, const float* act, float* h1, float* h2, float* h3, float* logits) {
   const int H = D4PG_HIDDEN;
   int l, p1;
-  tcc_chain_x0(fa, ci, w.s, x.Sp, x.S);
+  tcc_chain_x0(fa, ci, x.bt.s, x.Sp, x.S);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_x(fa, ci, l); tcc_slot_reconvert_x(fa, ci, l, act, x.Ap, x.A);
-  p1 = tcc_slot_group(fa, ci, l, U[U_C_F1], EPI_BIAS_RELU, x.Wc + dc.b_off[0], nullptr, 0, h1, H, 1);
+  p1 = tcc_fwd_group(fa, ci, l, x, CRITIC, 0, h1, H, 1);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8); tcc_slot_src_x(fa, ci, l);
-  p1 = tcc_slot_group(fa, ci, l, U[U_C_F2], EPI_BIAS_RELU, x.Wc + dc.b_off[1], nullptr, 0, h2, H, 1);
+  p1 = tcc_fwd_group(fa, ci, l, x, CRITIC, 1, h2, H, 1);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  p1 = tcc_slot_group(fa, ci, l, U[U_C_F22], EPI_BIAS_RELU, x.Wc + dc.b_off[2], nullptr, 0, h3, H, 1);
+  p1 = tcc_fwd_group(fa, ci, l, x, CRITIC, 2, h3, H, 1);
   l = tcc_slot_begin(fa, ci); tcc_slot_src_plane(fa, ci, l, p1, 8);
-  tcc_slot_group(fa, ci, l, U[U_C_F3], EPI_BIAS, x.Wc + dc.b_off[3], nullptr, 0, logits, x.Np, 0);
+  tcc_fwd_group(fa, ci, l, x, CRITIC, 3, logits, x.Np, 0);
 }
+// 2''. the three forward chains on the tensor cores.  pack_fwd: re-pack the hi/lo forward weight images first (the
+// caller may have changed the parameters; otherwise the previous step's Adam kernel kept them current)
+static int forward_tc_chain(Step& x, bool pack_fwd) {
+  d4pg_learner* L = x.L; const Workspace& w = x.w;
+  if (pack_fwd) RUN("launch_tcc_pack", false, launch_tcc_pack(L->tcc_pack_fwd, x.st));
+  // the transposed images of the dX chains are needed only after the forward chains and heads: packed on the side branch
+  D4PG_CUDA_OK(cudaEventRecord(L->ev_fork2, x.st));
+  D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork2, 0));
+  RUN("launch_tcc_pack", false, launch_tcc_pack(L->tcc_pack_dx, L->side));
+  D4PG_CUDA_OK(cudaEventRecord(L->ev_join2, L->side));
+  TccArgs& fa = L->tcc_fwd_args;
+  tcc_begin(x, fa, 1);
+  tcc_build_actor_critic(fa, 0, x, ACTOR_TARGET, CRITIC_TARGET, x.bt.s2, 0, 1, false);   // chain 0  T
+  tcc_build_actor_critic(fa, 1, x, ACTOR, CRITIC, x.bt.s, 3, 4, true, x.h7);             // chain 1  P (post-update plan: the actor alone)
+  tcc_build_Q(fa, 2, x, x.bt.a, w.h1[2], w.h2[2], w.h3[2], w.out[2]);   // chain 2  Q: critic(s, a)
+  if (host_pipe(x.c) && !x.cold) {
+    // warm host-pipeline variant: the batch comes from the ingest stream's sample kernel; instead of a stream event
+    // (event + graph start after the sample ends) every CTA polls the epochs that kernel publishes
+    fa.wait_epoch = w.pipe_epoch; fa.wait_clock = reinterpret_cast<const long long*>(&w.clock->steps_done);
+    fa.wait_n = cdiv(x.B, SAMPLE_ROWS);
+  }
+  RUN("launch_mlp_tc_chain", true, launch_mlp_tc_chain(fa, x.st));
+  return D4PG_OK;
+}
+
+// ---- forward, PLAN_CHAIN (mlp_chain.cu) -----------------------------------------------------------------------------
+static ChainSlot chain_layer(const Step& x, Net net, int l, float* C, int ldc, int publish) {
+  const Layer y = layer(x.L, net, l);
+  return chain_fwd(y.W, y.ldw, y.bias, y.n_out, y.k_in, y.epi, C, ldc, publish);
+}
+// pre-layers (a narrow layer computed inside the slot that consumes it): fp32 tile, |a| <= 8
+static bool chain_pre_ok(const Step& x) { return x.c.precision == 0 && x.A <= 8; }
+// actor `an` on `s`, then critic `cn` on (s, that action), as chain `ci`: T (the targets on s') and P (the online nets on
+// s).  ka / kc: the activation sets they write; c_h1: where the critic's h1 goes (nullptr: exchange only)
+static void chain_build_actor_critic(const Step& x, ChainArgs& ca, int ci, Net an, Net cn, const float* s, int ka,
+                                     float* c_h1, int kc) {
+  const Workspace& w = x.w;
+  const int H = D4PG_HIDDEN;
+  ChainSlot sl; int t, a3 = -1;
+  sl = chain_layer(x, an, 0, w.h1[ka], H, 1); chain_src_global(sl, s, x.Sp); t = chain_add(ca, ci, sl);
+  sl = chain_layer(x, an, 1, w.h2[ka], H, 1); chain_src_plane(sl, t); t = chain_add(ca, ci, sl);
+  sl = chain_layer(x, an, 2, w.h3[ka], H, 1); chain_src_plane(sl, t); const int a22 = chain_add(ca, ci, sl);
+  // the 6-wide actor fc3 is a PRE-LAYER of the critic's fc2 slot (every CTA computes it for its 32 rows) instead of
+  // a slot of its own, when it fits; otherwise it is a slot that publishes 8 plane rows
+  if (!chain_pre_ok(x)) { sl = chain_layer(x, an, 3, w.out[ka], x.Ap, 1); chain_src_plane(sl, a22); a3 = chain_add(ca, ci, sl); }
+  sl = chain_layer(x, cn, 0, c_h1, H, 1); chain_src_global(sl, s, x.Sp); t = chain_add(ca, ci, sl);
+  sl = chain_layer(x, cn, 1, w.h2[kc], H, 1); chain_src_plane(sl, t);
+  if (chain_pre_ok(x)) {
+    const Layer y = layer(x.L, an, 3);
+    chain_pre_layer(sl, y.W, y.ldw, y.bias, nullptr, 0, y.n_out, y.k_in, y.epi, w.out[ka], x.Ap, a22, H, false);
+  } else chain_src2_plane(sl, H, a3);
+  t = chain_add(ca, ci, sl);
+  sl = chain_layer(x, cn, 2, w.h3[kc], H, 1); chain_src_plane(sl, t); t = chain_add(ca, ci, sl);
+  sl = chain_layer(x, cn, 3, w.out[kc], x.Np, 0); chain_src_plane(sl, t); chain_add(ca, ci, sl);
+}
+// 2'. the three forward chains of the step as ONE cluster launch:
+//   chain 0  T: actor_target(s') -> critic_target(s', .)      ddpg.py:205-206
+//   chain 1  P: actor(s) -> critic(s, actor(s))                ddpg.py:236-238 (fc1 of the critic is recomputed: K=|s|)
+//   chain 2  Q: critic(s, a)                                   ddpg.py:208
+// The block scheduler fills SMs in launch order: the two 8-layer chains come first so that each of their CTAs
+// gets an SM of its own, and the short 4-layer chain is the one that doubles up
+static int forward_chain(Step& x) {
+  const Workspace& w = x.w;
+  const int H = D4PG_HIDDEN;
+  ChainArgs& ca = x.L->chain_fwd_args;
+  chain_args_begin(ca, x.B, w.xchg, x.c.precision);
+  chain_build_actor_critic(x, ca, 0, ACTOR_TARGET, CRITIC_TARGET, x.bt.s2, 0, w.h1[1], 1);
+  ChainSlot sl; int t;
+  sl = chain_layer(x, CRITIC, 0, w.h1[2], H, 1); chain_src_global(sl, x.bt.s, x.Sp); t = chain_add(ca, 2, sl);
+  sl = chain_layer(x, CRITIC, 1, w.h2[2], H, 1); chain_src_plane(sl, t); chain_src2_global(sl, H, x.bt.a, x.Ap); t = chain_add(ca, 2, sl);
+  sl = chain_layer(x, CRITIC, 2, w.h3[2], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 2, sl);
+  sl = chain_layer(x, CRITIC, 3, w.out[2], x.Np, 0); chain_src_plane(sl, t); chain_add(ca, 2, sl);
+  chain_build_actor_critic(x, ca, 1, ACTOR, CRITIC, x.bt.s, 3, nullptr, 4);
+  RUN("launch_mlp_chain", true, launch_mlp_chain(ca, x.st));
+  return D4PG_OK;
+}
+
+// ---- forward, PLAN_LEVELS: one grouped launch per dependency level ----------------------------------------------------
+static GemmProblem level_fwd(const Step& x, Net net, int l, const float* X, int ldx, float* Y, int ldy,
+                             const float* act = nullptr) {     // act: the action rows critic fc2 concatenates to X
+  const Layer y = layer(x.L, net, l);
+  return gemm_fwd(X, ldx, act, act ? x.Ap : 0, act ? D4PG_HIDDEN : 0, y.W, y.ldw, y.bias, Y, ldy, x.B, y.n_out, y.k_in, y.epi);
+}
+static int forward_levels(Step& x) {
+  const Workspace& w = x.w; const Batch& bt = x.bt;
+  const int H = D4PG_HIDDEN, Sp = x.Sp, Ap = x.Ap, Np = x.Np;
+  // 2. forward level 1: fc1 of actor_target(s'), critic_target(s'), critic(s), actor(s)
+  int rc = run_level(x, {level_fwd(x, ACTOR_TARGET, 0, bt.s2, Sp, w.h1[0], H),
+                         level_fwd(x, CRITIC_TARGET, 0, bt.s2, Sp, w.h1[1], H),
+                         level_fwd(x, CRITIC, 0, bt.s, Sp, w.h1[2], H),
+                         level_fwd(x, ACTOR, 0, bt.s, Sp, w.h1[3], H)});
+  // level 2: fc2 (actor: no activation, models.py:36; critic: cat(h1, a) + relu, models.py:80)
+  if (!rc) rc = run_level(x, {level_fwd(x, ACTOR_TARGET, 1, w.h1[0], H, w.h2[0], H),
+                              level_fwd(x, CRITIC, 1, w.h1[2], H, w.h2[2], H, bt.a),
+                              level_fwd(x, ACTOR, 1, w.h1[3], H, w.h2[3], H)});
+  // level 3: fc2_2 + relu
+  if (!rc) rc = run_level(x, {level_fwd(x, ACTOR_TARGET, 2, w.h2[0], H, w.h3[0], H),
+                              level_fwd(x, CRITIC, 2, w.h2[2], H, w.h3[2], H),
+                              level_fwd(x, ACTOR, 2, w.h2[3], H, w.h3[3], H)});
+  // level 4: fc3 (actor: tanh; critic: logits)
+  if (!rc) rc = run_level(x, {level_fwd(x, ACTOR_TARGET, 3, w.h3[0], H, w.out[0], Ap),
+                              level_fwd(x, CRITIC, 3, w.h3[2], H, w.out[2], Np),
+                              level_fwd(x, ACTOR, 3, w.h3[3], H, w.out[3], Ap)});
+  // level 5: critic_target.fc2([h1t, a_t(s')]) and critic.fc2([h1, actor(s)]) (h1 of the critic is reused)
+  if (!rc) rc = run_level(x, {level_fwd(x, CRITIC_TARGET, 1, w.h1[1], H, w.h2[1], H, w.out[0]),
+                              level_fwd(x, CRITIC, 1, w.h1[2], H, w.h2[4], H, w.out[3])});
+  if (!rc) rc = run_level(x, {level_fwd(x, CRITIC_TARGET, 2, w.h2[1], H, w.h3[1], H),
+                              level_fwd(x, CRITIC, 2, w.h2[4], H, w.h3[4], H)});
+  if (!rc) rc = run_level(x, {level_fwd(x, CRITIC_TARGET, 3, w.h3[1], H, w.out[1], Np),
+                              level_fwd(x, CRITIC, 3, w.h3[4], H, w.out[4], Np)});
+  return rc;
+}
+
+// 3. heads: softmaxes, projection, CE loss, td, priorities, logit gradients (ddpg.py:214-222,236-238); the mixture
+//    critic's quadrature cross-entropy (mog_heads.cu) or the quantile critic's quantile-Huber loss (qr_heads.cu) in their
+//    place.  only_policy: the second loss launch of the post-update plan, the policy head on the updated critic's output
+static HeadCommon head_common(const Step& x, bool only_policy) {
+  const d4pg_learner_config_t& c = x.c; const Workspace& w = x.w;
+  HeadCommon h{};
+  h.target = w.out[1]; h.q = w.out[2]; h.pi = (x.h7 && !only_policy) ? nullptr : w.out[4];
+  h.rewards = x.bt.r; h.dones = x.bt.done; h.B = x.B; h.ld = x.Np;
+  // live projection discounts with gamma even for n_steps>1 (SURVEY.md H5); mode 1 uses gamma**n (ddpg.py:24)
+  h.discount = (c.proj_mode == 1) ? pow(c.gamma, double(c.n_steps)) : c.gamma; h.prio_eps = c.prio_eps;
+  h.grad_scale = 1.0f / (float(x.B) * float(c.world_size > 1 ? c.world_size : 1));
+  h.loss_rows = w.loss_rows; h.td = x.b.td; h.prio = x.b.prio; h.dq = w.dlogits_q;
+  h.pi_rows = w.pi_rows; h.dpi = w.dlogits_pi;
+  h.is_weights = ((c.loss_flags & 1) && c.prioritized) ? x.bt.wts : nullptr;
+  h.only_policy = only_policy ? 1 : 0;
+  h.sampler_clock = (x.pf && !only_policy) ? w.clock : nullptr;    // sample(t) is done, sample(t+1) not yet launched
+  return h;
+}
+static int launch_step_heads(Step& x, bool only_policy) {
+  const d4pg_learner_config_t& c = x.c; const Workspace& w = x.w;
+  const HeadCommon h = head_common(x, only_policy);
+  const int ce_priority = (c.loss_flags & 2) ? 1 : 0;
+  // the loss kernel also advances the sampler clock under the pipelines: not idempotent there
+  const bool rep = !x.pf;
+  if (c.dist_type == 1) {
+    MogArgs ma{h, c.n_components};
+    RUN("launch_mog_heads", rep, launch_mog_heads(ma, x.st));
+  } else if (c.dist_type == 2) {
+    QrArgs qa{h, x.N, c.qr_kappa, ce_priority};
+    RUN("launch_qr_heads", rep, launch_qr_heads(qa, x.st));
+  } else {
+    HeadsArgs ha{};
+    ha.h = h; ha.N = x.N; ha.ce_priority = ce_priority;
+    ha.v_min = c.v_min; ha.v_max = c.v_max; ha.delta = (c.v_max - c.v_min) / double(x.N - 1);
+    ha.m = w.m; ha.target_probs = w.target_probs; ha.q_probs = w.q_probs;
+    RUN("launch_heads", rep, launch_heads(ha, c.proj_mode, x.st));
+  }
+  return D4PG_OK;
+}
+
+// 4. priorities into the trees (ddpg.py:252-255): independent of the backward pass, so it runs
+//    on a forked branch (side stream -> parallel graph branch) and joins before the step ends
+static int side_branch(Step& x) {
+  d4pg_learner* L = x.L; const d4pg_learner_config_t& c = x.c;
+  D4PG_CUDA_OK(cudaEventRecord(L->ev_fork, x.st));
+  D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork, 0));
+  // host pipeline: the write-back also opens the ingest gate of step k+1 (its tree add / presample wait for this step's
+  // loss kernel -- which advanced the sampler clock -- and for the priorities)
+  if (c.prioritized)
+    RUN("launch_tree_update", false,
+        launch_tree_update(L->replay, x.B, x.bt.idx, x.b.prio, L->side, host_pipe(c) ? L->gate_flag : nullptr));
+  else if (host_pipe(c)) RUN("launch_gate_signal", false, launch_gate_signal(L->gate_flag, L->side));
+  if (prefetching(c)) {
+    // 4'. the NEXT step's batch, sampled from the just-updated trees into the other half of the batch buffers
+    // while this step's backward pass, dW and Adam run (it needs the trees, not the weights)
+    const int q = x.par ^ 1;
+    const Batch& o = x.w.batch[q];
+    RUN("learner_sample", false,
+        learner_sample(L->replay, x.B, c.prioritized, nullptr, nullptr, c.philox_seed, x.w.clock, L->clock_params,
+                       o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, x.Sp, x.Ap, q, L->side));
+  }
+  if (x.pf) {                           // the caller-visible copies of this step's indices / IS weights (off the
+    // path to the next batch: after the write-back and the prefetch)
+    D4PG_CUDA_OK(cudaMemcpyAsync(x.b.idx, x.bt.idx, size_t(x.B) * sizeof(int32_t), cudaMemcpyDeviceToDevice, L->side));
+    if (x.b.weights && c.prioritized)
+      D4PG_CUDA_OK(cudaMemcpyAsync(x.b.weights, x.bt.wts, size_t(x.B) * sizeof(float), cudaMemcpyDeviceToDevice, L->side));
+  }
+  D4PG_CUDA_OK(cudaEventRecord(L->ev_join, L->side));
+  return D4PG_OK;
+}
+
+// Where this step's gradients go, and how the ranks will exchange them
+static int choose_gradient_buffers(Step& x) {
+  const d4pg_learner_buffers_t& b = x.b;
+  x.Ga = b.grad_actor; x.Gc = b.grad_critic;
+  x.peers = PeerInfo{};
+  x.xm = exchange_mode(x.L, &x.peers);
+  x.gpar = x.pf ? x.par : int(x.L->steps_done & 1);
+  // data parallel with IPC-mapped peers: this step's gradients go straight into this rank's half of the exchange
+  // buffer (double-buffered by step parity), the Adam kernel sums all ranks' halves over NVLink: the multicast-bound
+  // buffer when the in-switch reduction is set up, else the IPC-mapped one the peers read directly
+  if (peer_exchange(x)) {
+    const bool use_mc_buf = x.xm == XCHG_MC || x.xm == XCHG_MC2;
+    x.Ga = (use_mc_buf ? x.peers.mc_uc : x.peers.x[x.peers.rank]) + int64_t(x.gpar) * x.peers.n;
+    x.Gc = x.Ga + x.L->da.total;
+  }
+  if (x.B >= 1024)                // dW levels run split-K with fp32 atomics: the gradient buffer must start at zero
+    D4PG_CUDA_OK(cudaMemsetAsync(x.Ga, 0, size_t(x.L->da.total + x.L->dc.total) * sizeof(float), x.st));
+  return D4PG_OK;
+}
+
+// ---- backward -----------------------------------------------------------------------------------------------------
+// "c_" = critic-loss pass, "p_" = policy pass through the critic, "a_" = actor.
 // C: critic loss, dlogits_q -> fc3 -> fc2_2 -> fc2[:, :H]                                                  ddpg.py:230
-static void tcc_build_bwd_C(TccArgs& ba, int ci, const TccCtx& x) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w;
+static void tcc_build_bwd_C(TccArgs& ba, int ci, const Step& x) {
+  const TccImage* U = x.L->tcc_img; const Workspace& w = x.w;
   const int H = D4PG_HIDDEN;
   int l, p1;
   tcc_chain_pre(ba, ci, w.dlogits_q, x.Np, x.N);
@@ -304,8 +600,8 @@ static void tcc_build_bwd_C(TccArgs& ba, int ci, const TccCtx& x) {
   tcc_slot_group(ba, ci, l, U[U_C_D2H], EPI_RELU_MASK, nullptr, w.h1[2], H, w.c_dz1, H, 0);
 }
 // P: policy loss, dlogits_pi -> critic fc3 -> fc2_2 -> fc2[:, H:] (d action, tanh') -> actor fc3 -> fc2_2 -> fc2   ddpg.py:242
-static void tcc_build_bwd_P(TccArgs& ba, int ci, const TccCtx& x) {
-  const TccImage* U = x.L->tcc_img; const Workspace& w = *x.w;
+static void tcc_build_bwd_P(TccArgs& ba, int ci, const Step& x) {
+  const TccImage* U = x.L->tcc_img; const Workspace& w = x.w;
   const int H = D4PG_HIDDEN;
   int l, p1;
   tcc_chain_pre(ba, ci, w.dlogits_pi, x.Np, x.N);
@@ -322,467 +618,250 @@ static void tcc_build_bwd_P(TccArgs& ba, int ci, const TccCtx& x) {
   l = tcc_slot_begin(ba, ci); tcc_slot_src_plane(ba, ci, l, p1, 8);
   tcc_slot_group(ba, ci, l, U[U_A_D2], EPI_RELU_MASK, nullptr, w.h1[3], H, w.a_dz1, H, 0);
 }
+// 5''. both dX chains on the tensor cores (transposed weight images; masks applied by the epilogue)
+static int backward_tc_chain(Step& x) {
+  D4PG_CUDA_OK(cudaStreamWaitEvent(x.st, x.L->ev_join2, 0));     // transposed weight images are packed
+  TccArgs& ba = x.L->tcc_bwd_args;
+  tcc_begin(x, ba, 5);
+  tcc_build_bwd_C(ba, 0, x);                                   // C: critic loss
+  if (!x.h7) tcc_build_bwd_P(ba, 1, x);                        // P: policy loss (PRE-update critic weights, SURVEY.md H7)
+  RUN("launch_mlp_tc_chain", true, launch_mlp_tc_chain(ba, x.st));
+  return D4PG_OK;
+}
 
-// idempotent launches (pure functions of their inputs) are repeated in profile mode
-constexpr int PROFILE_REPS = 16;
+static ChainSlot chain_layer_dx(const LayerDx& d, int epi, const float* aux, int ldaux, float* C, int ldc, int publish) {
+  return chain_dx(d.W, d.ldw, d.n_in, d.k_out, epi, aux, ldaux, C, ldc, publish);
+}
+// 5'. both dX chains as ONE cluster launch
+//   C: critic loss  dlogits_q  -> fc3 -> fc2_2 -> fc2[:, :H]                         ddpg.py:230
+//   P: policy loss  dlogits_pi -> fc3 -> fc2_2 -> fc2[:, H:] (d action, tanh') ->
+//                   actor fc3 -> fc2_2 -> fc2   (PRE-update critic weights, SURVEY.md H7)  ddpg.py:242
+static int backward_chain(Step& x) {
+  d4pg_learner* L = x.L; const Workspace& w = x.w;
+  const int H = D4PG_HIDDEN, Ap = x.Ap, Np = x.Np;
+  ChainArgs& cb = L->chain_bwd_args;
+  chain_args_begin(cb, x.B, w.xchg, x.c.precision); cb.trace_base = 6 * CHAIN_MAX_SLOTS;
+  ChainSlot sl; int t;
+  sl = chain_layer_dx(layer_dx(L, CRITIC, 3), EPI_RELU_MASK, w.h3[2], H, w.c_dz22, H, 1); chain_src_global(sl, w.dlogits_q, Np); t = chain_add(cb, 0, sl);
+  sl = chain_layer_dx(layer_dx(L, CRITIC, 2), EPI_RELU_MASK, w.h2[2], H, w.c_dz2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 0, sl);
+  sl = chain_layer_dx(layer_dx(L, CRITIC, 1), EPI_RELU_MASK, w.h1[2], H, w.c_dz1, H, 0); chain_src_plane(sl, t); chain_add(cb, 0, sl);
 
-// par: half of the double-buffered batch this step trains on; cold: sample it first (no valid prefetch)
-// pack_fwd: re-pack the forward weight images first (start of a graph launch / eager step: the caller may have changed
-// the parameters); later steps of one multi-step graph rely on the images the previous step's Adam kernel wrote
-static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bool pack_fwd = true) {
-  const d4pg_learner_config_t& c = L->cfg;
-  const d4pg_learner_buffers_t& b = L->buf;
-  Workspace w = L->ws;                               // local copy: the batch pointers follow `par`
-  const bool pf = piped(c);
-  int32_t* bidx = b.idx; float* bwts = b.weights;
-  if (pf) {
-    if (par) { w.s = w.s_b; w.a = w.a_b; w.s2 = w.s2_b; w.r = w.r_b; w.done = w.done_b; }
-    bidx = w.idx2[par]; bwts = w.wts2[par];
-  }
-  const NetDims& da = L->da; const NetDims& dc = L->dc;
-  const int B = c.batch, S = c.obs_dim, A = c.act_dim, N = c.n_atoms, H = D4PG_HIDDEN;
-  const int Sp = pitch4(S), Ap = pitch4(A), Np = pitch4(N);          // activation row pitches
-  const int* la = da.ld; const int* lc = dc.ld;                        // weight row pitches per layer
-  int rc; int nk = 0;
-  bool splitk = false;               // the level being launched accumulates split-K slices with atomics
-#define LEVEL(gb) do { splitk = gemm_batch_has_splitk(gb); RUN(gemm_launch(gb, c.precision, st)); } while (0)
-#define RUN(expr)                                                                          \
-  do {                                                                                     \
-    if (L->profiling) { cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);    \
-      std::string nm0(#expr);                                                              \
-      /* the loss kernel also advances the sampler clock under the prefetch pipeline: not idempotent there; a split-K */ \
-      /* dW level adds into the step's zeroed gradient buffer, so a repeat would multiply the gradient */                \
-      const bool rep = (nm0.rfind("gemm_launch", 0) == 0 && !splitk) || ((nm0.rfind("launch_heads", 0) == 0 || nm0.rfind("launch_mog_heads", 0) == 0 || \
-                                                            nm0.rfind("launch_qr_heads", 0) == 0) && !pf) || \
-                       nm0.rfind("launch_mlp_chain", 0) == 0 || nm0.rfind("launch_mlp_tc_chain", 0) == 0; \
-      cudaEventRecord(e0, st); rc = (expr);                                                \
-      for (int _r = 1; rep && _r < PROFILE_REPS && rc == 0; ++_r) rc = (expr);             \
-      cudaEventRecord(e1, st);                                                             \
-      L->ev.push_back(e0); L->ev.push_back(e1); L->ev_reps.push_back(rep ? PROFILE_REPS : 1); \
-      std::string nm(#expr); L->ev_name.push_back(nm.substr(0, nm.find('('))); }           \
-    else rc = (expr);                                                                      \
-    if (rc) return rc;                                                                     \
-    ++nk;                                                                                  \
-  } while (0)
-
-  // 1. sample + gather (ddpg.py:187-197).  The same kernel derives this step's device-side
-  //    scalars (Adam bias corrections, PER beta, Philox counter) from the learner clock.
-  ClockParams cp{c.lr_actor, c.lr_critic, c.beta1, c.beta2, c.per_beta0, c.per_beta_final,
-                 c.per_beta_iters > 0 ? c.per_beta_iters : 1};
-  if (!pf || cold)
-    RUN(learner_sample(L->replay, B, c.prioritized, c.sample_mode == 0 ? b.uniforms : nullptr,
-                       (c.sample_mode == 0 && !c.prioritized) ? b.positions : nullptr,
-                       c.philox_seed, w.clock, cp,
-                       bidx, bwts, w.s, w.a, w.r, w.s2, w.done, Sp, Ap, pf ? par : -1, st));
-
-  const float* Wa = b.actor; const float* Wat = b.actor_target; const float* Wc = b.critic; const float* Wct = b.critic_target;
-  GemmBatch g;
-  const StepPlan plan = L->plan;
-  // corrected-semantics switch (SURVEY.md H7, loss_flags & 4): the actor gradient goes through the critic AFTER this
-  // step's critic update (the reference uses the stale local copy, ddpg.py:229-247).  Two half steps: critic forward /
-  // loss / backward / Adam, then the policy pass through the updated critic, actor backward / Adam.
-  const bool h7 = (c.loss_flags & 4) != 0;                            // PLAN_TC_CHAIN on one GPU (checked at create)
-  const bool pre_ok = plan == PLAN_CHAIN && c.precision == 0 && A <= 8;   // pre-layers: fp32 tile, |a| <= 8
-  if (plan == PLAN_TC_CHAIN) {
-    // 2''. the same three forward chains on the tensor cores (mlp_tc_chain.cu): clusters of 8 CTAs own 64 rows,
-    // every layer a wgmma tile.  The hi/lo weight images are re-packed first (Adam / Polyak changed them).
-    if (pack_fwd) RUN(launch_tcc_pack(L->tcc_pack_fwd, st));
-    // the transposed images of the dX chains are needed only after the forward chains and heads: packed on the side branch
-    D4PG_CUDA_OK(cudaEventRecord(L->ev_fork2, st));
-    D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork2, 0));
-    RUN(launch_tcc_pack(L->tcc_pack_dx, L->side));
-    D4PG_CUDA_OK(cudaEventRecord(L->ev_join2, L->side));
-    TccArgs& fa = L->tcc_fwd_args;
-    tcc_args_begin(fa, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); fa.step_slot = 1;
-    TccCtx cx{L, &w, &da, &dc, Wa, Wat, Wc, Wct, B, S, A, N, Sp, Ap, Np};
-    tcc_build_T(fa, 0, cx);                                      // chain 0  T: actor_target(s') -> critic_target(s', .)
-    if (h7) tcc_build_actor(fa, 1, cx, nullptr);                 // chain 1  (post-update plan) the actor alone; the critic pass follows the critic's Adam
-    else tcc_build_P(fa, 1, cx);                                 // chain 1  P: actor(s) -> critic(s, actor(s))
-    tcc_build_Q(fa, 2, cx, w.a, w.h1[2], w.h2[2], w.h3[2], w.out[2]);   // chain 2  Q: critic(s, a)
-    if (host_pipe(c) && !cold) {
-      // warm host-pipeline variant: the batch comes from the ingest stream's sample kernel; instead of a stream event
-      // (event + graph start after the sample ends) every CTA polls the epochs that kernel publishes
-      fa.wait_epoch = w.pipe_epoch; fa.wait_clock = reinterpret_cast<const long long*>(&w.clock->steps_done);
-      fa.wait_n = cdiv(B, SAMPLE_ROWS);
-    }
-    RUN(launch_mlp_tc_chain(fa, st));
-  } else if (plan == PLAN_CHAIN) {
-    // 2'. the three forward chains of the step as ONE cluster launch (mlp_chain.cu):
-    //   chain 0  T: actor_target(s') -> critic_target(s', .)      ddpg.py:205-206
-    //   chain 1  P: actor(s) -> critic(s, actor(s))                ddpg.py:236-238 (fc1 of the critic is recomputed: K=|s|)
-    //   chain 2  Q: critic(s, a)                                   ddpg.py:208
-    // The block scheduler fills SMs in launch order: the two 8-layer chains come first so that each of their CTAs
-    // gets an SM of its own, and the short 4-layer chain is the one that doubles up
-    ChainArgs& ca = L->chain_fwd_args;
-    chain_args_begin(ca, B, w.xchg, c.precision);
-    ChainSlot sl; int at3 = -1, ct1, q1, a3 = -1, c1;
-    (void)at3; (void)a3;
-    sl = chain_fwd(Wat + da.w_off[0], la[0], Wat + da.b_off[0], H, S, EPI_BIAS_RELU, w.h1[0], H, 1); chain_src_global(sl, w.s2, Sp); int t = chain_add(ca, 0, sl);
-    sl = chain_fwd(Wat + da.w_off[1], la[1], Wat + da.b_off[1], H, H, EPI_BIAS, w.h2[0], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 0, sl);
-    sl = chain_fwd(Wat + da.w_off[2], la[2], Wat + da.b_off[2], H, H, EPI_BIAS_RELU, w.h3[0], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 0, sl);
-    // the 6-wide actor fc3 is a PRE-LAYER of the critic's fc2 slot (every CTA computes it for its 32 rows) instead of
-    // a slot of its own, when it fits (|a| <= 8, fp32 tile); otherwise it is a slot that publishes 8 plane rows
-    const int t22 = t;
-    if (pre_ok) {
-      sl = chain_fwd(Wct + dc.w_off[0], lc[0], Wct + dc.b_off[0], H, S, EPI_BIAS_RELU, w.h1[1], H, 1); chain_src_global(sl, w.s2, Sp); ct1 = chain_add(ca, 0, sl);
-      sl = chain_fwd(Wct + dc.w_off[1], lc[1], Wct + dc.b_off[1], H, H + A, EPI_BIAS_RELU, w.h2[1], H, 1); chain_src_plane(sl, ct1);
-      chain_pre_layer(sl, Wat + da.w_off[3], la[3], Wat + da.b_off[3], nullptr, 0, A, H, EPI_BIAS_TANH, w.out[0], Ap, t22, H, false);
-      t = chain_add(ca, 0, sl);
-    } else {
-    sl = chain_fwd(Wat + da.w_off[3], la[3], Wat + da.b_off[3], A, H, EPI_BIAS_TANH, w.out[0], Ap, 1); chain_src_plane(sl, t); at3 = chain_add(ca, 0, sl);
-    sl = chain_fwd(Wct + dc.w_off[0], lc[0], Wct + dc.b_off[0], H, S, EPI_BIAS_RELU, w.h1[1], H, 1); chain_src_global(sl, w.s2, Sp); ct1 = chain_add(ca, 0, sl);
-    sl = chain_fwd(Wct + dc.w_off[1], lc[1], Wct + dc.b_off[1], H, H + A, EPI_BIAS_RELU, w.h2[1], H, 1); chain_src_plane(sl, ct1); chain_src2_plane(sl, H, at3); t = chain_add(ca, 0, sl);
-    }
-    sl = chain_fwd(Wct + dc.w_off[2], lc[2], Wct + dc.b_off[2], H, H, EPI_BIAS_RELU, w.h3[1], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 0, sl);
-    sl = chain_fwd(Wct + dc.w_off[3], lc[3], Wct + dc.b_off[3], N, H, EPI_BIAS, w.out[1], Np, 0); chain_src_plane(sl, t); chain_add(ca, 0, sl);
-
-    sl = chain_fwd(Wc + dc.w_off[0], lc[0], Wc + dc.b_off[0], H, S, EPI_BIAS_RELU, w.h1[2], H, 1); chain_src_global(sl, w.s, Sp); q1 = chain_add(ca, 2, sl);
-    sl = chain_fwd(Wc + dc.w_off[1], lc[1], Wc + dc.b_off[1], H, H + A, EPI_BIAS_RELU, w.h2[2], H, 1); chain_src_plane(sl, q1); chain_src2_global(sl, H, w.a, Ap); t = chain_add(ca, 2, sl);
-    sl = chain_fwd(Wc + dc.w_off[2], lc[2], Wc + dc.b_off[2], H, H, EPI_BIAS_RELU, w.h3[2], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 2, sl);
-    sl = chain_fwd(Wc + dc.w_off[3], lc[3], Wc + dc.b_off[3], N, H, EPI_BIAS, w.out[2], Np, 0); chain_src_plane(sl, t); chain_add(ca, 2, sl);
-
-    sl = chain_fwd(Wa + da.w_off[0], la[0], Wa + da.b_off[0], H, S, EPI_BIAS_RELU, w.h1[3], H, 1); chain_src_global(sl, w.s, Sp); t = chain_add(ca, 1, sl);
-    sl = chain_fwd(Wa + da.w_off[1], la[1], Wa + da.b_off[1], H, H, EPI_BIAS, w.h2[3], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 1, sl);
-    sl = chain_fwd(Wa + da.w_off[2], la[2], Wa + da.b_off[2], H, H, EPI_BIAS_RELU, w.h3[3], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 1, sl);
-    const int a22 = t;
-    if (pre_ok) {
-      sl = chain_fwd(Wc + dc.w_off[0], lc[0], Wc + dc.b_off[0], H, S, EPI_BIAS_RELU, nullptr, H, 1); chain_src_global(sl, w.s, Sp); c1 = chain_add(ca, 1, sl);
-      sl = chain_fwd(Wc + dc.w_off[1], lc[1], Wc + dc.b_off[1], H, H + A, EPI_BIAS_RELU, w.h2[4], H, 1); chain_src_plane(sl, c1);
-      chain_pre_layer(sl, Wa + da.w_off[3], la[3], Wa + da.b_off[3], nullptr, 0, A, H, EPI_BIAS_TANH, w.out[3], Ap, a22, H, false);
-      t = chain_add(ca, 1, sl);
-    } else {
-    sl = chain_fwd(Wa + da.w_off[3], la[3], Wa + da.b_off[3], A, H, EPI_BIAS_TANH, w.out[3], Ap, 1); chain_src_plane(sl, t); a3 = chain_add(ca, 1, sl);
-    sl = chain_fwd(Wc + dc.w_off[0], lc[0], Wc + dc.b_off[0], H, S, EPI_BIAS_RELU, nullptr, H, 1); chain_src_global(sl, w.s, Sp); c1 = chain_add(ca, 1, sl);
-    sl = chain_fwd(Wc + dc.w_off[1], lc[1], Wc + dc.b_off[1], H, H + A, EPI_BIAS_RELU, w.h2[4], H, 1); chain_src_plane(sl, c1); chain_src2_plane(sl, H, a3); t = chain_add(ca, 1, sl);
-    }
-    sl = chain_fwd(Wc + dc.w_off[2], lc[2], Wc + dc.b_off[2], H, H, EPI_BIAS_RELU, w.h3[4], H, 1); chain_src_plane(sl, t); t = chain_add(ca, 1, sl);
-    sl = chain_fwd(Wc + dc.w_off[3], lc[3], Wc + dc.b_off[3], N, H, EPI_BIAS, w.out[4], Np, 0); chain_src_plane(sl, t); chain_add(ca, 1, sl);
-    RUN(launch_mlp_chain(ca, st));
+  sl = chain_layer_dx(layer_dx(L, CRITIC, 3), EPI_RELU_MASK, w.h3[4], H, w.p_dz22, H, 1); chain_src_global(sl, w.dlogits_pi, Np); t = chain_add(cb, 1, sl);
+  sl = chain_layer_dx(layer_dx(L, CRITIC, 2), EPI_RELU_MASK, w.h2[4], H, w.p_dz2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
+  const LayerDx da = critic_fc2_action_dx(L);
+  if (chain_pre_ok(x)) {      // d action (6 wide) as a pre-layer of the step through actor fc3
+    sl = chain_layer_dx(layer_dx(L, ACTOR, 3), EPI_RELU_MASK, w.h3[3], H, w.a_dz22, H, 1);
+    chain_pre_layer(sl, da.W, da.ldw, nullptr, w.out[3], Ap, da.n_in, da.k_out, EPI_TANH_MASK, w.a_dz3, Ap, t, H, true);
+    t = chain_add(cb, 1, sl);
   } else {
-  // 2. forward level 1: fc1 of actor_target(s'), critic_target(s'), critic(s), actor(s)
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.s2, Sp, nullptr, 0, 0, Wat + da.w_off[0], la[0], Wat + da.b_off[0], w.h1[0], H, B, H, S, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.s2, Sp, nullptr, 0, 0, Wct + dc.w_off[0], lc[0], Wct + dc.b_off[0], w.h1[1], H, B, H, S, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.s, Sp, nullptr, 0, 0, Wc + dc.w_off[0], lc[0], Wc + dc.b_off[0], w.h1[2], H, B, H, S, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.s, Sp, nullptr, 0, 0, Wa + da.w_off[0], la[0], Wa + da.b_off[0], w.h1[3], H, B, H, S, EPI_BIAS_RELU));
-  LEVEL(g);
-  // level 2: fc2 (actor: no activation, models.py:36; critic: cat(h1, a) + relu, models.py:80)
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h1[0], H, nullptr, 0, 0, Wat + da.w_off[1], la[1], Wat + da.b_off[1], w.h2[0], H, B, H, H, EPI_BIAS));
-  gemm_batch_add(g, gemm_fwd(w.h1[2], H, w.a, Ap, H, Wc + dc.w_off[1], lc[1], Wc + dc.b_off[1], w.h2[2], H, B, H, H + A, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.h1[3], H, nullptr, 0, 0, Wa + da.w_off[1], la[1], Wa + da.b_off[1], w.h2[3], H, B, H, H, EPI_BIAS));
-  LEVEL(g);
-  // level 3: fc2_2 + relu
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h2[0], H, nullptr, 0, 0, Wat + da.w_off[2], la[2], Wat + da.b_off[2], w.h3[0], H, B, H, H, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.h2[2], H, nullptr, 0, 0, Wc + dc.w_off[2], lc[2], Wc + dc.b_off[2], w.h3[2], H, B, H, H, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.h2[3], H, nullptr, 0, 0, Wa + da.w_off[2], la[2], Wa + da.b_off[2], w.h3[3], H, B, H, H, EPI_BIAS_RELU));
-  LEVEL(g);
-  // level 4: fc3 (actor: tanh; critic: logits)
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h3[0], H, nullptr, 0, 0, Wat + da.w_off[3], la[3], Wat + da.b_off[3], w.out[0], Ap, B, A, H, EPI_BIAS_TANH));
-  gemm_batch_add(g, gemm_fwd(w.h3[2], H, nullptr, 0, 0, Wc + dc.w_off[3], lc[3], Wc + dc.b_off[3], w.out[2], Np, B, N, H, EPI_BIAS));
-  gemm_batch_add(g, gemm_fwd(w.h3[3], H, nullptr, 0, 0, Wa + da.w_off[3], la[3], Wa + da.b_off[3], w.out[3], Ap, B, A, H, EPI_BIAS_TANH));
-  LEVEL(g);
-  // level 5: critic_target.fc2([h1t, a_t(s')]) and critic.fc2([h1, actor(s)]) (h1 of the critic is reused)
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h1[1], H, w.out[0], Ap, H, Wct + dc.w_off[1], lc[1], Wct + dc.b_off[1], w.h2[1], H, B, H, H + A, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.h1[2], H, w.out[3], Ap, H, Wc + dc.w_off[1], lc[1], Wc + dc.b_off[1], w.h2[4], H, B, H, H + A, EPI_BIAS_RELU));
-  LEVEL(g);
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h2[1], H, nullptr, 0, 0, Wct + dc.w_off[2], lc[2], Wct + dc.b_off[2], w.h3[1], H, B, H, H, EPI_BIAS_RELU));
-  gemm_batch_add(g, gemm_fwd(w.h2[4], H, nullptr, 0, 0, Wc + dc.w_off[2], lc[2], Wc + dc.b_off[2], w.h3[4], H, B, H, H, EPI_BIAS_RELU));
-  LEVEL(g);
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_fwd(w.h3[1], H, nullptr, 0, 0, Wct + dc.w_off[3], lc[3], Wct + dc.b_off[3], w.out[1], Np, B, N, H, EPI_BIAS));
-  gemm_batch_add(g, gemm_fwd(w.h3[4], H, nullptr, 0, 0, Wc + dc.w_off[3], lc[3], Wc + dc.b_off[3], w.out[4], Np, B, N, H, EPI_BIAS));
-  LEVEL(g);
-
+    sl = chain_layer_dx(da, EPI_TANH_MASK, w.out[3], Ap, w.a_dz3, Ap, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
+    sl = chain_layer_dx(layer_dx(L, ACTOR, 3), EPI_RELU_MASK, w.h3[3], H, w.a_dz22, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
   }
+  sl = chain_layer_dx(layer_dx(L, ACTOR, 2), EPI_NONE, nullptr, 0, w.a_dh2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
+  sl = chain_layer_dx(layer_dx(L, ACTOR, 1), EPI_RELU_MASK, w.h1[3], H, w.a_dz1, H, 0); chain_src_plane(sl, t); chain_add(cb, 1, sl);
+  RUN("launch_mlp_chain", true, launch_mlp_chain(cb, x.st));
+  return D4PG_OK;
+}
 
-  // 3. heads: softmaxes, projection, CE loss, td, priorities, logit gradients (ddpg.py:214-222,236-238)
-  //    (mixture critic: the quadrature cross-entropy, td, priorities and raw-head gradients of mog_heads.cu)
-  const bool mog = c.dist_type == 1;
-  MogArgs ma{};
-  ma.target_raw = w.out[1]; ma.q_raw = w.out[2]; ma.pi_raw = h7 ? nullptr : w.out[4];
-  ma.rewards = w.r; ma.dones = w.done; ma.B = B; ma.K = c.n_components; ma.ld = Np;
-  ma.discount = (c.proj_mode == 1) ? pow(c.gamma, double(c.n_steps)) : c.gamma; ma.prio_eps = c.prio_eps;
-  ma.grad_scale = 1.0f / (float(B) * float(c.world_size > 1 ? c.world_size : 1));
-  ma.loss_rows = w.loss_rows; ma.td = b.td; ma.prio = b.prio; ma.dq_raw = w.dlogits_q;
-  ma.pi_rows = w.pi_rows; ma.dpi_raw = w.dlogits_pi;
-  ma.is_weights = ((c.loss_flags & 1) && c.prioritized) ? bwts : nullptr;
-  ma.sampler_clock = pf ? w.clock : nullptr;
-  //    (quantile critic: the quantile-Huber loss, td, priorities and quantile gradients of qr_heads.cu)
-  const bool qr = c.dist_type == 2;
-  QrArgs qa{};
-  qa.target_q = w.out[1]; qa.q = w.out[2]; qa.pi_q = h7 ? nullptr : w.out[4];
-  qa.rewards = w.r; qa.dones = w.done; qa.B = B; qa.N = N; qa.ld = Np;
-  qa.discount = ma.discount; qa.kappa = c.qr_kappa; qa.prio_eps = c.prio_eps; qa.grad_scale = ma.grad_scale;
-  qa.loss_rows = w.loss_rows; qa.td = b.td; qa.prio = b.prio; qa.dq = w.dlogits_q;
-  qa.pi_rows = w.pi_rows; qa.dpi = w.dlogits_pi;
-  qa.is_weights = ma.is_weights; qa.ce_priority = (c.loss_flags & 2) ? 1 : 0;
-  qa.sampler_clock = ma.sampler_clock;
-  HeadsArgs ha{};
-  ha.target_logits = w.out[1]; ha.q_logits = w.out[2]; ha.pi_logits = h7 ? nullptr : w.out[4];
-  ha.rewards = w.r; ha.dones = w.done; ha.B = B; ha.N = N; ha.flags = 0; ha.ld = Np;
-  ha.v_min = c.v_min; ha.v_max = c.v_max; ha.delta = (c.v_max - c.v_min) / double(N - 1);
-  // live projection discounts with gamma even for n_steps>1 (SURVEY.md H5); mode 1 uses gamma**n (ddpg.py:24)
-  ha.discount = (c.proj_mode == 1) ? pow(c.gamma, double(c.n_steps)) : c.gamma; ha.prio_eps = c.prio_eps;
-  ha.grad_scale = 1.0f / (float(B) * float(c.world_size > 1 ? c.world_size : 1));
-  ha.m = w.m; ha.target_probs = w.target_probs; ha.q_probs = w.q_probs;
-  ha.loss_rows = w.loss_rows; ha.td = b.td; ha.prio = b.prio; ha.dlogits_q = w.dlogits_q;
-  ha.pi_rows = w.pi_rows; ha.dlogits_pi = w.dlogits_pi;
-  ha.is_weights = ((c.loss_flags & 1) && c.prioritized) ? bwts : nullptr;
-  ha.sampler_clock = pf ? w.clock : nullptr;          // sample(t) is done, sample(t+1) not yet launched
-  ha.ce_priority = (c.loss_flags & 2) ? 1 : 0;
-  if (mog) RUN(launch_mog_heads(ma, st));
-  else if (qr) RUN(launch_qr_heads(qa, st));
-  else RUN(launch_heads(ha, c.proj_mode, st));
-
-  // 4. priorities into the trees (ddpg.py:252-255): independent of the backward pass, so it runs
-  //    on a forked branch (side stream -> parallel graph branch) and joins before the step ends
-  if (c.prioritized || pf) {
-    D4PG_CUDA_OK(cudaEventRecord(L->ev_fork, st));
-    D4PG_CUDA_OK(cudaStreamWaitEvent(L->side, L->ev_fork, 0));
-    // host pipeline: the write-back also opens the ingest gate of step k+1 (its tree add / presample wait for this step's
-    // loss kernel -- which advanced the sampler clock -- and for the priorities)
-    if (c.prioritized) RUN(launch_tree_update(L->replay, B, bidx, b.prio, L->side, host_pipe(c) ? L->gate_flag : nullptr));
-    else if (host_pipe(c)) RUN(launch_gate_signal(L->gate_flag, L->side));
-    if (prefetching(c)) {
-      // 4'. the NEXT step's batch, sampled from the just-updated trees into the other half of the batch buffers
-      // while this step's backward pass, dW and Adam run (it needs the trees, not the weights)
-      const int q = par ^ 1;
-      const Workspace& o = L->ws;
-      RUN(learner_sample(L->replay, B, c.prioritized, nullptr, nullptr, c.philox_seed, w.clock, cp, o.idx2[q], o.wts2[q],
-                         q ? o.s_b : o.s, q ? o.a_b : o.a, q ? o.r_b : o.r, q ? o.s2_b : o.s2, q ? o.done_b : o.done,
-                         Sp, Ap, q, L->side));
-    }
-    if (pf) {                           // the caller-visible copies of this step's indices / IS weights (off the
-      // path to the next batch: after the write-back and the prefetch)
-      D4PG_CUDA_OK(cudaMemcpyAsync(b.idx, bidx, size_t(B) * sizeof(int32_t), cudaMemcpyDeviceToDevice, L->side));
-      if (b.weights && c.prioritized)
-        D4PG_CUDA_OK(cudaMemcpyAsync(b.weights, bwts, size_t(B) * sizeof(float), cudaMemcpyDeviceToDevice, L->side));
-    }
-    D4PG_CUDA_OK(cudaEventRecord(L->ev_join, L->side));
+// The weight (and bias) gradient of layer l of the critic (from the critic-loss pass) or of the actor
+static GemmProblem dw_problem(const Step& x, Net net, int l) {
+  const Workspace& w = x.w; const NetDims& da = x.L->da; const NetDims& dc = x.L->dc;
+  const int B = x.B, S = x.S, A = x.A, N = x.N, H = D4PG_HIDDEN, Sp = x.Sp, Ap = x.Ap, Np = x.Np;
+  const int* la = da.ld; const int* lc = dc.ld;
+  float* Ga = x.Ga; float* Gc = x.Gc;
+  if (net == CRITIC) switch (l) {
+    case 0: return gemm_dw(w.c_dz1, H, x.bt.s, Sp, Gc + dc.w_off[0], lc[0], Gc + dc.b_off[0], H, S, B);
+    case 1: return gemm_dw(w.c_dz2, H, w.h1[2], H, Gc + dc.w_off[1], lc[1], Gc + dc.b_off[1], H, H, B);   // the h1 columns
+    case 2: return gemm_dw(w.c_dz22, H, w.h2[2], H, Gc + dc.w_off[2], lc[2], Gc + dc.b_off[2], H, H, B);
+    default: return gemm_dw(w.dlogits_q, Np, w.h3[2], H, Gc + dc.w_off[3], lc[3], Gc + dc.b_off[3], N, H, B);
   }
-
-  float* Ga = b.grad_actor; float* Gc = b.grad_critic;
-  // data parallel with IPC-mapped peers: this step's gradients go straight into this rank's half of the exchange
-  // buffer (double-buffered by step parity), the Adam kernel sums all ranks' halves over NVLink
-  PeerInfo peers{};
-  const bool peer_mode = c.world_size > 1 && comm_peer_info(L->comm, &peers);
-  const int gpar = pf ? par : int(L->steps_done & 1);
-  // Exchange shapes (D4PG_COMM_MODE=mc|mc2|pull|rs; default: "mc" from D4PG_COMM_MC_FROM = 3 ranks up when the communicator
-  // set up a multicast object, else "pull").  These defaults were chosen on another GPU generation and have NOT been
-  // validated on Hopper (no multi-GPU H100 measurement exists yet; tools/ab_mc8.sh compares the modes):
-  //   "mc"   in-switch reduction: ONE hop and 1.15 MB inbound per rank -- the Adam kernel's multimem.ld_reduce over an NVLS
-  //          multicast object returns the sum over all ranks, added by the NVSwitch;
-  //   "mc2"  its two-phase form: every rank ld_reduces its 1/N slice and multimem.st's it to everyone (2 x 1.15 MB per GPU
-  //          whatever N), then a second flag hop;
-  //   "pull" one hop, every rank sums all N halves inside Adam (N x 1.15 MB inbound over NVLink);
-  //   "rs"   reduce-scatter + all-gather over peer memory: TWO hops of 16-B remote accesses.
-  static const int comm_mode = [] { const char* e = getenv("D4PG_COMM_MODE");
-                                    return !e ? 0 : (e[0] == 'p' ? 1 : (e[0] == 'r' ? 2 : (e[0] == 'm' && e[1] == 'c' && e[2] == '2' ? 4 : 3))); }();
-  static const int mc_from = [] { const char* e = getenv("D4PG_COMM_MC_FROM"); return e ? atoi(e) : 3; }();
-  static const int mc2_from = [] { const char* e = getenv("D4PG_COMM_MC2_FROM"); return e ? atoi(e) : 1000; }();
-  const bool mc_avail = peer_mode && peers.mc != nullptr && plan != PLAN_LEVELS;
-  const bool peer_mc2 = mc_avail && (comm_mode == 4 || (comm_mode == 0 && peers.world >= mc2_from));
-  const bool peer_mc = mc_avail && !peer_mc2 && (comm_mode == 3 || (comm_mode == 0 && peers.world >= mc_from));
-  const bool peer_rs = peer_mode && !peer_mc && !peer_mc2 && comm_mode == 2;
-  const bool use_mc_buf = peer_mc || peer_mc2;
-  // this step's gradients go into this rank's half of the exchange buffer: the multicast-bound one when the in-switch
-  // reduction is set up, else the IPC-mapped one the peers read directly
-  if (peer_mode) { Ga = (use_mc_buf ? peers.mc_uc : peers.x[peers.rank]) + int64_t(gpar) * peers.n; Gc = Ga + da.total; }
-  if (B >= 1024)                // dW levels run split-K with fp32 atomics: the gradient buffer must start at zero
-    D4PG_CUDA_OK(cudaMemsetAsync(Ga, 0, size_t(da.total + dc.total) * sizeof(float), st));
-  if (plan == PLAN_TC_CHAIN) {
-    // 5''. both dX chains on the tensor cores (transposed weight images; masks applied by the epilogue)
-    D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_join2, 0));       // transposed weight images are packed
-    TccArgs& ba = L->tcc_bwd_args;
-    tcc_args_begin(ba, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); ba.step_slot = 5;
-    TccCtx cx{L, &w, &da, &dc, Wa, Wat, Wc, Wct, B, S, A, N, Sp, Ap, Np};
-    tcc_build_bwd_C(ba, 0, cx);                                  // C: critic loss
-    if (!h7) tcc_build_bwd_P(ba, 1, cx);                         // P: policy loss (PRE-update critic weights, SURVEY.md H7)
-    RUN(launch_mlp_tc_chain(ba, st));
+  switch (l) {
+    case 0: return gemm_dw(w.a_dz1, H, x.bt.s, Sp, Ga + da.w_off[0], la[0], Ga + da.b_off[0], H, S, B);
+    case 1: return gemm_dw(w.a_dh2, H, w.h1[3], H, Ga + da.w_off[1], la[1], Ga + da.b_off[1], H, H, B);
+    case 2: return gemm_dw(w.a_dz22, H, w.h2[3], H, Ga + da.w_off[2], la[2], Ga + da.b_off[2], H, H, B);
+    default: return gemm_dw(w.a_dz3, Ap, w.h3[3], H, Ga + da.w_off[3], la[3], Ga + da.b_off[3], A, H, B);
   }
-  if (plan == PLAN_CHAIN) {
-    // 5'. both dX chains as ONE cluster launch, then every dW of the step as ONE grouped launch
-    //   C: critic loss  dlogits_q  -> fc3 -> fc2_2 -> fc2[:, :H]                         ddpg.py:230
-    //   P: policy loss  dlogits_pi -> fc3 -> fc2_2 -> fc2[:, H:] (d action, tanh') ->
-    //                   actor fc3 -> fc2_2 -> fc2   (PRE-update critic weights, SURVEY.md H7)  ddpg.py:242
-    ChainArgs& cb = L->chain_bwd_args;
-    chain_args_begin(cb, B, w.xchg, c.precision); cb.trace_base = 6 * CHAIN_MAX_SLOTS;
-    ChainSlot sl; int t;
-    sl = chain_dx(Wc + dc.w_off[3], lc[3], H, N, EPI_RELU_MASK, w.h3[2], H, w.c_dz22, H, 1); chain_src_global(sl, w.dlogits_q, Np); t = chain_add(cb, 0, sl);
-    sl = chain_dx(Wc + dc.w_off[2], lc[2], H, H, EPI_RELU_MASK, w.h2[2], H, w.c_dz2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 0, sl);
-    sl = chain_dx(Wc + dc.w_off[1], lc[1], H, H, EPI_RELU_MASK, w.h1[2], H, w.c_dz1, H, 0); chain_src_plane(sl, t); chain_add(cb, 0, sl);
+}
+// critic fc2's action columns: dW2 = [dz2^T h1 | dz2^T a]
+static GemmProblem dw_critic_fc2_action(const Step& x) {
+  return gemm_dw(x.w.c_dz2, D4PG_HIDDEN, x.bt.a, x.Ap, x.Gc + critic_fc2_action_off(x.L), x.L->dc.ld[1], nullptr,
+                 D4PG_HIDDEN, x.A, x.B);
+}
+// chain plans: every dW of the step as ONE grouped launch (the post-update plan: the critic's, later the actor's)
+static int dw_wide(Step& x, bool critic, bool actor) {
+  GemmWideBatch& gw = x.L->dw_batch;
+  PeerSignal sig1{};
+  if (peer_exchange(x)) sig1 = comm_peer_signal(x.peers, 0);
+  gemm_wide_begin(gw, peer_exchange(x) ? &sig1 : nullptr);         // its last CTA signals the peers
+  if (critic) gemm_wide_add(gw, dw_problem(x, CRITIC, 2));
+  if (critic) gemm_wide_add(gw, dw_problem(x, CRITIC, 1));
+  if (actor) gemm_wide_add(gw, dw_problem(x, ACTOR, 2));
+  if (actor) gemm_wide_add(gw, dw_problem(x, ACTOR, 1));
+  if (critic) gemm_wide_add(gw, dw_problem(x, CRITIC, 3));
+  if (critic) gemm_wide_add(gw, dw_critic_fc2_action(x));
+  if (critic) gemm_wide_add(gw, dw_problem(x, CRITIC, 0));
+  if (actor) gemm_wide_add(gw, dw_problem(x, ACTOR, 3));
+  if (actor) gemm_wide_add(gw, dw_problem(x, ACTOR, 0));
+  RUN("gemm_wide_launch", false, gemm_wide_launch(gw, x.st));
+  return D4PG_OK;
+}
 
-    sl = chain_dx(Wc + dc.w_off[3], lc[3], H, N, EPI_RELU_MASK, w.h3[4], H, w.p_dz22, H, 1); chain_src_global(sl, w.dlogits_pi, Np); t = chain_add(cb, 1, sl);
-    sl = chain_dx(Wc + dc.w_off[2], lc[2], H, H, EPI_RELU_MASK, w.h2[4], H, w.p_dz2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
-    if (pre_ok) {      // d action (6 wide) as a pre-layer of the step through actor fc3
-      sl = chain_dx(Wa + da.w_off[3], la[3], H, A, EPI_RELU_MASK, w.h3[3], H, w.a_dz22, H, 1);
-      chain_pre_layer(sl, Wc + dc.w_off[1] + H, lc[1], nullptr, w.out[3], Ap, A, H, EPI_TANH_MASK, w.a_dz3, Ap, t, H, true);
-      t = chain_add(cb, 1, sl);
-    } else {
-    sl = chain_dx(Wc + dc.w_off[1] + H, lc[1], A, H, EPI_TANH_MASK, w.out[3], Ap, w.a_dz3, Ap, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
-    sl = chain_dx(Wa + da.w_off[3], la[3], H, A, EPI_RELU_MASK, w.h3[3], H, w.a_dz22, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
-    }
-    sl = chain_dx(Wa + da.w_off[2], la[2], H, H, EPI_NONE, nullptr, 0, w.a_dh2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
-    sl = chain_dx(Wa + da.w_off[1], la[1], H, H, EPI_RELU_MASK, w.h1[3], H, w.a_dz1, H, 0); chain_src_plane(sl, t); chain_add(cb, 1, sl);
-    RUN(launch_mlp_chain(cb, st));
-  }
-  if (plan != PLAN_LEVELS) {              // every dW of the step as ONE grouped launch
-    GemmWideBatch& gw = L->dw_batch;
-    PeerSignal sig1{};
-    if (peer_mode) sig1 = comm_peer_signal(peers, 0);
-    gemm_wide_begin(gw, peer_mode ? &sig1 : nullptr);              // its last CTA signals the peers
-    gemm_wide_add(gw, gemm_dw(w.c_dz22, H, w.h2[2], H, Gc + dc.w_off[2], lc[2], Gc + dc.b_off[2], H, H, B));
-    gemm_wide_add(gw, gemm_dw(w.c_dz2, H, w.h1[2], H, Gc + dc.w_off[1], lc[1], Gc + dc.b_off[1], H, H, B));
-    if (!h7) gemm_wide_add(gw, gemm_dw(w.a_dz22, H, w.h2[3], H, Ga + da.w_off[2], la[2], Ga + da.b_off[2], H, H, B));
-    if (!h7) gemm_wide_add(gw, gemm_dw(w.a_dh2, H, w.h1[3], H, Ga + da.w_off[1], la[1], Ga + da.b_off[1], H, H, B));
-    gemm_wide_add(gw, gemm_dw(w.dlogits_q, Np, w.h3[2], H, Gc + dc.w_off[3], lc[3], Gc + dc.b_off[3], N, H, B));
-    gemm_wide_add(gw, gemm_dw(w.c_dz2, H, w.a, Ap, Gc + dc.w_off[1] + H, lc[1], nullptr, H, A, B));
-    gemm_wide_add(gw, gemm_dw(w.c_dz1, H, w.s, Sp, Gc + dc.w_off[0], lc[0], Gc + dc.b_off[0], H, S, B));
-    if (!h7) gemm_wide_add(gw, gemm_dw(w.a_dz3, Ap, w.h3[3], H, Ga + da.w_off[3], la[3], Ga + da.b_off[3], A, H, B));
-    if (!h7) gemm_wide_add(gw, gemm_dw(w.a_dz1, H, w.s, Sp, Ga + da.w_off[0], la[0], Ga + da.b_off[0], H, S, B));
-    RUN(gemm_wide_launch(gw, st));
-  } else {
-  // 5. backward.  "c_" = critic-loss pass, "p_" = policy pass through the critic, "a_" = actor.
+static GemmProblem level_dx(const Step& x, const LayerDx& d, const float* dZ, int lddz, float* dX, int lddx, int epi,
+                            const float* aux, int ldaux) {
+  return gemm_dx(dZ, lddz, d.W, d.ldw, dX, lddx, x.B, d.n_in, d.k_out, epi, aux, ldaux);
+}
+// 5. backward of the level plan: dX and dW of a layer share a level
+static int backward_levels(Step& x) {
+  d4pg_learner* L = x.L; const Workspace& w = x.w;
+  const int H = D4PG_HIDDEN, Ap = x.Ap, Np = x.Np;
   // level B1: through critic.fc3
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(w.dlogits_q, Np, Wc + dc.w_off[3], lc[3], w.c_dz22, H, B, H, N, EPI_RELU_MASK, w.h3[2], H));
-  gemm_batch_add(g, gemm_dx(w.dlogits_pi, Np, Wc + dc.w_off[3], lc[3], w.p_dz22, H, B, H, N, EPI_RELU_MASK, w.h3[4], H));
-  gemm_batch_add(g, gemm_dw(w.dlogits_q, Np, w.h3[2], H, Gc + dc.w_off[3], lc[3], Gc + dc.b_off[3], N, H, B));
-  LEVEL(g);
+  int rc = run_level(x, {level_dx(x, layer_dx(L, CRITIC, 3), w.dlogits_q, Np, w.c_dz22, H, EPI_RELU_MASK, w.h3[2], H),
+                         level_dx(x, layer_dx(L, CRITIC, 3), w.dlogits_pi, Np, w.p_dz22, H, EPI_RELU_MASK, w.h3[4], H),
+                         dw_problem(x, CRITIC, 3)});
   // level B2: through critic.fc2_2
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(w.c_dz22, H, Wc + dc.w_off[2], lc[2], w.c_dz2, H, B, H, H, EPI_RELU_MASK, w.h2[2], H));
-  gemm_batch_add(g, gemm_dx(w.p_dz22, H, Wc + dc.w_off[2], lc[2], w.p_dz2, H, B, H, H, EPI_RELU_MASK, w.h2[4], H));
-  gemm_batch_add(g, gemm_dw(w.c_dz22, H, w.h2[2], H, Gc + dc.w_off[2], lc[2], Gc + dc.b_off[2], H, H, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {level_dx(x, layer_dx(L, CRITIC, 2), w.c_dz22, H, w.c_dz2, H, EPI_RELU_MASK, w.h2[2], H),
+                              level_dx(x, layer_dx(L, CRITIC, 2), w.p_dz22, H, w.p_dz2, H, EPI_RELU_MASK, w.h2[4], H),
+                              dw_problem(x, CRITIC, 2)});
   // level B3: through critic.fc2: dh1 (critic loss), d action (policy, tanh' folded in), dW2 = [dz2^T h1 | dz2^T a]
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(w.c_dz2, H, Wc + dc.w_off[1], lc[1], w.c_dz1, H, B, H, H, EPI_RELU_MASK, w.h1[2], H));
-  gemm_batch_add(g, gemm_dx(w.p_dz2, H, Wc + dc.w_off[1] + H, lc[1], w.a_dz3, Ap, B, A, H, EPI_TANH_MASK, w.out[3], Ap));
-  gemm_batch_add(g, gemm_dw(w.c_dz2, H, w.h1[2], H, Gc + dc.w_off[1], lc[1], Gc + dc.b_off[1], H, H, B));
-  gemm_batch_add(g, gemm_dw(w.c_dz2, H, w.a, Ap, Gc + dc.w_off[1] + H, lc[1], nullptr, H, A, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {level_dx(x, layer_dx(L, CRITIC, 1), w.c_dz2, H, w.c_dz1, H, EPI_RELU_MASK, w.h1[2], H),
+                              level_dx(x, critic_fc2_action_dx(L), w.p_dz2, H, w.a_dz3, Ap, EPI_TANH_MASK, w.out[3], Ap),
+                              dw_problem(x, CRITIC, 1),
+                              dw_critic_fc2_action(x)});
   // level B4: critic.fc1 weights; actor.fc3
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dw(w.c_dz1, H, w.s, Sp, Gc + dc.w_off[0], lc[0], Gc + dc.b_off[0], H, S, B));
-  gemm_batch_add(g, gemm_dx(w.a_dz3, Ap, Wa + da.w_off[3], la[3], w.a_dz22, H, B, H, A, EPI_RELU_MASK, w.h3[3], H));
-  gemm_batch_add(g, gemm_dw(w.a_dz3, Ap, w.h3[3], H, Ga + da.w_off[3], la[3], Ga + da.b_off[3], A, H, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {dw_problem(x, CRITIC, 0),
+                              level_dx(x, layer_dx(L, ACTOR, 3), w.a_dz3, Ap, w.a_dz22, H, EPI_RELU_MASK, w.h3[3], H),
+                              dw_problem(x, ACTOR, 3)});
   // level B5: actor.fc2_2 (its input h2 has no activation -> plain dX)
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(w.a_dz22, H, Wa + da.w_off[2], la[2], w.a_dh2, H, B, H, H, EPI_NONE, nullptr, 0));
-  gemm_batch_add(g, gemm_dw(w.a_dz22, H, w.h2[3], H, Ga + da.w_off[2], la[2], Ga + da.b_off[2], H, H, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {level_dx(x, layer_dx(L, ACTOR, 2), w.a_dz22, H, w.a_dh2, H, EPI_NONE, nullptr, 0),
+                              dw_problem(x, ACTOR, 2)});
   // level B6: actor.fc2
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(w.a_dh2, H, Wa + da.w_off[1], la[1], w.a_dz1, H, B, H, H, EPI_RELU_MASK, w.h1[3], H));
-  gemm_batch_add(g, gemm_dw(w.a_dh2, H, w.h1[3], H, Ga + da.w_off[1], la[1], Ga + da.b_off[1], H, H, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {level_dx(x, layer_dx(L, ACTOR, 1), w.a_dh2, H, w.a_dz1, H, EPI_RELU_MASK, w.h1[3], H),
+                              dw_problem(x, ACTOR, 1)});
   // level B7: actor.fc1
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dw(w.a_dz1, H, w.s, Sp, Ga + da.w_off[0], la[0], Ga + da.b_off[0], H, S, B));
-  LEVEL(g);
+  if (!rc) rc = run_level(x, {dw_problem(x, ACTOR, 0)});
+  return rc;
+}
 
-  }
-
-  // 6. data-parallel gradient exchange: ONE all-reduce over the flat [P_a + P_c] buffer
-  // every rank's half of this step must be complete before Adam sums them: the chain plans signal from the dW
-  // kernel and wait inside the Adam kernel; the level plan (several dW launches) uses a small barrier launch
-  const bool inline_sync = peer_mode && plan != PLAN_LEVELS;
-  if (peer_mode && !inline_sync) RUN(comm_peer_barrier(L->comm, st));
+// 6. data-parallel gradient exchange: ONE all-reduce over the flat [P_a + P_c] buffer.
+// Every rank's half of this step must be complete before Adam sums them: the chain plans signal from the dW
+// kernel and wait inside the Adam kernel; the level plan (several dW launches) uses a small barrier launch
+static bool inline_sync(const Step& x) { return peer_exchange(x) && x.L->plan != PLAN_LEVELS; }
+static int exchange_gradients(Step& x) {
+  d4pg_learner* L = x.L;
+  if (peer_exchange(x) && !inline_sync(x)) RUN("comm_peer_barrier", false, comm_peer_barrier(L->comm, x.st));
   // reduce-scatter + all-gather over peer memory: each rank reduces its 1/N slice and pushes it to everyone
-  if (peer_mc2) RUN(comm_mc_reduce_bcast(L->comm, gpar, st));
-  else if (peer_rs) RUN(comm_peer_reduce_scatter(L->comm, gpar, st));
-  else if (!peer_mode && c.world_size > 1) RUN(comm_allreduce(L->comm, Ga, da.total + dc.total, st));
+  if (x.xm == XCHG_MC2) RUN("comm_mc_reduce_bcast", false, comm_mc_reduce_bcast(L->comm, x.gpar, x.st));
+  else if (x.xm == XCHG_RS) RUN("comm_peer_reduce_scatter", false, comm_peer_reduce_scatter(L->comm, x.gpar, x.st));
+  else if (x.xm == XCHG_ALLREDUCE)
+    RUN("comm_allreduce", false, comm_allreduce(L->comm, x.Ga, L->da.total + L->dc.total, x.st));
+  return D4PG_OK;
+}
 
-  // 7. Adam (actor + critic), sync (identity), Polyak -- one launch, two segments
+// 7. Adam (actor + critic), sync (identity), Polyak -- one launch, two segments
+static AdamArgs adam_args(const Step& x) {
+  d4pg_learner* L = x.L; const d4pg_learner_config_t& c = x.c; const d4pg_learner_buffers_t& b = x.b;
+  const NetDims& da = L->da; const NetDims& dc = L->dc; const PeerInfo& peers = x.peers;
   AdamArgs aa{};
-  aa.seg[0] = AdamSeg{b.actor, Ga, b.adam_m_actor, b.adam_v_actor, b.actor_target, da.total, nullptr, 0, 0.f, 0};
-  aa.seg[1] = AdamSeg{b.critic, Gc, b.adam_m_critic, b.adam_v_critic, b.critic_target, dc.total, nullptr, 0, 0.f, 1};
-  if (peer_mode) {                                              // sum of the ranks' halves, also stored in the caller's buffer
+  aa.seg[0] = AdamSeg{b.actor, x.Ga, b.adam_m_actor, b.adam_v_actor, b.actor_target, da.total, nullptr, 0, 0.f, 0};
+  aa.seg[1] = AdamSeg{b.critic, x.Gc, b.adam_m_critic, b.adam_v_critic, b.critic_target, dc.total, nullptr, 0, 0.f, 1};
+  if (peer_exchange(x)) {                                       // sum of the ranks' halves, also stored in the caller's buffer
     aa.npeers = peers.world;
-    for (int r = 0; r < peers.world; ++r) aa.peer_g[r] = peers.x[r] + int64_t(gpar) * peers.n;
+    for (int r = 0; r < peers.world; ++r) aa.peer_g[r] = peers.x[r] + int64_t(x.gpar) * peers.n;
     aa.seg[0].g_out = b.grad_actor; aa.seg[0].g_off = 0;
     aa.seg[1].g_out = b.grad_critic; aa.seg[1].g_off = da.total;
-    aa.my_flags = inline_sync ? peers.flag[peers.rank] : nullptr; aa.rank = peers.rank;
-    if (peer_mc) aa.mc_g = peers.mc + int64_t(gpar) * peers.n;    // NVSwitch reduces; signal 0 (every rank's dW done) is awaited in-kernel
-    if (peer_mc2) {                                             // the reduced gradient was broadcast into the local multicast-bound buffer
+    aa.my_flags = inline_sync(x) ? peers.flag[peers.rank] : nullptr; aa.rank = peers.rank;
+    if (x.xm == XCHG_MC) aa.mc_g = peers.mc + int64_t(x.gpar) * peers.n;   // NVSwitch reduces; signal 0 (every rank's dW done) is awaited in-kernel
+    if (x.xm == XCHG_MC2) {                                     // the reduced gradient was broadcast into the local multicast-bound buffer
       aa.peer_reduced = 1;
       aa.seg[0].g = peers.mc_uc + 2 * peers.n; aa.seg[1].g = peers.mc_uc + 2 * peers.n + da.total;
       aa.my_flags = peers.flag2[peers.rank];
     }
-    if (peer_rs) {                                              // the reduced gradient is local: wait for every rank's "slice pushed", then stream it
+    if (x.xm == XCHG_RS) {                                      // the reduced gradient is local: wait for every rank's "slice pushed", then stream it
       aa.peer_reduced = 1;
       aa.seg[0].g = peers.red[peers.rank]; aa.seg[1].g = peers.red[peers.rank] + da.total;
       aa.my_flags = peers.flag2[peers.rank];
     }
   }
   aa.nseg = 2;
-  if (plan == PLAN_TC_CHAIN) {                                  // keep the forward weight images of the tensor-core chains current
+  if (L->plan == PLAN_TC_CHAIN) {                               // keep the forward weight images of the tensor-core chains current
     const TccImage* U = L->tcc_img;
     const NetDims* nd[2] = {&da, &dc};
-    const int base[2] = {U_A_F1, U_C_F1}, tbase[2] = {U_AT_F1, U_CT_F1};
+    const Net online[2] = {ACTOR, CRITIC}, target[2] = {ACTOR_TARGET, CRITIC_TARGET};
     for (int sg = 0; sg < 2; ++sg) {
       aa.seg[sg].nimg = 4;
       for (int ly = 0; ly < 4; ++ly) {
         AdamImgLayer& I = aa.seg[sg].imgl[ly];
         I.w_off = nd[sg]->w_off[ly]; I.w_end = I.w_off + int64_t(nd[sg]->out[ly]) * nd[sg]->ld[ly];
-        I.ld = nd[sg]->ld[ly]; I.nchunks = U[base[sg] + ly].kchunks;
-        I.img = const_cast<uint8_t*>(U[base[sg] + ly].ptr); I.img_t = const_cast<uint8_t*>(U[tbase[sg] + ly].ptr);
+        I.ld = nd[sg]->ld[ly]; I.nchunks = U[fwd_image(online[sg], ly)].kchunks;
+        I.img = const_cast<uint8_t*>(U[fwd_image(online[sg], ly)].ptr);
+        I.img_t = const_cast<uint8_t*>(U[fwd_image(target[sg], ly)].ptr);
       }
     }
   }
   aa.w1 = float(1.0 - c.beta1); aa.w2 = float(1.0 - c.beta2); aa.beta2 = float(c.beta2); aa.eps = float(c.adam_eps);
-  aa.tau = float(c.tau); aa.one_minus_tau = float(1.0 - c.tau); aa.grad_scale = 1.0f; aa.clock = w.clock;
-  aa.pipe_slot = pf ? par : -1;
+  aa.tau = float(c.tau); aa.one_minus_tau = float(1.0 - c.tau); aa.grad_scale = 1.0f; aa.clock = x.w.clock;
+  aa.pipe_slot = x.pf ? x.par : -1;
   // tail slice of the same launch: reported batch-mean losses + advance the device clock
-  aa.loss_rows = w.loss_rows; aa.pi_rows = w.pi_rows; aa.B = B; aa.inv_count = 1.0f / float(B); aa.loss_out = b.losses;
-  if (h7) {
-    // ---- post-update-critic plan, second half ---------------------------------------------------------------------
-    AdamArgs ac = aa;                                            // critic update alone (writes the critic's forward images too)
-    ac.seg[0] = aa.seg[1]; ac.nseg = 1; ac.skip_tail = 1;
-    RUN(launch_adam(ac, st));
-    RUN(launch_tcc_pack(L->tcc_pack_dx, st));                    // transposed images of the UPDATED critic for the policy backward
-    TccCtx cx{L, &w, &da, &dc, Wa, Wat, Wc, Wct, B, S, A, N, Sp, Ap, Np};
-    TccArgs& fb = L->tcc_fwd_args;
-    tcc_args_begin(fb, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); fb.step_slot = 1;
-    tcc_build_Q(fb, 0, cx, w.out[3], nullptr, w.h2[4], w.h3[4], w.out[4]);      // critic(s, actor(s)) with the new critic weights
-    RUN(launch_mlp_tc_chain(fb, st));
-    HeadsArgs hp = ha;
-    hp.pi_logits = w.out[4]; hp.only_policy = 1; hp.sampler_clock = nullptr;
-    MogArgs mp = ma;
-    mp.pi_raw = w.out[4]; mp.only_policy = 1; mp.sampler_clock = nullptr;
-    QrArgs qp = qa;
-    qp.pi_q = w.out[4]; qp.only_policy = 1; qp.sampler_clock = nullptr;
-    if (mog) RUN(launch_mog_heads(mp, st));
-    else if (qr) RUN(launch_qr_heads(qp, st));
-    else RUN(launch_heads(hp, c.proj_mode, st));
-    TccArgs& bb = L->tcc_bwd_args;
-    tcc_args_begin(bb, B, reinterpret_cast<uint8_t*>(w.xchg), c.precision == 1 ? 3 : 1); bb.step_slot = 5;
-    tcc_build_bwd_P(bb, 0, cx);
-    RUN(launch_mlp_tc_chain(bb, st));
-    GemmWideBatch& gw = L->dw_batch;
-    gemm_wide_begin(gw, nullptr);
-    gemm_wide_add(gw, gemm_dw(w.a_dz22, H, w.h2[3], H, Ga + da.w_off[2], la[2], Ga + da.b_off[2], H, H, B));
-    gemm_wide_add(gw, gemm_dw(w.a_dh2, H, w.h1[3], H, Ga + da.w_off[1], la[1], Ga + da.b_off[1], H, H, B));
-    gemm_wide_add(gw, gemm_dw(w.a_dz3, Ap, w.h3[3], H, Ga + da.w_off[3], la[3], Ga + da.b_off[3], A, H, B));
-    gemm_wide_add(gw, gemm_dw(w.a_dz1, H, w.s, Sp, Ga + da.w_off[0], la[0], Ga + da.b_off[0], H, S, B));
-    RUN(gemm_wide_launch(gw, st));
-    AdamArgs ab = aa;                                            // actor update + the step's tail (loss means, clock)
-    ab.nseg = 1;
-    RUN(launch_adam(ab, st));
-  } else RUN(launch_adam(aa, st));
-  if (c.prioritized || pf) D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_join, 0));
-#undef LEVEL
-#undef RUN
-  L->kernels_per_step = nk;
+  aa.loss_rows = x.w.loss_rows; aa.pi_rows = x.w.pi_rows; aa.B = x.B; aa.inv_count = 1.0f / float(x.B); aa.loss_out = b.losses;
+  return aa;
+}
+// the second half of a post-update-critic step: the critic's Adam, then the policy pass through the updated critic
+static int post_update_half(Step& x, const AdamArgs& aa) {
+  d4pg_learner* L = x.L; const Workspace& w = x.w;
+  AdamArgs ac = aa;                                            // critic update alone (writes the critic's forward images too)
+  ac.seg[0] = aa.seg[1]; ac.nseg = 1; ac.skip_tail = 1;
+  RUN("launch_adam", false, launch_adam(ac, x.st));
+  RUN("launch_tcc_pack", false, launch_tcc_pack(L->tcc_pack_dx, x.st));   // transposed images of the UPDATED critic for the policy backward
+  TccArgs& fb = L->tcc_fwd_args;
+  tcc_begin(x, fb, 1);
+  tcc_build_Q(fb, 0, x, w.out[3], nullptr, w.h2[4], w.h3[4], w.out[4]);      // critic(s, actor(s)) with the new critic weights
+  RUN("launch_mlp_tc_chain", true, launch_mlp_tc_chain(fb, x.st));
+  if (int rc = launch_step_heads(x, true)) return rc;
+  TccArgs& bb = L->tcc_bwd_args;
+  tcc_begin(x, bb, 5);
+  tcc_build_bwd_P(bb, 0, x);
+  RUN("launch_mlp_tc_chain", true, launch_mlp_tc_chain(bb, x.st));
+  if (int rc = dw_wide(x, false, true)) return rc;
+  AdamArgs ab = aa;                                            // actor update + the step's tail (loss means, clock)
+  ab.nseg = 1;
+  RUN("launch_adam", false, launch_adam(ab, x.st));
   return D4PG_OK;
 }
+
+// 7'. one launch for both networks, or the two half steps of the post-update plan
+static int update(Step& x) {
+  const AdamArgs aa = adam_args(x);
+  if (x.h7) return post_update_half(x, aa);
+  RUN("launch_adam", false, launch_adam(aa, x.st));
+  return D4PG_OK;
+}
+
+// par: half of the double-buffered batch this step trains on; cold: sample it first (no valid prefetch)
+// pack_fwd: re-pack the forward weight images first (start of a graph launch / eager step: the caller may have changed
+// the parameters); later steps of one multi-step graph rely on the images the previous step's Adam kernel wrote
+static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bool pack_fwd) {
+  const d4pg_learner_config_t& c = L->cfg;
+  const bool pf = piped(c);
+  Step x{L, st, c, L->buf, L->ws, L->ws.batch[par], par, cold, pf, (c.loss_flags & 4) != 0,
+         c.batch, c.obs_dim, c.act_dim, c.n_atoms, pitch4(c.obs_dim), pitch4(c.act_dim), pitch4(c.n_atoms)};
+  const StepPlan plan = L->plan;
+  const bool side = c.prioritized || pf;                         // the step has a side branch
+  int rc = (!pf || cold) ? sample_batch(x) : D4PG_OK;
+  if (!rc) rc = plan == PLAN_TC_CHAIN ? forward_tc_chain(x, pack_fwd) : plan == PLAN_CHAIN ? forward_chain(x) : forward_levels(x);
+  if (!rc) rc = launch_step_heads(x, false);
+  if (!rc && side) rc = side_branch(x);
+  if (!rc) rc = choose_gradient_buffers(x);
+  if (!rc && plan == PLAN_TC_CHAIN) rc = backward_tc_chain(x);
+  if (!rc && plan == PLAN_CHAIN) rc = backward_chain(x);
+  if (!rc) rc = plan == PLAN_LEVELS ? backward_levels(x) : dw_wide(x, true, !x.h7);
+  if (!rc) rc = exchange_gradients(x);
+  if (!rc) rc = update(x);
+  if (rc) return rc;
+  if (side) D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_join, 0));
+  L->kernels_per_step = x.nk;
+  return D4PG_OK;
+}
+#undef RUN
 
 extern "C" int64_t d4pg_learner_workspace_floats(const d4pg_learner_config_t* cfg) {
   if (!cfg) return -1;
@@ -833,6 +912,9 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
     delete L; return D4PG_EINVAL;
   }
   L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec));
+  if (!piped(ec)) { L->ws.batch[0].idx = buf->idx; L->ws.batch[0].wts = buf->weights; }   // sampled straight into the caller's buffers
+  L->clock_params = ClockParams{ec.lr_actor, ec.lr_critic, ec.beta1, ec.beta2, ec.per_beta0, ec.per_beta_final,
+                                ec.per_beta_iters > 0 ? ec.per_beta_iters : 1};
   for (int i = 0; i < 4; ++i) { L->graph_exec[i] = nullptr; L->graph_ready[i] = false; }
   for (int i = 0; i < 2; ++i) { L->multi_exec[i] = nullptr; L->multi_ready[i] = false; }
   L->pipe_par = 0; L->last_par = 0; L->prefetch_valid = false; L->seen_gen = -1;
@@ -921,62 +1003,72 @@ static void commit_variant(d4pg_learner* L, int par) {
   L->last_par = par; L->pipe_par = par ^ 1; L->prefetch_valid = true; L->seen_gen = replay_generation(L->replay);
 }
 
-static int launch_variant(d4pg_learner* L, cudaStream_t st, int par, bool cold);
+// adds issued on the ingest stream come before the step
+static int wait_for_ingest(d4pg_learner* L, cudaStream_t st) {
+  if (!L->ing) return D4PG_OK;
+  D4PG_CUDA_OK(cudaEventRecord(L->ev_ing, L->ing));
+  D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_ing, 0));
+  return D4PG_OK;
+}
+
+// capture what `body` enqueues on `st` into an executable graph
+template <class F>
+static int capture_graph(cudaStream_t st, cudaGraphExec_t* exec, const char* what, F body) {
+  D4PG_REQUIRE(st != nullptr, D4PG_EINVAL, "%s: graph capture needs a non-default stream", what);
+  cudaGraph_t graph = nullptr;
+  D4PG_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  const int rc = body();
+  cudaError_t e = cudaStreamEndCapture(st, &graph);
+  if (rc != D4PG_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
+  if (e != cudaSuccess) { set_error("%s: end capture: %s", what, cudaGetErrorString(e)); return D4PG_ECUDA; }
+  e = cudaGraphInstantiate(exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (e != cudaSuccess) { set_error("%s: instantiate: %s", what, cudaGetErrorString(e)); return D4PG_ECUDA; }
+  return D4PG_OK;
+}
+
+// one step of variant (par, cold) enqueued directly on `st`; arms the ingest gate of the next step
+static int step_eager(d4pg_learner* L, cudaStream_t st, int par, bool cold) {
+  // warm host-pipeline variants start from a sampled batch AND packed forward images (d4pg_learner_step_host packs
+  // eagerly on the learner stream while the ingest stream still samples)
+  const int rc = enqueue_step(L, st, par, cold, !(host_pipe(L->cfg) && !cold));
+  if (rc == D4PG_OK) { commit_variant(L, par); if (L->ing) replay_arm_gate(L->replay); }
+  return rc;
+}
+
+// the step graph of variant (par, cold) on `st` (captured on first use); arms the ingest gate of the next step
+static int launch_variant(d4pg_learner* L, cudaStream_t st, int par, bool cold) {
+  if (!L->cfg.use_graph) return step_eager(L, st, par, cold);
+  // without the prefetch pipeline the only per-step variation is the gradient half of the peer exchange
+  const int v = piped(L->cfg) ? par * 2 + (cold ? 1 : 0) : int(L->steps_done & 1);
+  if (!L->graph_ready[v]) {
+    const int rc = capture_graph(st, &L->graph_exec[v], "d4pg_learner_step",
+                                 [&] { return enqueue_step(L, st, par, cold, !(host_pipe(L->cfg) && !cold)); });
+    if (rc) return rc;
+    L->graph_ready[v] = true;
+  }
+  D4PG_CUDA_OK(cudaGraphLaunch(L->graph_exec[v], st));
+  commit_variant(L, par);
+  if (L->ing) replay_arm_gate(L->replay);
+  return D4PG_OK;
+}
 
 extern "C" int32_t d4pg_learner_step(d4pg_learner_t* L, d4pg_stream_t stream) {
   D4PG_REQUIRE(L, D4PG_EINVAL, "d4pg_learner_step: null handle");
   cudaStream_t st = as_stream(stream);
   int par; bool cold;
   next_variant(L, &par, &cold);
-  if (L->ing) {                                      // adds issued on the ingest stream come first
-    D4PG_CUDA_OK(cudaEventRecord(L->ev_ing, L->ing));
-    D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_ing, 0));
-  }
+  if (int rc = wait_for_ingest(L, st)) return rc;
   return launch_variant(L, st, par, cold);
-}
-
-// the step graph of variant (par, cold) on `st` (captured on first use); arms the ingest gate of the next step
-static int launch_variant(d4pg_learner* L, cudaStream_t st, int par, bool cold) {
-  auto arm_gate = [&] { if (L->ing) replay_arm_gate(L->replay); };
-  if (!L->cfg.use_graph) {
-    int rc = enqueue_step(L, st, par, cold, !(host_pipe(L->cfg) && !cold));
-    if (rc == D4PG_OK) { commit_variant(L, par); arm_gate(); }
-    return rc;
-  }
-  // without the prefetch pipeline the only per-step variation is the gradient half of the peer exchange
-  const int v = piped(L->cfg) ? par * 2 + (cold ? 1 : 0) : int(L->steps_done & 1);
-  if (!L->graph_ready[v]) {
-    D4PG_REQUIRE(st != nullptr, D4PG_EINVAL, "d4pg_learner_step: graph capture needs a non-default stream");
-    cudaGraph_t graph = nullptr;
-    D4PG_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    // warm host-pipeline variants start from a sampled batch AND packed forward images (d4pg_learner_step_host packs
-    // eagerly on the learner stream while the ingest stream still samples)
-    int rc = enqueue_step(L, st, par, cold, !(host_pipe(L->cfg) && !cold));
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    if (rc != D4PG_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) { set_error("d4pg_learner_step: end capture: %s", cudaGetErrorString(e)); return D4PG_ECUDA; }
-    e = cudaGraphInstantiate(&L->graph_exec[v], graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { set_error("d4pg_learner_step: instantiate: %s", cudaGetErrorString(e)); return D4PG_ECUDA; }
-    L->graph_ready[v] = true;
-  }
-  D4PG_CUDA_OK(cudaGraphLaunch(L->graph_exec[v], st));
-  commit_variant(L, par);
-  arm_gate();
-  return D4PG_OK;
 }
 
 // host pipeline: sample + gather batch `par` from the device copy of this step's uniforms / positions (the launch the
 // cold graph variant starts with, issued on the ingest stream instead)
 static int presample(d4pg_learner* L, int par, const double* uniforms, const int32_t* positions, cudaStream_t st) {
-  const d4pg_learner_config_t& c = L->cfg; const d4pg_learner_buffers_t& b = L->buf; const Workspace& o = L->ws;
-  const ClockParams cp{c.lr_actor, c.lr_critic, c.beta1, c.beta2, c.per_beta0, c.per_beta_final,
-                       c.per_beta_iters > 0 ? c.per_beta_iters : 1};
-  (void)b;
+  const d4pg_learner_config_t& c = L->cfg; const Workspace& w = L->ws; const Batch& o = w.batch[par];
   return learner_sample(L->replay, c.batch, c.prioritized, uniforms, !c.prioritized ? positions : nullptr, c.philox_seed,
-                        o.clock, cp, o.idx2[par], o.wts2[par], par ? o.s_b : o.s, par ? o.a_b : o.a, par ? o.r_b : o.r,
-                        par ? o.s2_b : o.s2, par ? o.done_b : o.done, pitch4(c.obs_dim), pitch4(c.act_dim), par, st,
-                        /*dependent=*/true, o.pipe_epoch);
+                        w.clock, L->clock_params, o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, pitch4(c.obs_dim),
+                        pitch4(c.act_dim), par, st, /*dependent=*/true, w.pipe_epoch);
 }
 
 // The host-facing step: stage this step's host inputs in pinned memory, H2D, the step, order the caller after it.
@@ -1019,8 +1111,7 @@ static int step_host_common(d4pg_learner_t* L, const double* uniforms, const uin
   if (pipe) {
     // batch k on the ingest stream: behind the caller's add(k) (same stream) and the gate of step k-1, while step k-1's
     // backward pass / dW / Adam still run on the learner stream; the step graph starts from the sampled batch
-    int bpar; bool cold_unused;
-    next_variant(L, &bpar, &cold_unused);
+    const int bpar = L->pipe_par;
     rc = replay_gate_consume(L->replay, L->ing);
     if (rc) return rc;
     rc = presample(L, bpar, du, dpos, L->ing);
@@ -1094,16 +1185,12 @@ extern "C" int32_t d4pg_learner_run(d4pg_learner_t* L, int32_t n_steps, d4pg_str
     next_variant(L, &par, &cold);
     if (L->cfg.use_graph && prefetching(L->cfg) && !cold && n >= RUN_UNROLL && st != nullptr) {
       if (!L->multi_ready[par]) {
-        cudaGraph_t graph = nullptr;
-        D4PG_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        int rc = D4PG_OK;
-        for (int i = 0; i < RUN_UNROLL && rc == D4PG_OK; ++i) rc = enqueue_step(L, st, par ^ (i & 1), false, i == 0);
-        cudaError_t e = cudaStreamEndCapture(st, &graph);
-        if (rc != D4PG_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (e != cudaSuccess) { set_error("d4pg_learner_run: end capture: %s", cudaGetErrorString(e)); return D4PG_ECUDA; }
-        e = cudaGraphInstantiate(&L->multi_exec[par], graph, 0);
-        cudaGraphDestroy(graph);
-        if (e != cudaSuccess) { set_error("d4pg_learner_run: instantiate: %s", cudaGetErrorString(e)); return D4PG_ECUDA; }
+        const int rc = capture_graph(st, &L->multi_exec[par], "d4pg_learner_run", [&] {
+          int rc = D4PG_OK;
+          for (int i = 0; i < RUN_UNROLL && rc == D4PG_OK; ++i) rc = enqueue_step(L, st, par ^ (i & 1), false, i == 0);
+          return rc;
+        });
+        if (rc) return rc;
         L->multi_ready[par] = true;
       }
       D4PG_CUDA_OK(cudaGraphLaunch(L->multi_exec[par], st));
@@ -1122,13 +1209,12 @@ extern "C" int32_t d4pg_learner_profile_step(d4pg_learner_t* L, d4pg_stream_t st
                                              float* ms_out, char* names_out, int32_t name_stride, int32_t* n_out) {
   D4PG_REQUIRE(L && ms_out && n_out && max_launches > 0, D4PG_EINVAL, "d4pg_learner_profile_step: bad arguments");
   cudaStream_t st = as_stream(stream);
-  L->profiling = true; L->ev.clear(); L->ev_name.clear(); L->ev_reps.clear();
   int par; bool cold;
   next_variant(L, &par, &cold);
-  if (L->ing) { D4PG_CUDA_OK(cudaEventRecord(L->ev_ing, L->ing)); D4PG_CUDA_OK(cudaStreamWaitEvent(st, L->ev_ing, 0)); }
-  int rc = enqueue_step(L, st, par, cold);
+  if (int rc = wait_for_ingest(L, st)) return rc;
+  L->profiling = true; L->ev.clear(); L->ev_name.clear(); L->ev_reps.clear();
+  const int rc = step_eager(L, st, par, cold);
   L->profiling = false;
-  if (rc == D4PG_OK) { commit_variant(L, par); if (L->ing) replay_arm_gate(L->replay); }
   cudaError_t e = cudaStreamSynchronize(st);
   const int n = int(L->ev_name.size());
   *n_out = n < max_launches ? n : max_launches;
@@ -1173,13 +1259,12 @@ extern "C" int32_t d4pg_learner_set_counters(d4pg_learner_t* L, int64_t adam_ste
 
 extern "C" int32_t d4pg_learner_tensor(d4pg_learner_t* L, const char* name, void** ptr, int64_t* count, int32_t* ld) {
   D4PG_REQUIRE(L && name && ptr && count && ld, D4PG_EINVAL, "d4pg_learner_tensor: null argument");
-  Workspace w = L->ws;
-  if (piped(L->cfg) && L->last_par) { w.s = w.s_b; w.a = w.a_b; w.s2 = w.s2_b; w.r = w.r_b; w.done = w.done_b; }
+  const Workspace& w = L->ws; const Batch& bt = w.batch[L->last_par];     // the half the last step trained on
   const int64_t B = L->cfg.batch;
   const int Sp = pitch4(L->cfg.obs_dim), Ap = pitch4(L->cfg.act_dim), Np = pitch4(L->cfg.n_atoms);
   struct E { const char* n; void* p; int64_t c; int ld; };
   const E table[] = {
-      {"s", w.s, B * Sp, Sp}, {"a", w.a, B * Ap, Ap}, {"r", w.r, B, 1}, {"s2", w.s2, B * Sp, Sp}, {"done", w.done, B, 1},
+      {"s", bt.s, B * Sp, Sp}, {"a", bt.a, B * Ap, Ap}, {"r", bt.r, B, 1}, {"s2", bt.s2, B * Sp, Sp}, {"done", bt.done, B, 1},
       {"target_logits", w.out[1], B * Np, Np}, {"q_logits", w.out[2], B * Np, Np}, {"pi_logits", w.out[4], B * Np, Np},
       {"m", w.m, B * Np, Np}, {"q_probs", w.q_probs, B * Np, Np}, {"target_probs", w.target_probs, B * Np, Np},
       {"dlogits_q", w.dlogits_q, B * Np, Np}, {"dlogits_pi", w.dlogits_pi, B * Np, Np},

@@ -65,13 +65,13 @@ __device__ __forceinline__ MogComp mog_comp(const float* __restrict__ raw, int K
 template <int NT>
 __device__ __forceinline__ void mog_critic_row(const MogArgs& a, int row, int lane) {
   const int K = a.K;
-  const size_t ro = size_t(row) * a.ld;
+  const size_t ro = size_t(row) * a.h.ld;
   const bool on = lane < K;
-  const MogComp t = mog_comp(a.target_raw + ro, K, lane);
-  const MogComp q = mog_comp(a.q_raw + ro, K, lane);
-  const double r = a.rewards[row];
-  const double c = a.dones[row] ? 0.0 : a.discount;
-  const float isw = a.is_weights ? __ldg(a.is_weights + row) : 1.f;
+  const MogComp t = mog_comp(a.h.target + ro, K, lane);
+  const MogComp q = mog_comp(a.h.q + ro, K, lane);
+  const double r = a.h.rewards[row];
+  const double c = a.h.dones[row] ? 0.0 : a.h.discount;
+  const float isw = a.h.is_weights ? __ldg(a.h.is_weights + row) : 1.f;
   const double LOG_2PI = 1.8378770664093453, SQRT2 = 1.4142135623730951, INV_SQRTPI = 0.5641895835477563;
   const double inv_sig = 1.0 / q.sigma;
   const double lc = on ? q.logw - log(q.sigma) - 0.5 * LOG_2PI : -INFINITY;
@@ -123,33 +123,33 @@ __device__ __forceinline__ void mog_critic_row(const MogArgs& a, int row, int la
   }
   const double sum_gl = warp_sum_d(gl);
   const double ev = warp_sum_d(q.w * q.mu), evt = warp_sum_d(t.w * t.mu);
-  const double gscale = double(a.grad_scale) * double(isw);
-  if (on && a.dq_raw) {
-    a.dq_raw[ro + lane] = float((gl - q.w * sum_gl) * gscale);       // softmax Jacobian
-    a.dq_raw[ro + K + lane] = float(gm * gscale);
-    a.dq_raw[ro + 2 * K + lane] = float(gs * q.dsigma * gscale);     // softplus'
+  const double gscale = double(a.h.grad_scale) * double(isw);
+  if (on && a.h.dq) {
+    a.h.dq[ro + lane] = float((gl - q.w * sum_gl) * gscale);       // softmax Jacobian
+    a.h.dq[ro + K + lane] = float(gm * gscale);
+    a.h.dq[ro + 2 * K + lane] = float(gs * q.dsigma * gscale);     // softplus'
   }
   if (lane == 0) {
     const float tdv = float(ev - (r + c * evt));
-    if (a.loss_rows) a.loss_rows[row] = float(loss * double(isw));
-    if (a.td) a.td[row] = tdv;
-    if (a.prio) a.prio[row] = fabsf(tdv) + float(a.prio_eps);
+    if (a.h.loss_rows) a.h.loss_rows[row] = float(loss * double(isw));
+    if (a.h.td) a.h.td[row] = tdv;
+    if (a.h.prio) a.h.prio[row] = fabsf(tdv) + float(a.h.prio_eps);
   }
 }
 
 // policy part of one row: -E[Q] and its raw-head gradient (sigma does not enter)
 __device__ __forceinline__ void mog_policy_row(const MogArgs& a, int row, int lane) {
   const int K = a.K;
-  const size_t ro = size_t(row) * a.ld;
-  const MogComp p = mog_comp(a.pi_raw + ro, K, lane);
+  const size_t ro = size_t(row) * a.h.ld;
+  const MogComp p = mog_comp(a.h.pi + ro, K, lane);
   const double ev = warp_sum_d(p.w * p.mu);
-  const double gsc = double(a.grad_scale);
-  if (lane < K && a.dpi_raw) {
-    a.dpi_raw[ro + lane] = float(-gsc * p.w * (p.mu - ev));
-    a.dpi_raw[ro + K + lane] = float(-gsc * p.w);
-    a.dpi_raw[ro + 2 * K + lane] = 0.f;
+  const double gsc = double(a.h.grad_scale);
+  if (lane < K && a.h.dpi) {
+    a.h.dpi[ro + lane] = float(-gsc * p.w * (p.mu - ev));
+    a.h.dpi[ro + K + lane] = float(-gsc * p.w);
+    a.h.dpi[ro + 2 * K + lane] = 0.f;
   }
-  if (lane == 0 && a.pi_rows) a.pi_rows[row] = float(-ev);
+  if (lane == 0 && a.h.pi_rows) a.h.pi_rows[row] = float(-ev);
 }
 
 // warps [0, B): critic part of row g; [B, 2B): policy part of row g - B (only_policy: warps [0, B) run the policy part).
@@ -158,26 +158,26 @@ __device__ __forceinline__ void mog_policy_row(const MogArgs& a, int row, int la
 // __maxnreg__(255): without it ptxas aims at 64-96 registers and spills the per-point arrays (blocks are 128 threads)
 template <int NT>
 __global__ void __maxnreg__(255) mog_heads_kernel(const MogArgs a) {
-  pdl_trigger(a.pdl);
+  pdl_trigger(a.h.pdl);
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = blockIdx.x * MOG_WARPS + warp;
-  step_stamp(a.trace, 2);
-  if (a.only_policy) { if (g < a.B) mog_policy_row(a, g, lane); }
-  else if (g < a.B) mog_critic_row<NT>(a, g, lane);
-  else if (g < 2 * a.B) mog_policy_row(a, g - a.B, lane);
-  step_stamp(a.trace, 2 + 16);
-  if (a.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
-    a.sampler_clock->s_adam_step += 1; a.sampler_clock->s_beta_t += 1; a.sampler_clock->s_steps_done += 1;
+  step_stamp(a.h.trace, 2);
+  if (a.h.only_policy) { if (g < a.h.B) mog_policy_row(a, g, lane); }
+  else if (g < a.h.B) mog_critic_row<NT>(a, g, lane);
+  else if (g < 2 * a.h.B) mog_policy_row(a, g - a.h.B, lane);
+  step_stamp(a.h.trace, 2 + 16);
+  if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
+    a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;
   }
-  pdl_trigger_end(a.pdl);
+  pdl_trigger_end(a.h.pdl);
 }
 
 int launch_mog_heads(const MogArgs& a_in, cudaStream_t st) {
   MogArgs a = a_in;
-  a.pdl = pdl_mode();
-  a.trace = (a.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
-  dim3 grid(cdiv(((a.pi_raw && !a.only_policy) ? 2 : 1) * a.B, MOG_WARPS)), block(MOG_WARPS * 32);
+  a.h.pdl = pdl_mode();
+  a.h.trace = (a.h.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
+  dim3 grid(cdiv(((a.h.pi && !a.h.only_policy) ? 2 : 1) * a.h.B, MOG_WARPS)), block(MOG_WARPS * 32);
   D4PG_MAX_CARVEOUT(mog_heads_kernel<1>); D4PG_MAX_CARVEOUT(mog_heads_kernel<2>);
   D4PG_MAX_CARVEOUT(mog_heads_kernel<4>); D4PG_MAX_CARVEOUT(mog_heads_kernel<8>);
   // NT = quadrature points per lane: 8K points over 32 lanes
@@ -252,10 +252,10 @@ extern "C" int32_t d4pg_mog_loss(const float* target_raw, const float* q_raw, co
   D4PG_REQUIRE(B > 0 && K >= 1 && K <= D4PG_MAX_COMPONENTS, D4PG_EINVAL,
                "d4pg_mog_loss: need B>0, 1<=K<=%d (got B=%d K=%d)", D4PG_MAX_COMPONENTS, B, K);
   MogArgs a{};
-  a.target_raw = target_raw; a.q_raw = q_raw; a.pi_raw = pi_raw;
-  a.rewards = rewards; a.dones = dones; a.B = B; a.K = K; a.ld = 3 * K;
-  a.discount = discount; a.prio_eps = prio_eps; a.grad_scale = grad_scale;
-  a.loss_rows = loss_rows; a.td = td; a.prio = prio; a.dq_raw = dq_raw; a.pi_rows = pi_rows; a.dpi_raw = dpi_raw;
+  a.h.target = target_raw; a.h.q = q_raw; a.h.pi = pi_raw;
+  a.h.rewards = rewards; a.h.dones = dones; a.h.B = B; a.K = K; a.h.ld = 3 * K;
+  a.h.discount = discount; a.h.prio_eps = prio_eps; a.h.grad_scale = grad_scale;
+  a.h.loss_rows = loss_rows; a.h.td = td; a.h.prio = prio; a.h.dq = dq_raw; a.h.pi_rows = pi_rows; a.h.dpi = dpi_raw;
   return launch_mog_heads(a, as_stream(stream));
 }
 

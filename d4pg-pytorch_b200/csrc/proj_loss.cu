@@ -20,9 +20,9 @@ namespace d4pg {
 
 int launch_heads(const HeadsArgs& a_in, int mode, cudaStream_t st) {
   HeadsArgs a = a_in;
-  a.pdl = pdl_mode();
-  a.trace = (a.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
-  dim3 grid(cdiv(((a.pi_logits && !a.only_policy) ? 2 : 1) * a.B, HEAD_WARPS)), block(HEAD_WARPS * 32);   // policy heads on warps of their own
+  a.h.pdl = pdl_mode();
+  a.h.trace = (a.h.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
+  dim3 grid(cdiv(((a.h.pi && !a.h.only_policy) ? 2 : 1) * a.h.B, HEAD_WARPS)), block(HEAD_WARPS * 32);   // policy heads on warps of their own
   D4PG_MAX_CARVEOUT((heads_kernel<0, 2>)); D4PG_MAX_CARVEOUT((heads_kernel<1, 2>));
   D4PG_MAX_CARVEOUT((heads_kernel<0, 4>)); D4PG_MAX_CARVEOUT((heads_kernel<1, 4>));
   // NT = atom slots per lane: 2 covers N<=64 (51 atoms), 4 covers N<=128 (101 atoms)
@@ -53,14 +53,14 @@ extern "C" int32_t d4pg_proj_loss(const float* target_logits, const float* q_log
   D4PG_REQUIRE((bins_l == nullptr) == (bins_u == nullptr), D4PG_EINVAL, "d4pg_proj_loss: bins_l/bins_u must both be set or both NULL");
   D4PG_REQUIRE(v_max > v_min, D4PG_EINVAL, "d4pg_proj_loss: v_max <= v_min");
   HeadsArgs a{};
-  a.target_logits = target_logits; a.q_logits = q_logits; a.pi_logits = pi_logits;
-  a.rewards = rewards; a.dones = dones; a.B = B; a.N = N; a.flags = flags; a.ld = N;
+  a.h.target = target_logits; a.h.q = q_logits; a.h.pi = pi_logits;
+  a.h.rewards = rewards; a.h.dones = dones; a.h.B = B; a.N = N; a.flags = flags; a.h.ld = N;
   a.v_min = v_min; a.v_max = v_max;
   a.delta = (v_max - v_min) / double(N - 1);        // ddpg.py:46
-  a.discount = discount; a.prio_eps = prio_eps; a.grad_scale = grad_scale;
+  a.h.discount = discount; a.h.prio_eps = prio_eps; a.h.grad_scale = grad_scale;
   a.m = m; a.bins_l = bins_l; a.bins_u = bins_u; a.target_probs = target_probs; a.q_probs = q_probs;
-  a.loss_rows = loss_rows; a.td = td; a.prio = prio; a.dlogits_q = dlogits_q;
-  a.pi_rows = pi_rows; a.dlogits_pi = dlogits_pi;
-  a.is_weights = nullptr; a.ce_priority = 0; a.only_policy = 0;
+  a.h.loss_rows = loss_rows; a.h.td = td; a.h.prio = prio; a.h.dq = dlogits_q;
+  a.h.pi_rows = pi_rows; a.h.dpi = dlogits_pi;
+  a.h.is_weights = nullptr; a.ce_priority = 0; a.h.only_policy = 0;
   return launch_heads(a, proj_mode, as_stream(stream));
 }

@@ -29,10 +29,10 @@ __device__ __forceinline__ double qr_warp_sum(double v) {
 template <int NT>
 __device__ __forceinline__ void qr_critic_row(const QrArgs& a, int row, int lane, double* ys) {
   const int N = a.N;
-  const size_t ro = size_t(row) * a.ld;
-  const double r = a.rewards[row];
-  const double c = a.dones[row] ? 0.0 : a.discount;
-  const float isw = a.is_weights ? __ldg(a.is_weights + row) : 1.f;
+  const size_t ro = size_t(row) * a.h.ld;
+  const double r = a.h.rewards[row];
+  const double c = a.h.dones[row] ? 0.0 : a.h.discount;
+  const float isw = a.h.is_weights ? __ldg(a.h.is_weights + row) : 1.f;
   const double kap = a.kappa;
   double th[NT], tau[NT], g[NT], ls[NT];
   double sum_t = 0.0, sum_q = 0.0;
@@ -40,10 +40,10 @@ __device__ __forceinline__ void qr_critic_row(const QrArgs& a, int row, int lane
   for (int t = 0; t < NT; ++t) {
     const int k = lane + 32 * t;
     const bool on = k < N;
-    const double tp = on ? double(__ldg(a.target_q + ro + k)) : 0.0;
+    const double tp = on ? double(__ldg(a.h.target + ro + k)) : 0.0;
     if (on) ys[k] = r + c * tp;
     sum_t += tp;
-    th[t] = on ? double(__ldg(a.q + ro + k)) : 0.0;
+    th[t] = on ? double(__ldg(a.h.q + ro + k)) : 0.0;
     sum_q += th[t];
     tau[t] = double(2 * k + 1) / double(2 * N);
     g[t] = 0.0; ls[t] = 0.0;
@@ -67,20 +67,20 @@ __device__ __forceinline__ void qr_critic_row(const QrArgs& a, int row, int lane
   for (int t = 0; t < NT; ++t) loss += (lane + 32 * t < N) ? ls[t] : 0.0;
   const double invN = 1.0 / double(N);
   loss = qr_warp_sum(loss) * invN / kap;
-  const double gscale = double(a.grad_scale) * double(isw);
-  if (a.dq) {
+  const double gscale = double(a.h.grad_scale) * double(isw);
+  if (a.h.dq) {
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
       const int k = lane + 32 * t;
-      if (k < N) a.dq[ro + k] = float(-g[t] * invN / kap * gscale);
+      if (k < N) a.h.dq[ro + k] = float(-g[t] * invN / kap * gscale);
     }
   }
   sum_t = qr_warp_sum(sum_t); sum_q = qr_warp_sum(sum_q);
   if (lane == 0) {
     const float tdv = float(sum_q * invN - (r + c * (sum_t * invN)));
-    if (a.loss_rows) a.loss_rows[row] = float(loss * double(isw));
-    if (a.td) a.td[row] = tdv;
-    if (a.prio) a.prio[row] = (a.ce_priority ? float(loss) : fabsf(tdv)) + float(a.prio_eps);
+    if (a.h.loss_rows) a.h.loss_rows[row] = float(loss * double(isw));
+    if (a.h.td) a.h.td[row] = tdv;
+    if (a.h.prio) a.h.prio[row] = (a.ce_priority ? float(loss) : fabsf(tdv)) + float(a.h.prio_eps);
   }
 }
 
@@ -88,23 +88,23 @@ __device__ __forceinline__ void qr_critic_row(const QrArgs& a, int row, int lane
 template <int NT>
 __device__ __forceinline__ void qr_policy_row(const QrArgs& a, int row, int lane) {
   const int N = a.N;
-  const size_t ro = size_t(row) * a.ld;
+  const size_t ro = size_t(row) * a.h.ld;
   double s = 0.0;
 #pragma unroll
   for (int t = 0; t < NT; ++t) {
     const int k = lane + 32 * t;
-    if (k < N) s += double(__ldg(a.pi_q + ro + k));
+    if (k < N) s += double(__ldg(a.h.pi + ro + k));
   }
   s = qr_warp_sum(s);
-  if (a.dpi) {
-    const float gk = float(-double(a.grad_scale) / double(N));
+  if (a.h.dpi) {
+    const float gk = float(-double(a.h.grad_scale) / double(N));
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
       const int k = lane + 32 * t;
-      if (k < N) a.dpi[ro + k] = gk;
+      if (k < N) a.h.dpi[ro + k] = gk;
     }
   }
-  if (lane == 0 && a.pi_rows) a.pi_rows[row] = float(-s / double(N));
+  if (lane == 0 && a.h.pi_rows) a.h.pi_rows[row] = float(-s / double(N));
 }
 
 // warps [0, B): critic part of row g; [B, 2B): policy part of row g - B (only_policy: warps [0, B) run the policy part).
@@ -113,26 +113,26 @@ __device__ __forceinline__ void qr_policy_row(const QrArgs& a, int row, int lane
 template <int NT>
 __global__ void __launch_bounds__(QR_WARPS * 32) qr_heads_kernel(const QrArgs a) {
   __shared__ double ys[QR_WARPS][32 * NT];
-  pdl_trigger(a.pdl);
+  pdl_trigger(a.h.pdl);
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = blockIdx.x * QR_WARPS + warp;
-  step_stamp(a.trace, 2);
-  if (a.only_policy) { if (g < a.B) qr_policy_row<NT>(a, g, lane); }
-  else if (g < a.B) qr_critic_row<NT>(a, g, lane, ys[warp]);
-  else if (g < 2 * a.B) qr_policy_row<NT>(a, g - a.B, lane);
-  step_stamp(a.trace, 2 + 16);
-  if (a.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
-    a.sampler_clock->s_adam_step += 1; a.sampler_clock->s_beta_t += 1; a.sampler_clock->s_steps_done += 1;
+  step_stamp(a.h.trace, 2);
+  if (a.h.only_policy) { if (g < a.h.B) qr_policy_row<NT>(a, g, lane); }
+  else if (g < a.h.B) qr_critic_row<NT>(a, g, lane, ys[warp]);
+  else if (g < 2 * a.h.B) qr_policy_row<NT>(a, g - a.h.B, lane);
+  step_stamp(a.h.trace, 2 + 16);
+  if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
+    a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;
   }
-  pdl_trigger_end(a.pdl);
+  pdl_trigger_end(a.h.pdl);
 }
 
 int launch_qr_heads(const QrArgs& a_in, cudaStream_t st) {
   QrArgs a = a_in;
-  a.pdl = pdl_mode();
-  a.trace = (a.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
-  dim3 grid(cdiv(((a.pi_q && !a.only_policy) ? 2 : 1) * a.B, QR_WARPS)), block(QR_WARPS * 32);
+  a.h.pdl = pdl_mode();
+  a.h.trace = (a.h.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
+  dim3 grid(cdiv(((a.h.pi && !a.h.only_policy) ? 2 : 1) * a.h.B, QR_WARPS)), block(QR_WARPS * 32);
   D4PG_MAX_CARVEOUT(qr_heads_kernel<1>); D4PG_MAX_CARVEOUT(qr_heads_kernel<2>);
   D4PG_MAX_CARVEOUT(qr_heads_kernel<3>); D4PG_MAX_CARVEOUT(qr_heads_kernel<4>);
   // NT = quantiles per lane
@@ -156,10 +156,10 @@ extern "C" int32_t d4pg_qr_loss(const float* target_q, const float* q, const flo
                "d4pg_qr_loss: need B>0, 2<=N<=%d (got B=%d N=%d)", D4PG_MAX_ATOMS, B, N);
   D4PG_REQUIRE(std::isfinite(kappa) && kappa > 0.0, D4PG_EINVAL, "d4pg_qr_loss: kappa must be finite and > 0 (got %g)", kappa);
   QrArgs a{};
-  a.target_q = target_q; a.q = q; a.pi_q = pi_q;
-  a.rewards = rewards; a.dones = dones; a.B = B; a.N = N; a.ld = N;
-  a.discount = discount; a.kappa = kappa; a.prio_eps = prio_eps; a.grad_scale = grad_scale;
+  a.h.target = target_q; a.h.q = q; a.h.pi = pi_q;
+  a.h.rewards = rewards; a.h.dones = dones; a.h.B = B; a.N = N; a.h.ld = N;
+  a.h.discount = discount; a.kappa = kappa; a.h.prio_eps = prio_eps; a.h.grad_scale = grad_scale;
   a.ce_priority = ce_priority ? 1 : 0;
-  a.loss_rows = loss_rows; a.td = td; a.prio = prio; a.dq = dq; a.pi_rows = pi_rows; a.dpi = dpi;
+  a.h.loss_rows = loss_rows; a.h.td = td; a.h.prio = prio; a.h.dq = dq; a.h.pi_rows = pi_rows; a.h.dpi = dpi;
   return launch_qr_heads(a, as_stream(stream));
 }
