@@ -162,6 +162,19 @@ def assert_tree_close_and_sync(buf, want_sum, want_min, max_mismatch_frac=0.01):
     return mism
 
 
+def philox_uniform53(seed, counter, lane):
+    """Host restatement of Philox::uniform53 (csrc/common.cuh): Philox4x32-10, counter (lo, hi, lane, 0x9E3779B9),
+    key = seed; 53-bit uniform built like CPython's random.random() from two 32-bit outputs."""
+    M0, M1, MASK = 0xD2511F53, 0xCD9E8D57, 0xFFFFFFFF
+    c = [counter & MASK, (counter >> 32) & MASK, lane & MASK, 0x9E3779B9]
+    k0, k1 = seed & MASK, (seed >> 32) & MASK
+    for _ in range(10):
+        p0, p1 = M0 * c[0], M1 * c[2]
+        c = [((p1 >> 32) ^ c[1] ^ k0) & MASK, p1 & MASK, ((p0 >> 32) ^ c[3] ^ k1) & MASK, p0 & MASK]
+        k0, k1 = (k0 + 0x9E3779B9) & MASK, (k1 + 0xBB67AE85) & MASK
+    return ((c[0] >> 5) * 67108864.0 + (c[1] >> 6)) * (1.0 / 9007199254740992.0)
+
+
 def rel_l2(mine, ref):
     mine, ref = np.asarray(mine, np.float64).reshape(-1), np.asarray(ref, np.float64).reshape(-1)
     return float(np.linalg.norm(mine - ref) / max(np.linalg.norm(ref), 1e-30))
