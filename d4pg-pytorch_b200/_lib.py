@@ -47,6 +47,8 @@ class LearnerConfig(C.Structure):
         ("loss_flags", C.c_int32), ("chain", C.c_int32), ("prefetch", C.c_int32),
         ("dist_type", C.c_int32), ("n_components", C.c_int32),
         ("qr_kappa", C.c_double),
+        ("max_grad_norm_actor", C.c_double), ("max_grad_norm_critic", C.c_double),
+        ("weight_decay_actor", C.c_double), ("weight_decay_critic", C.c_double),
     ]
 
 
@@ -109,6 +111,8 @@ _PROTOS = {
                                              _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_adam_polyak": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
                                      C.c_int64, C.c_double, C.c_float, _P]),
+    "d4pg_adam_polyak_ex": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
+                                        C.c_int64, C.c_double, C.c_float, _P, C.c_double, C.c_double, _P, _P]),
     "d4pg_polyak": (C.c_int32, [_P, _P, C.c_int64, C.c_double, _P]),
     "d4pg_copy_f32": (C.c_int32, [_P, _P, C.c_int64, _P]),
     "d4pg_learner_workspace_floats": (C.c_int64, [C.POINTER(LearnerConfig)]),

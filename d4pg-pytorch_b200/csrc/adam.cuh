@@ -110,6 +110,11 @@ struct AdamSeg {
   float* g_out; int64_t g_off;                 // peer mode: the summed gradient is also stored here; offset in the exchange half
   float neg_step_size; int clock_slot;        // clock_slot >= 0: read -step_size from the device clock
   AdamImgLayer imgl[4]; int nimg;              // nimg = 0: no images
+  // global-norm clipping (sq_partials non-null) and Adam weight decay (wd != 0); both off: the plain update
+  const double* sq_partials;                   // GRAD_NORM_CTAS fp64 partial sums of g^2 over this segment (grad_sqnorm_kernel)
+  double max_norm;                             // clipping threshold; +inf: measure and report only
+  float* norm_out;                             // optional: float32 of the segment's gradient norm
+  float wd;                                    // the effective gradient is coef * g + wd * p (p = pre-update value)
 };
 struct AdamArgs {
   AdamSeg seg[2]; int nseg;
@@ -132,6 +137,19 @@ struct AdamArgs {
   int skip_tail;                              // 1: no loss means / clock advance in this launch (first of two Adam launches of a step)
 };
 int launch_adam(const AdamArgs& a, cudaStream_t st);
+
+// Sum of squares of each segment's gradient, ahead of a clipping Adam launch: a FIXED grid of GRAD_NORM_CTAS CTAs per
+// segment (not sized by the SM count, so the summation order belongs to the build, not to the card), fp64 accumulation,
+// one fp64 partial per CTA into seg.sq_partials, no atomics.  The Adam kernel sums the partials in a fixed order.
+constexpr int GRAD_NORM_CTAS = 64;
+constexpr double GRAD_NORM_EPS = 1e-6;         // torch.nn.utils.clip_grad_norm_: coef = max_norm / (norm + 1e-6)
+struct GradNormArgs { const float* g[2]; double* partials[2]; int64_t n[2]; int nseg; int pdl; };
+static inline bool adam_clips(const AdamArgs& a) {
+  for (int i = 0; i < a.nseg; ++i) if (a.seg[i].sq_partials) return true;
+  return false;
+}
+// the norm launch of the segments of `a` that clip (reads the gradient the Adam launch will read)
+int launch_grad_sqnorm(const AdamArgs& a, cudaStream_t st);
 
 
 }  // namespace d4pg

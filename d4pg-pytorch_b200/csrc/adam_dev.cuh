@@ -28,9 +28,35 @@ __device__ __forceinline__ void adam_tail(const AdamArgs& a, float (*red)[8]) {
   if (threadIdx.x == 0 && a.clock) { a.clock->adam_step += 1; a.clock->beta_t += 1; a.clock->steps_done += 1; }
 }
 
-// segment `seg`, grid-stride over float4 groups: CTA bx of gx (256 threads each)
-__device__ __forceinline__ void adam_segment(const AdamArgs& a, int seg, int bx, int gx) {
+// fp64 sum over a warp, every lane holding the same bits (fp add commutes, so both sides of each exchange agree)
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Clipping coefficient of segment `s` from the GRAD_NORM_CTAS partial sums grad_sqnorm_kernel left: warp 0 sums them in
+// a fixed order and broadcasts through shared memory, so every CTA of the launch derives the same bits and no grid-wide
+// synchronisation is needed.  norm = |scale| * sqrt(sum g^2) is the norm of the scaled gradient;
+// coef = scale * min(1, max_norm / (norm + 1e-6)) formed in fp64 and cast once: exactly `scale` when nothing is clipped.
+__device__ __forceinline__ float clip_coef(const AdamSeg& s, float scale, bool report, double* bcast) {
+  if (threadIdx.x < 32) {
+    const double sq = warp_sum_f64(s.sq_partials[threadIdx.x] + s.sq_partials[threadIdx.x + 32]);
+    if (threadIdx.x == 0) *bcast = fabs(double(scale)) * sqrt(sq);
+  }
+  __syncthreads();
+  const double norm = *bcast;
+  if (report && threadIdx.x == 0 && s.norm_out) *s.norm_out = float(norm);
+  return float(double(scale) * fmin(1.0, s.max_norm / (norm + GRAD_NORM_EPS)));
+}
+
+// segment `seg`, grid-stride over float4 groups: CTA bx of gx (256 threads each).  EX: the launch clips to a global norm
+// and / or applies weight decay (a separate instantiation, so the plain update keeps its instructions)
+template <bool EX>
+__device__ __forceinline__ void adam_segment(const AdamArgs& a, int seg, int bx, int gx, double* bcast = nullptr) {
   const AdamSeg& s = a.seg[seg];
+  float coef = a.grad_scale;
+  if (EX && s.sq_partials) coef = clip_coef(s, a.grad_scale, bx == 0, bcast);
   float nss = s.neg_step_size, bc2s = a.bc2_sqrt;
   if (a.clock) {
     if (a.pipe_slot >= 0) {
@@ -73,7 +99,11 @@ __device__ __forceinline__ void adam_segment(const AdamArgs& a, int seg, int bx,
     float* pp = &p.x; float* gg = &g.x; float* mm = &m.x; float* vv = &v.x; float* tt = &t.x;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      const float gr = gg[c] * a.grad_scale;
+      float gr;
+      if (EX) {
+        gr = __fmul_rn(gg[c], coef);
+        if (s.wd != 0.f) gr = __fadd_rn(gr, __fmul_rn(s.wd, pp[c]));
+      } else gr = gg[c] * a.grad_scale;
       mm[c] = fmaf(a.w1, gr - mm[c], mm[c]);                                   // lerp, weight < 0.5
       vv[c] = __fadd_rn(__fmul_rn(vv[c], a.beta2), __fmul_rn(__fmul_rn(a.w2, gr), gr));
       const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv[c]), bc2s), a.eps);

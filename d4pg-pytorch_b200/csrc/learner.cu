@@ -15,6 +15,7 @@
 //   ddpg.py:236-243 policy backward           -> uses the PRE-update critic weights (SURVEY.md H7):
 //                                                both backward passes run before any Adam update
 //   ddpg.py:232,244,247,250 Adam x2, sync, Polyak -> exchange_gradients, then one fused adam_polyak_kernel (2 segments)
+//   (no reference line) max_grad_norm        -> launch_update: grad_sqnorm_kernel before each Adam launch, only when configured
 #include "common.cuh"
 #include "gemm_ffma.cuh"
 #include "adam.cuh"
@@ -47,6 +48,7 @@ struct Workspace {
   LearnerClock* clock;
   float* xchg;                     // exchange planes of the cluster-fused chain kernels (chain mode)
   unsigned long long* pipe_epoch;  // host pipeline: per-CTA completion epochs of the presample kernel (polled by the forward chains)
+  double* sq_partials;             // [2][GRAD_NORM_CTAS] partial sums of g^2 (actor, critic); only when a network clips
   int64_t total;
 };
 
@@ -78,7 +80,7 @@ static_assert((CHAIN_MAX_BATCH + SAMPLE_ROWS - 1) / SAMPLE_ROWS <= TCC_THREADS, 
 
 // Every 2-D plane has a row pitch that is a multiple of 4 floats (16-B rows): |s|=17 -> 20,
 // |a|=6 -> 8, N=51 -> 52.  That makes every GEMM operand TMA- and float4-addressable.
-static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, bool prefetch) {
+static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, bool prefetch, bool clip) {
   Workspace w{};
   int64_t off = 0;
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += align4(n); return p; };
@@ -109,6 +111,7 @@ static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, b
     take_rows(w.batch[1]);
     for (int k = 0; k < 2; ++k) { w.batch[k].idx = reinterpret_cast<int32_t*>(take(B)); w.batch[k].wts = take(B); }
   }
+  if (clip) w.sq_partials = reinterpret_cast<double*>(take(2 * GRAD_NORM_CTAS * 2));
   w.total = off;
   return w;
 }
@@ -171,6 +174,8 @@ static bool prefetching(const d4pg_learner_config_t& c) { return c.prefetch != 0
 // (update_priorities(k-1) -> add(k) -> sample(k), main.py / ddpg.py:200-255).
 static bool host_pipe(const d4pg_learner_config_t& c) { return c.prefetch != 0 && c.sample_mode == 0 && c.use_graph != 0; }
 static bool piped(const d4pg_learner_config_t& c) { return prefetching(c) || host_pipe(c); }
+// some network's gradient is clipped to (or measured against) a global norm: the step has a norm launch before each Adam
+static bool clipping(const d4pg_learner_config_t& c) { return c.max_grad_norm_actor != 0.0 || c.max_grad_norm_critic != 0.0; }
 
 // ---- the layers ---------------------------------------------------------------------------------------------------
 enum Net { ACTOR, ACTOR_TARGET, CRITIC, CRITIC_TARGET };
@@ -783,6 +788,13 @@ static AdamArgs adam_args(const Step& x) {
     }
   }
   aa.nseg = 2;
+  aa.seg[0].wd = float(c.weight_decay_actor); aa.seg[1].wd = float(c.weight_decay_critic);
+  const double max_norm[2] = {c.max_grad_norm_actor, c.max_grad_norm_critic};
+  for (int sg = 0; sg < 2; ++sg)
+    if (max_norm[sg] != 0.0) {                                  // its norm goes to losses[2] (actor) / losses[3] (critic)
+      aa.seg[sg].sq_partials = x.w.sq_partials + sg * GRAD_NORM_CTAS; aa.seg[sg].max_norm = max_norm[sg];
+      aa.seg[sg].norm_out = b.losses + 2 + sg;
+    }
   if (L->plan == PLAN_TC_CHAIN) {                               // keep the forward weight images of the tensor-core chains current
     const TccImage* U = L->tcc_img;
     const NetDims* nd[2] = {&da, &dc};
@@ -805,12 +817,18 @@ static AdamArgs adam_args(const Step& x) {
   aa.loss_rows = x.w.loss_rows; aa.pi_rows = x.w.pi_rows; aa.B = x.B; aa.inv_count = 1.0f / float(x.B); aa.loss_out = b.losses;
   return aa;
 }
+// An Adam launch; when a segment of it clips, the sum of squares of that segment's complete gradient right before it
+static int launch_update(Step& x, const AdamArgs& a) {
+  if (adam_clips(a)) RUN("launch_grad_sqnorm", true, launch_grad_sqnorm(a, x.st));
+  RUN("launch_adam", false, launch_adam(a, x.st));
+  return D4PG_OK;
+}
 // the second half of a post-update-critic step: the critic's Adam, then the policy pass through the updated critic
 static int post_update_half(Step& x, const AdamArgs& aa) {
   d4pg_learner* L = x.L; const Workspace& w = x.w;
   AdamArgs ac = aa;                                            // critic update alone (writes the critic's forward images too)
   ac.seg[0] = aa.seg[1]; ac.nseg = 1; ac.skip_tail = 1;
-  RUN("launch_adam", false, launch_adam(ac, x.st));
+  if (int rc = launch_update(x, ac)) return rc;
   RUN("launch_tcc_pack", false, launch_tcc_pack(L->tcc_pack_dx, x.st));   // transposed images of the UPDATED critic for the policy backward
   TccArgs& fb = L->tcc_fwd_args;
   tcc_begin(x, fb, 1);
@@ -824,16 +842,14 @@ static int post_update_half(Step& x, const AdamArgs& aa) {
   if (int rc = dw_wide(x, false, true)) return rc;
   AdamArgs ab = aa;                                            // actor update + the step's tail (loss means, clock)
   ab.nseg = 1;
-  RUN("launch_adam", false, launch_adam(ab, x.st));
-  return D4PG_OK;
+  return launch_update(x, ab);
 }
 
 // 7'. one launch for both networks, or the two half steps of the post-update plan
 static int update(Step& x) {
   const AdamArgs aa = adam_args(x);
   if (x.h7) return post_update_half(x, aa);
-  RUN("launch_adam", false, launch_adam(aa, x.st));
-  return D4PG_OK;
+  return launch_update(x, aa);
 }
 
 // par: half of the double-buffered batch this step trains on; cold: sample it first (no valid prefetch)
@@ -866,7 +882,7 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
 extern "C" int64_t d4pg_learner_workspace_floats(const d4pg_learner_config_t* cfg) {
   if (!cfg) return -1;
   const d4pg_learner_config_t ec = with_head_width(*cfg);
-  return carve(nullptr, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, step_plan(ec), piped(ec)).total;
+  return carve(nullptr, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, step_plan(ec), piped(ec), clipping(ec)).total;
 }
 
 extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d4pg_learner_buffers_t* buf,
@@ -893,8 +909,16 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   D4PG_REQUIRE(cfg->proj_mode == 0 || cfg->proj_mode == 1, D4PG_EINVAL, "d4pg_learner_create: proj_mode must be 0/1");
   D4PG_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, D4PG_ENOTSUP,
                "d4pg_learner_create: precision %d unknown (0 fp32 FFMA, 1 3xTF32 wgmma, 2 TF32 wgmma, 3 bf16 wgmma)", cfg->precision);
+  D4PG_REQUIRE(!clipping(*cfg) || cfg->world_size <= 1, D4PG_EINVAL,
+               "d4pg_learner_create: max_grad_norm is not supported with world_size > 1: the ranks' gradients are summed "
+               "inside the Adam kernel, so the norm of the summed gradient does not exist before the update");
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
+  for (double mn : {cfg->max_grad_norm_actor, cfg->max_grad_norm_critic})
+    D4PG_REQUIRE(mn == 0.0 || mn > 0.0, D4PG_EINVAL,
+                 "d4pg_learner_create: max_grad_norm must be 0 (off), +inf (report only) or > 0 (got %g)", mn);
+  for (double wd : {cfg->weight_decay_actor, cfg->weight_decay_critic})
+    D4PG_REQUIRE(std::isfinite(wd) && wd >= 0.0, D4PG_EINVAL, "d4pg_learner_create: weight_decay must be finite and >= 0 (got %g)", wd);
   D4PG_REQUIRE(!(cfg->loss_flags & 4) || (step_plan(ec) == PLAN_TC_CHAIN && cfg->world_size <= 1), D4PG_ENOTSUP,
                "d4pg_learner_create: loss_flags & 4 (post-update-critic actor gradient) needs the tensor-core chain plan: precision 1 or 2 (not 0 or 3), chain 1, "
                "batch <= 512, obs_dim <= 32, act_dim <= 32, on one GPU");
@@ -911,7 +935,7 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
     set_error("d4pg_learner_create: grad_critic must equal grad_actor + P_a (one flat gradient buffer)");
     delete L; return D4PG_EINVAL;
   }
-  L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec));
+  L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec), clipping(ec));
   if (!piped(ec)) { L->ws.batch[0].idx = buf->idx; L->ws.batch[0].wts = buf->weights; }   // sampled straight into the caller's buffers
   L->clock_params = ClockParams{ec.lr_actor, ec.lr_critic, ec.beta1, ec.beta2, ec.per_beta0, ec.per_beta_final,
                                 ec.per_beta_iters > 0 ? ec.per_beta_iters : 1};

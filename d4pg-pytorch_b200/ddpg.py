@@ -22,7 +22,7 @@ from .models import actor, critic
 from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer
 from .random_process import GaussianNoise
 from .replay_memory import Replay
-from .shared_adam import SharedAdam
+from .shared_adam import SharedAdam, check_max_grad_norm
 from .utils import default_device
 
 
@@ -85,6 +85,13 @@ class _Learner(object):
         # pipeline -- train() samples batch k on the learner's ingest stream, behind the add()s issued there, while step
         # k-1 still runs (needs the CUDA-graph step)
         cfg.prefetch = 1 if (ddpg.prefetch and (cfg.sample_mode == 1 or ddpg.use_graph)) else 0
+        # per-network clipping thresholds from DDPG, decay from the two global optimisers (which may differ)
+        cfg.max_grad_norm_actor, cfg.max_grad_norm_critic = ddpg.max_grad_norm
+        cfg.weight_decay_actor, cfg.weight_decay_critic = opt_a.weight_decay(), opt_c.weight_decay()
+        if any(ddpg.max_grad_norm) and cfg.world_size > 1:
+            raise _lib.D4PGError("max_grad_norm is not supported with a communicator of world size > 1: the ranks' "
+                                 "gradients are summed inside the Adam kernel, so the norm of the summed gradient does "
+                                 "not exist before the update")
         self.cfg = cfg
         nws = L.d4pg_learner_workspace_floats(C.byref(cfg))
         f32 = torch.float32
@@ -179,7 +186,7 @@ class DDPG:
                  # ---- GPU build extensions (keyword-only in spirit; reference callers never pass them)
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
-                 importance_weighted=False, priority="reference", actor_critic="reference"):
+                 importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None):
         self.gamma = gamma
         self.n_steps = n_steps
         self.n_step_gamma = self.gamma ** self.n_steps
@@ -206,6 +213,13 @@ class DDPG:
         # "post_update": the actor gradient flows through the critic AFTER this step's critic update (corrected SURVEY.md
         # H7); "reference": through the stale pre-update copy, as ddpg.py:229-247 does.  Tensor-core chain plan, one GPU.
         self.actor_critic = actor_critic
+        # clip each network's gradient to a global norm before its Adam update (torch.nn.utils.clip_grad_norm_): None =
+        # off, a positive float for both networks, float("inf") = measure and report only, or an (actor, critic) pair.
+        # The norms of every step are then read with last_grad_norms(); .grad keeps the unclipped gradient.  One GPU.
+        pair = max_grad_norm if isinstance(max_grad_norm, (tuple, list)) else (max_grad_norm, max_grad_norm)
+        if len(pair) != 2:
+            raise ValueError("max_grad_norm must be None, a number or an (actor, critic) pair")
+        self.max_grad_norm = tuple(check_max_grad_norm(x) for x in pair)
 
         self.dist_type = critic_dist_info["type"]
         self.n_quantiles = self.qr_kappa = None
@@ -426,6 +440,16 @@ class DDPG:
         if rc:
             _lib.check(rc, "d4pg_learner_read_losses")
         return L.losses_out[0], L.losses_out[1]
+
+    def last_grad_norms(self, lag=0):
+        """(actor_norm, critic_norm): the global gradient norms, before clipping, of the step `last_losses(lag)` reports,
+        read the same way.  A network without a threshold reports 0.0.  Needs DDPG(max_grad_norm=...)."""
+        if not any(self.max_grad_norm):
+            raise _lib.D4PGError("last_grad_norms needs DDPG(max_grad_norm=...): the norm is only measured when a "
+                                 "threshold (or float('inf')) is set")
+        self.last_losses(lag)
+        out = self._learner.losses_out
+        return out[2], out[3]
 
     def last_batch_info(self):
         """Device tensors of the most recent step: sampled idx, IS weights, td, new priorities."""

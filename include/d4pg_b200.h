@@ -319,6 +319,17 @@ int32_t d4pg_critic_backward_mog(const float* params, int32_t obs_dim, int32_t a
 int32_t d4pg_adam_polyak(float* p, const float* g, float* m, float* v, float* target, int64_t n,
                          double lr, double beta1, double beta2, double eps, int64_t step,
                          double tau, float grad_scale, d4pg_stream_t stream);
+/* The same update on the effective gradient coef * (grad_scale * g) + weight_decay * p (p = the pre-update value):
+ *   weight_decay   finite, >= 0; 0 = none
+ *   max_grad_norm  0 = no clipping; otherwise coef = min(1, max_grad_norm / (norm + 1e-6)) with norm = |grad_scale| *
+ *                  sqrt(sum g^2) in fp64 (+inf: coef = 1, the norm is only reported).  Runs grad_sqnorm_kernel, then the
+ *                  update, on `stream`
+ *   partials       device workspace of 64 doubles; may be NULL when max_grad_norm == 0
+ *   norm_out       optional device float: float32 of norm (written only when max_grad_norm != 0) */
+int32_t d4pg_adam_polyak_ex(float* p, const float* g, float* m, float* v, float* target, int64_t n,
+                            double lr, double beta1, double beta2, double eps, int64_t step,
+                            double tau, float grad_scale, d4pg_stream_t stream,
+                            double weight_decay, double max_grad_norm, double* partials, float* norm_out);
 /* update_target_parameters alone (ddpg.py:110-116): target <- (1-tau)*target + tau*src */
 int32_t d4pg_polyak(float* target, const float* src, int64_t n, double tau, d4pg_stream_t stream);
 /* hard_update (ddpg.py:92-94) / load_state_dict copies */
@@ -382,6 +393,16 @@ typedef struct {
                                  priority = L_i + eps (the quantile-Huber loss is non-negative) */
   int32_t n_components;
   double  qr_kappa;           /* dist_type 2: Huber threshold kappa, finite and > 0 (1.0 is the usual choice) */
+  /* Optimiser options, per network; all zero = the plain update.  On the step's complete gradient g (the flat buffer,
+   * which keeps the UNCLIPPED gradient) and the pre-update parameters p:
+   *   norm = sqrt(sum g_i^2) (fp64, fixed order);  coef = float(min(1, max_grad_norm / (norm + 1e-6)))
+   *   g_eff = coef * g + weight_decay * p, then Adam on g_eff  (torch clip_grad_norm_ + torch.optim.Adam(weight_decay=))
+   * max_grad_norm: 0 = off, +inf = measure and report only (coef is exactly 1), otherwise > 0.  A threshold on either
+   * network adds one grad_sqnorm_kernel launch before each Adam launch; the norms land in losses[2], losses[3].
+   * Not supported with world_size > 1 (the ranks' gradients are summed inside the Adam kernel).
+   * weight_decay: 0 = off, otherwise finite and > 0 (L2 decay added to the gradient, not AdamW); any world size. */
+  double  max_grad_norm_actor, max_grad_norm_critic;
+  double  weight_decay_actor, weight_decay_critic;
 } d4pg_learner_config_t;
 
 /* Caller-owned device buffers.  P_a / P_c = d4pg_*_layout().total. */
@@ -395,7 +416,8 @@ typedef struct {
   float*    weights;       /* [B] f32 out: IS weights (unused by the loss, SURVEY.md H3) */
   float*    prio;          /* [B] f32 out: new priorities */
   float*    td;            /* [B] f32 out */
-  float*    losses;        /* [4]  f32 out: critic loss, actor loss, reserved, reserved */
+  float*    losses;        /* [4]  f32 out: critic loss, actor loss, then the gradient norm (before clipping) of the actor
+                              and of the critic -- each written only when that network has a max_grad_norm, else untouched */
   float*    workspace;     /* f32 [d4pg_learner_workspace_floats()] */
 } d4pg_learner_buffers_t;
 
