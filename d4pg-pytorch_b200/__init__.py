@@ -16,9 +16,10 @@ import sys as _sys
 
 from . import _lib
 from ._lib import D4PGError, LIB_PATH
-from . import utils, random_process, models, prioritized_replay_memory, replay_memory, shared_adam, ddpg, dist
+from . import utils, random_process, models, obs_norm, prioritized_replay_memory, replay_memory, shared_adam, ddpg, dist
 from .ddpg import DDPG
 from .models import actor, critic, fanin_init
+from .obs_norm import ObsNormalizer
 from .prioritized_replay_memory import (LinearSchedule, SegmentTree, SumSegmentTree, MinSegmentTree,
                                         ReplayBuffer, PrioritizedReplayBuffer)
 from .replay_memory import Replay

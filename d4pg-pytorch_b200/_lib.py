@@ -49,6 +49,7 @@ class LearnerConfig(C.Structure):
         ("qr_kappa", C.c_double),
         ("max_grad_norm_actor", C.c_double), ("max_grad_norm_critic", C.c_double),
         ("weight_decay_actor", C.c_double), ("weight_decay_critic", C.c_double),
+        ("obs_norm", C.c_int32),
     ]
 
 
@@ -100,6 +101,10 @@ _PROTOS = {
     "d4pg_her_relabel": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                      C.c_double, C.c_int32, _P, _P, _P, _P, _P, _P]),
     "d4pg_replay_set_len": (C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int32, _P]),
+    "d4pg_replay_set_obs_norm": (C.c_int32, [_P, _P, _P, C.c_double, C.c_double, _P]),
+    "d4pg_replay_obs_norm_refresh": (C.c_int32, [_P, _P]),
+    "d4pg_obs_norm_update": (C.c_int32, [_P, _P, C.c_int32, _P, C.c_int64, C.c_int64, C.c_double, _P]),
+    "d4pg_obs_normalize": (C.c_int32, [_P, C.c_int32, C.c_double, _P, C.c_int64, _P, _P, _P]),
     "d4pg_actor_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, _P]),
     "d4pg_critic_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, C.c_int32, _P]),
     "d4pg_actor_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),

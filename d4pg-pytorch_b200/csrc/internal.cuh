@@ -59,11 +59,13 @@ constexpr int SAMPLE_ROWS = 32;      // batch rows per CTA of the sample + gathe
 int learner_sample(d4pg_replay* h, int B, int prioritized, const double* uniforms, const int32_t* positions,
                    uint64_t seed, LearnerClock* clock, const ClockParams& cp,
                    int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d,
-                   int ld_obs, int ld_act, int pipe_slot, cudaStream_t st, bool dependent = false,
-                   unsigned long long* done_epoch = nullptr);
+                   int ld_obs, int ld_act, const float* norm, float norm_clip, int pipe_slot, cudaStream_t st,
+                   bool dependent = false, unsigned long long* done_epoch = nullptr);
 // gate != nullptr: *gate is bumped (release) once the trees are complete -- by the update kernel itself when it can
 int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* prio, cudaStream_t st, unsigned long long* gate = nullptr);
 int64_t replay_generation(const d4pg_replay* h);
+// the replay's observation normalizer: its affine (nullptr when none is registered) and clip
+const float* replay_obs_norm(const d4pg_replay* h, double* clip);
 // ingest gate (host pipeline): every gated learner step bumps the buffer's flag once (launch_gate_signal) and arms the
 // gate after its launch; the next add / presample on the ingest stream first waits for flag >= number of armed steps
 unsigned long long* replay_gate_flag(d4pg_replay* h);

@@ -159,6 +159,8 @@ struct d4pg_learner {
   // priority write-back bumps, how many gated steps were launched
   cudaStream_t ing; cudaEvent_t ev_ing; unsigned long long* gate_flag;
   bool images_dirty;               // parameters were written outside the library since the forward weight images were last current
+  // cfg.obs_norm: the replay's observation normalizer, applied to s / s2 by every sample launch of the step
+  const float* norm_affine; float norm_clip;
   bool profiling;
   std::vector<cudaEvent_t> ev;
   std::vector<std::string> ev_name;
@@ -329,7 +331,8 @@ static int sample_batch(Step& x) {
       learner_sample(x.L->replay, x.B, c.prioritized, c.sample_mode == 0 ? x.b.uniforms : nullptr,
                      (c.sample_mode == 0 && !c.prioritized) ? x.b.positions : nullptr,
                      c.philox_seed, x.w.clock, x.L->clock_params,
-                     x.bt.idx, x.bt.wts, x.bt.s, x.bt.a, x.bt.r, x.bt.s2, x.bt.done, x.Sp, x.Ap, x.pf ? x.par : -1, x.st));
+                     x.bt.idx, x.bt.wts, x.bt.s, x.bt.a, x.bt.r, x.bt.s2, x.bt.done, x.Sp, x.Ap, x.L->norm_affine,
+                     x.L->norm_clip, x.pf ? x.par : -1, x.st));
   return D4PG_OK;
 }
 
@@ -557,7 +560,7 @@ static int side_branch(Step& x) {
     const Batch& o = x.w.batch[q];
     RUN("learner_sample", false,
         learner_sample(L->replay, x.B, c.prioritized, nullptr, nullptr, c.philox_seed, x.w.clock, L->clock_params,
-                       o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, x.Sp, x.Ap, q, L->side));
+                       o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, x.Sp, x.Ap, L->norm_affine, L->norm_clip, q, L->side));
   }
   if (x.pf) {                           // the caller-visible copies of this step's indices / IS weights (off the
     // path to the next batch: after the write-back and the prefetch)
@@ -912,6 +915,14 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   D4PG_REQUIRE(!clipping(*cfg) || cfg->world_size <= 1, D4PG_EINVAL,
                "d4pg_learner_create: max_grad_norm is not supported with world_size > 1: the ranks' gradients are summed "
                "inside the Adam kernel, so the norm of the summed gradient does not exist before the update");
+  D4PG_REQUIRE(cfg->obs_norm == 0 || cfg->obs_norm == 1, D4PG_EINVAL, "d4pg_learner_create: obs_norm must be 0 or 1");
+  D4PG_REQUIRE(!cfg->obs_norm || cfg->world_size <= 1, D4PG_EINVAL,
+               "d4pg_learner_create: obs_norm is not supported with world_size > 1: each rank would normalize with the "
+               "statistics of its own shard");
+  double norm_clip = 0.0;
+  const float* norm_affine = cfg->obs_norm ? replay_obs_norm(replay, &norm_clip) : nullptr;
+  D4PG_REQUIRE(!cfg->obs_norm || norm_affine, D4PG_EINVAL,
+               "d4pg_learner_create: obs_norm needs a replay with an observation normalizer (d4pg_replay_set_obs_norm)");
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
   for (double mn : {cfg->max_grad_norm_actor, cfg->max_grad_norm_critic})
@@ -952,6 +963,7 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   for (int i = 0; i < 2; ++i) { L->loss_ring[i] = nullptr; L->ev_loss[i] = nullptr; }
   L->loss_steps = 0;
   L->ing = nullptr; L->ev_ing = nullptr; L->gate_flag = nullptr; L->images_dirty = true;
+  L->norm_affine = norm_affine; L->norm_clip = float(norm_clip);
   if (host_pipe(*cfg)) {
     L->gate_flag = replay_gate_flag(replay);
     const bool ok = L->gate_flag && cudaStreamCreateWithFlags(&L->ing, cudaStreamNonBlocking) == cudaSuccess &&
@@ -1092,7 +1104,7 @@ static int presample(d4pg_learner* L, int par, const double* uniforms, const int
   const d4pg_learner_config_t& c = L->cfg; const Workspace& w = L->ws; const Batch& o = w.batch[par];
   return learner_sample(L->replay, c.batch, c.prioritized, uniforms, !c.prioritized ? positions : nullptr, c.philox_seed,
                         w.clock, L->clock_params, o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, pitch4(c.obs_dim),
-                        pitch4(c.act_dim), par, st, /*dependent=*/true, w.pipe_epoch);
+                        pitch4(c.act_dim), L->norm_affine, L->norm_clip, par, st, /*dependent=*/true, w.pipe_epoch);
 }
 
 // The host-facing step: stage this step's host inputs in pinned memory, H2D, the step, order the caller after it.

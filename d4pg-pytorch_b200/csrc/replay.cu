@@ -35,6 +35,8 @@ struct d4pg_replay {
   // The flag lives with the buffer (learners come and go); every gated step bumps it once and arms target = #armed.
   unsigned long long* gate_flag; unsigned long long gate_target; bool gate_pending;
   cudaEvent_t order_ev;
+  // observation normalizer (d4pg_replay_set_obs_norm): caller-owned stats / affine, updated by every insert
+  double* norm_stats; float* norm_affine; double norm_clip, norm_eps;
 };
 
 namespace d4pg {
@@ -42,12 +44,15 @@ namespace d4pg {
 static unsigned long long* step_trace() { unsigned long long* p = debug_trace_buffer(); return p ? p + STEP_TRACE_BASE : nullptr; }
 
 
-__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_kernel(const SampleArgs a) {
+// NORM: the learner's batch goes through the observation normalizer as it is gathered (sample_body<true>).  The two
+// instantiations are separate non-template kernels so that the plain one compiles to what it was before the option.
+template <bool NORM>
+__device__ __forceinline__ void sample_gather_body(const SampleArgs& a) {
   __shared__ SampleSmem sm;
   pdl_trigger(a.pdl);
   pdl_wait();
   step_stamp(a.trace, a.trace_slot);
-  sample_body(a, blockIdx.x, sm);
+  sample_body<NORM>(a, blockIdx.x, sm);
   if (a.done_epoch) {                          // the forward chains of the step poll these instead of a stream event
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -59,6 +64,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_kernel(const Sam
   step_stamp(a.trace, a.trace_slot + 16);
   pdl_trigger_end(a.pdl);
 }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_kernel(const SampleArgs a) { sample_gather_body<false>(a); }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_norm_kernel(const SampleArgs a) { sample_gather_body<true>(a); }
 
 template <int MODE>
 __global__ void __launch_bounds__(TREE_THREADS) tree_write_kernel(const TreeArgs a) {
@@ -290,7 +297,10 @@ int launch_sample(const d4pg_replay* h, SampleArgs& a, cudaStream_t st, bool dep
   a.pdl = pdl_mode();
   a.trace = (a.clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
   a.trace_slot = a.pipe_slot >= 0 && a.uniforms == nullptr && st_is_side(st) ? 4 : 0;
-  D4PG_MAX_CARVEOUT(sample_gather_kernel);
+  // a.norm (learner with an observation normalizer): s / s2 are normalized as they are gathered
+  void (*kernel)(const SampleArgs) = a.norm ? sample_gather_norm_kernel : sample_gather_kernel;
+  if (a.norm) D4PG_MAX_CARVEOUT(sample_gather_norm_kernel);
+  else D4PG_MAX_CARVEOUT(sample_gather_kernel);
   if (dependent) {
     // programmatic dependent launch behind the previous kernel of the stream (the host pipeline's tree add): the grid is
     // resident when that kernel ends, griddepcontrol.wait at the top of the kernel holds it until its writes are visible
@@ -300,19 +310,21 @@ int launch_sample(const d4pg_replay* h, SampleArgs& a, cudaStream_t st, bool dep
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    D4PG_CUDA_OK(cudaLaunchKernelEx(&cfg, sample_gather_kernel, a));
+    D4PG_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, a));
     return D4PG_OK;
   }
-  D4PG_CUDA_OK(launch_pdl(sample_gather_kernel, dim3(cdiv(a.B, SAMPLE_ROWS)), dim3(SAMPLE_THREADS), 0, st, a));
+  D4PG_CUDA_OK(launch_pdl(kernel, dim3(cdiv(a.B, SAMPLE_ROWS)), dim3(SAMPLE_THREADS), 0, st, a));
   return D4PG_OK;
 }
 
 int learner_sample(d4pg_replay* h, int B, int prioritized, const double* uniforms, const int32_t* positions,
                    uint64_t seed, LearnerClock* clock, const ClockParams& cp,
                    int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d,
-                   int ld_obs, int ld_act, int pipe_slot, cudaStream_t st, bool dependent, unsigned long long* done_epoch) {
+                   int ld_obs, int ld_act, const float* norm, float norm_clip, int pipe_slot, cudaStream_t st, bool dependent,
+                   unsigned long long* done_epoch) {
   SampleArgs sa{};
   sa.done_epoch = done_epoch;
+  sa.norm = norm; sa.norm_clip = norm_clip;
   sa.ld_obs = ld_obs; sa.ld_act = ld_act; sa.pipe_slot = pipe_slot;
   sa.uniforms = uniforms; sa.seed = seed; sa.counter = 0; sa.clock = clock; sa.clock_params = cp;
   sa.beta = 1.f; sa.B = B; sa.idx = idx; sa.weights = prioritized ? weights : nullptr;
@@ -344,6 +356,7 @@ void tree_update_args(d4pg_replay* h, int B, const int32_t* idx, const float* pr
 }
 
 int64_t replay_generation(const d4pg_replay* h) { return h->gen; }
+const float* replay_obs_norm(const d4pg_replay* h, double* clip) { if (clip) *clip = h->norm_clip; return h->norm_affine; }
 
 int launch_gate_signal(unsigned long long* flag, cudaStream_t st);
 int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* prio, cudaStream_t st, unsigned long long* gate) {
@@ -401,6 +414,7 @@ extern "C" int32_t d4pg_replay_create(int64_t size, int32_t obs_dim, int32_t act
   h->stage_host = nullptr; h->stage_dev = nullptr; h->stage_bytes = 0; h->stage_slot = 0;
   for (int i = 0; i < 2; ++i) { h->stage_ev[i] = nullptr; h->stage_busy[i] = false; }
   h->gate_flag = nullptr; h->gate_target = 0; h->gate_pending = false; h->order_ev = nullptr;
+  h->norm_stats = nullptr; h->norm_affine = nullptr; h->norm_clip = 0.0; h->norm_eps = 0.0;
   tree_init_kernel<<<2 * device_sm_count(), 256, 0, as_stream(stream)>>>(h->sum, h->mn, h->scratch,
                                                         reinterpret_cast<ReplayState*>(h->state), h->cap);
   cudaError_t e = cudaGetLastError();
@@ -636,6 +650,30 @@ extern "C" int32_t d4pg_replay_set_len(d4pg_replay_t* h, int64_t len, int64_t ne
   return D4PG_OK;
 }
 
+extern "C" int32_t d4pg_replay_set_obs_norm(d4pg_replay_t* h, double* stats, float* affine, double clip, double eps,
+                                           d4pg_stream_t stream) {
+  if (h) ++h->gen;
+  D4PG_REQUIRE(h, D4PG_EINVAL, "d4pg_replay_set_obs_norm: null handle");
+  if (!stats) {
+    h->norm_stats = nullptr; h->norm_affine = nullptr;
+    return D4PG_OK;
+  }
+  D4PG_REQUIRE(affine, D4PG_EINVAL, "d4pg_replay_set_obs_norm: null affine buffer");
+  D4PG_REQUIRE(std::isfinite(clip) && clip > 0.0, D4PG_EINVAL, "d4pg_replay_set_obs_norm: clip must be finite and > 0 (got %g)", clip);
+  D4PG_REQUIRE(std::isfinite(eps) && eps > 0.0, D4PG_EINVAL, "d4pg_replay_set_obs_norm: eps must be finite and > 0 (got %g)", eps);
+  int rc = launch_obs_norm_reset(stats, affine, h->obs_dim, as_stream(stream));
+  if (rc) return rc;
+  h->norm_stats = stats; h->norm_affine = affine; h->norm_clip = clip; h->norm_eps = eps;
+  return D4PG_OK;
+}
+
+extern "C" int32_t d4pg_replay_obs_norm_refresh(d4pg_replay_t* h, d4pg_stream_t stream) {
+  if (h) ++h->gen;
+  D4PG_REQUIRE(h, D4PG_EINVAL, "d4pg_replay_obs_norm_refresh: null handle");
+  D4PG_REQUIRE(h->norm_stats, D4PG_ESTATE, "d4pg_replay_obs_norm_refresh: no observation normalizer registered");
+  return launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, nullptr, 0, h->obs_dim, h->norm_eps, as_stream(stream));
+}
+
 extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs, const float* act,
                                    const double* rew, const float* obs2, const uint8_t* done,
                                    int32_t prioritized, d4pg_stream_t stream) {
@@ -651,6 +689,12 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
                                              n, h->obs_dim, h->act_dim, h->size, start,
                                              reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
   D4PG_LAUNCH_OK();
+  if (h->norm_stats) {
+    // the normalizer's statistics: the same rows, in the same order.  Before the ingest gate and the tree kernels, so
+    // the host pipeline's tree add stays the kernel the presample is programmatically dependent on
+    int nrc = launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, obs, n, h->obs_dim, h->norm_eps, st);
+    if (nrc) return nrc;
+  }
   if (prioritized) {
     // ingest gate (host pipeline): the rows above only had to follow the previous gather (stream order); the trees wait for
     // the last launched learner step's priority write-back -- inside the first tree kernel when that is the 1-CTA fast one

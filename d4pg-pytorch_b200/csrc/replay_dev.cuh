@@ -2,6 +2,7 @@
 #pragma once
 #include "internal.cuh"
 #include "adam.cuh"
+#include "obs_norm.cuh"
 
 namespace d4pg {
 
@@ -72,6 +73,8 @@ struct SampleArgs {
   int pipe_slot;                    // >= 0 (prefetch pipeline): use the sampler's own counters, derive into this slot
   unsigned long long* trace; int trace_slot;
   unsigned long long* done_epoch;   // host pipeline: CTA b publishes (release) s_steps_done + 1 in [b] when its rows are gathered
+  const float* norm;                // observation normalizer affine {shift[S], scale[S]} (sample_body<true> only)
+  float norm_clip;
 };
 
 constexpr int SAMPLE_THREADS = 256;
@@ -103,7 +106,9 @@ struct SampleSmem {
   int32_t idx[SAMPLE_ROWS];
   float total;
 };
-// rows [bid*32, bid*32+32) of the batch, executed by one 256-thread CTA
+// rows [bid*32, bid*32+32) of the batch, executed by one 256-thread CTA.  NORM: s and s2 are written through the
+// observation normalizer's affine (obs_norm.cuh) -- before the CTA's rows count as gathered.
+template <bool NORM>
 __device__ __forceinline__ void sample_body(const SampleArgs& a, int bid, SampleSmem& sm) {
   int32_t* idx_s = sm.idx;
   float* top_s = sm.top;
@@ -216,8 +221,14 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, int bid, Sample
   for (int e = t; e < nrows * od; e += SAMPLE_THREADS) {
     const int rr = e / od, c = e - rr * od;
     const size_t src = size_t(idx_s[rr]) * od + c, dst = size_t(row0 + rr) * lo + c;
-    a.s[dst] = __ldg(a.obs + src);
-    a.s2[dst] = __ldg(a.obs2 + src);
+    if (NORM) {
+      const float sh = __ldg(a.norm + c), sc = __ldg(a.norm + od + c);
+      a.s[dst] = obs_norm_apply(__ldg(a.obs + src), sh, sc, a.norm_clip);
+      a.s2[dst] = obs_norm_apply(__ldg(a.obs2 + src), sh, sc, a.norm_clip);
+    } else {
+      a.s[dst] = __ldg(a.obs + src);
+      a.s2[dst] = __ldg(a.obs2 + src);
+    }
   }
   for (int e = t; e < nrows * ad; e += SAMPLE_THREADS) {
     const int rr = e / ad, c = e - rr * ad;

@@ -19,6 +19,7 @@ import torch
 
 from . import _lib
 from .models import actor, critic
+from .obs_norm import make_obs_normalizer
 from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer
 from .random_process import GaussianNoise
 from .replay_memory import Replay
@@ -88,6 +89,9 @@ class _Learner(object):
         # per-network clipping thresholds from DDPG, decay from the two global optimisers (which may differ)
         cfg.max_grad_norm_actor, cfg.max_grad_norm_critic = ddpg.max_grad_norm
         cfg.weight_decay_actor, cfg.weight_decay_critic = opt_a.weight_decay(), opt_c.weight_decay()
+        cfg.obs_norm = 1 if ddpg.obs_normalizer is not None else 0
+        if cfg.obs_norm and cfg.world_size > 1:
+            raise _lib.D4PGError("obs_norm is not supported with a communicator of world size > 1")
         if any(ddpg.max_grad_norm) and cfg.world_size > 1:
             raise _lib.D4PGError("max_grad_norm is not supported with a communicator of world size > 1: the ranks' "
                                  "gradients are summed inside the Adam kernel, so the norm of the summed gradient does "
@@ -186,7 +190,8 @@ class DDPG:
                  # ---- GPU build extensions (keyword-only in spirit; reference callers never pass them)
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
-                 importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None):
+                 importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None,
+                 obs_norm=None):
         self.gamma = gamma
         self.n_steps = n_steps
         self.n_step_gamma = self.gamma ** self.n_steps
@@ -220,6 +225,13 @@ class DDPG:
         if len(pair) != 2:
             raise ValueError("max_grad_norm must be None, a number or an (actor, critic) pair")
         self.max_grad_norm = tuple(check_max_grad_norm(x) for x in pair)
+        # running per-feature observation normalization (obs_norm.py): None / False = off, True = clip 5, eps 1e-8, or
+        # {"clip": c, "eps": e}.  Every replay insert updates the statistics; the learner's s / s2 and the `state` input
+        # of the four networks below are normalized with them.  One GPU.
+        self.obs_normalizer = make_obs_normalizer(obs_norm, obs_dim, self.device)
+        if self.obs_normalizer is not None and comm is not None and comm.world_size > 1:
+            raise _lib.D4PGError("obs_norm is not supported with a communicator of world size > 1: each rank would "
+                                 "normalize with the statistics of its own replay shard")
 
         self.dist_type = critic_dist_info["type"]
         self.n_quantiles = self.qr_kappa = None
@@ -260,6 +272,9 @@ class DDPG:
         self.critic = critic(state_size=obs_dim, action_size=act_dim, dist_info=critic_dist_info, device=self.device)
         self.critic_target = critic(state_size=obs_dim, action_size=act_dim, dist_info=critic_dist_info, device=self.device)
         self.critic_target.load_state_dict(self.critic.state_dict())
+        if self.obs_normalizer is not None:
+            for net in (self.actor, self.actor_target, self.critic, self.critic_target):
+                net.obs_normalizer = self.obs_normalizer
 
         # constructed for attribute compatibility; like the reference's, never stepped by train()
         self.optimizer_actor = SharedAdam(self.actor.parameters(), lr=lr_actor, betas=(0.9, 0.999))
@@ -272,12 +287,12 @@ class DDPG:
         self.prioritized_replay = prioritized_replay
         if self.prioritized_replay:                                                          # ddpg.py:78-87
             self.replayBuffer = PrioritizedReplayBuffer(self.memory_size, alpha=0.6, obs_dim=obs_dim,
-                                                        act_dim=act_dim, device=self.device)
+                                                        act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer)
             self.beta_schedule = LinearSchedule(100000, initial_p=0.4, final_p=1.0)
             self.prioritized_replay_eps = 1e-6
         else:
             self.replayBuffer = Replay(self.memory_size, self.env, n_steps=self.n_steps, gamma=self.gamma,
-                                       obs_dim=obs_dim, act_dim=act_dim, device=self.device)
+                                       obs_dim=obs_dim, act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer)
         self._learner = None
 
     # ---- reference plumbing methods ------------------------------------------------------

@@ -59,6 +59,9 @@ class _FlatNet(nn.Module):
     # runs d4pg_*_backward (loss.backward() fills .grad -- kept in the flat gradient buffer -- and d input).
     # False: forward() returns a plain tensor.
     differentiable = False
+    # ObsNormalizer (obs_norm.py) or None: when set, the `state` input goes through it before fc1 (a DDPG with obs_norm
+    # attaches its normalizer to all four networks); the critic's action input is never normalized
+    obs_normalizer = None
 
     def __init__(self, dims, device=None):
         super().__init__()
@@ -192,6 +195,15 @@ class _FlatNet(nn.Module):
         assert x.shape[1] == width, "expected input width %d, got %s" % (width, tuple(x.shape))
         return x.contiguous()
 
+    def _state_input(self, state, width, grad):
+        """The `state` input as the kernels take it: through the observation normalizer when one is attached (on the
+        autograd graph when `grad`)."""
+        x = self._as_grad_input(state, width) if grad else self._as_input(state, width)
+        norm = self.obs_normalizer
+        if norm is None:
+            return x
+        return norm.apply(x) if grad else norm.normalize(x)
+
     # ---- autograd path (differentiable=True) ----------------------------------------------
     def _param_list(self):
         out = []
@@ -246,9 +258,9 @@ class actor(_FlatNet):
     def forward(self, state):
         _lib.require_cuda()
         if self._use_autograd((state,)):
-            x = self._as_grad_input(state, self.input_size)
+            x = self._state_input(state, self.input_size, True)
             return _ActorFn.apply(self, int(self.precision), x, *self._grad_params())
-        x = self._as_input(state, self.input_size)
+        x = self._state_input(state, self.input_size, False)
         B = x.shape[0]
         out = torch.empty(B, self.output_size, dtype=torch.float32, device=x.device)
         _lib.check(_lib.lib().d4pg_actor_forward(_lib.ptr(self._flat), self.input_size, self.output_size,
@@ -313,11 +325,11 @@ class critic(_FlatNet):
         if self.n_quantiles is not None:
             return self._forward_qr(state, action)
         if self._use_autograd((state, action)):
-            x = self._as_grad_input(state, self.state_size)
+            x = self._state_input(state, self.state_size, True)
             a = self._as_grad_input(action, self.action_size)
             probs, logits = _CriticFn.apply(self, int(self.precision), x, a, *self._grad_params())
             return (probs, logits) if return_logits else probs
-        x = self._as_input(state, self.state_size)
+        x = self._state_input(state, self.state_size, False)
         a = self._as_input(action, self.action_size)
         B = x.shape[0]
         probs = torch.empty(B, self.n_atoms, dtype=torch.float32, device=x.device)
@@ -330,11 +342,11 @@ class critic(_FlatNet):
 
     def _forward_mog(self, state, action, return_raw):
         if self._use_autograd((state, action)):
-            x = self._as_grad_input(state, self.state_size)
+            x = self._state_input(state, self.state_size, True)
             a = self._as_grad_input(action, self.action_size)
             w, mu, sigma, raw = _CriticMogFn.apply(self, int(self.precision), x, a, *self._grad_params())
             return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
-        x = self._as_input(state, self.state_size)
+        x = self._state_input(state, self.state_size, False)
         a = self._as_input(action, self.action_size)
         B, K = x.shape[0], self.n_components
         w, mu, sigma = (torch.empty(B, K, dtype=torch.float32, device=x.device) for _ in range(3))
@@ -347,10 +359,10 @@ class critic(_FlatNet):
 
     def _forward_qr(self, state, action):
         if self._use_autograd((state, action)):
-            x = self._as_grad_input(state, self.state_size)
+            x = self._state_input(state, self.state_size, True)
             a = self._as_grad_input(action, self.action_size)
             return _CriticQrFn.apply(self, int(self.precision), x, a, *self._grad_params())
-        x = self._as_input(state, self.state_size)
+        x = self._state_input(state, self.state_size, False)
         a = self._as_input(action, self.action_size)
         B = x.shape[0]
         theta = torch.empty(B, self.n_atoms, dtype=torch.float32, device=x.device)

@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .obs_norm import make_obs_normalizer
 from .utils import default_device
 
 
@@ -46,8 +47,9 @@ class _DeviceReplay(object):
 
     STAGE_ROWS = 4096
 
-    def __init__(self, size, alpha, prioritized, obs_dim=None, act_dim=None, device=None):
+    def __init__(self, size, alpha, prioritized, obs_dim=None, act_dim=None, device=None, obs_norm=None):
         self.size = int(size)
+        self.obs_norm = obs_norm         # ObsNormalizer (obs_norm.py): registered when the store is allocated
         self.alpha = float(alpha)
         self.prioritized = bool(prioritized)
         self.device = torch.device(device) if device is not None else None
@@ -91,6 +93,8 @@ class _DeviceReplay(object):
                                                  _lib.ptr(self.state), _lib.stream_ptr(), C.byref(h)),
                    "d4pg_replay_create")
         self.handle = h
+        if self.obs_norm is not None:
+            self.obs_norm._bind(self)
         R = self.STAGE_ROWS
         pin = dict(pin_memory=True)
         self._st_obs = torch.empty(R, self.obs_dim, dtype=f32, **pin)
@@ -128,6 +132,13 @@ class _DeviceReplay(object):
                            "d4pg_replay_order_after")
                 self._ing_dirty = False
             self._cs_dirty = True
+
+    def _order_ingest_after_caller(self):
+        """The caller's stream wrote something the ingest stream's next sample reads (normalizer statistics)."""
+        if self._ingest_stream is not None and self.handle is not None:
+            _lib.check(_lib.lib().d4pg_replay_order_after(self.handle, _lib.stream_ptr(), C.c_void_p(self._ingest_stream)),
+                       "d4pg_replay_order_after")
+            self._cs_dirty = False
 
     def _ingest_ptr(self):
         """Stream of a host add: the ingest stream when attached (ordered after the caller's earlier buffer operations)."""
@@ -497,9 +508,15 @@ class ReplayBuffer(object):
 
     _prioritized = False
 
-    def __init__(self, size, obs_dim=None, act_dim=None, device=None, _alpha=1.0):
+    def __init__(self, size, obs_dim=None, act_dim=None, device=None, _alpha=1.0, obs_norm=None):
         self._maxsize = size
-        self._store = _DeviceReplay(size, _alpha, self._prioritized, obs_dim, act_dim, device)
+        self._store = _DeviceReplay(size, _alpha, self._prioritized, obs_dim, act_dim, device,
+                                    make_obs_normalizer(obs_norm, obs_dim, device))
+
+    @property
+    def obs_normalizer(self):
+        """The ObsNormalizer every insert updates (None without obs_norm=)."""
+        return self._store.obs_norm
 
     def __len__(self):
         return len(self._store)
@@ -540,10 +557,10 @@ class PrioritizedReplayBuffer(ReplayBuffer):
 
     _prioritized = True
 
-    def __init__(self, size, alpha, obs_dim=None, act_dim=None, device=None):
+    def __init__(self, size, alpha, obs_dim=None, act_dim=None, device=None, obs_norm=None):
         assert alpha >= 0                                                                    # :240
         self._alpha = alpha
-        super(PrioritizedReplayBuffer, self).__init__(size, obs_dim, act_dim, device, _alpha=alpha)
+        super(PrioritizedReplayBuffer, self).__init__(size, obs_dim, act_dim, device, _alpha=alpha, obs_norm=obs_norm)
         self._it_sum = _TreeView(self._store, 0)
         self._it_min = _TreeView(self._store, 1)
 

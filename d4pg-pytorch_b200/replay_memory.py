@@ -12,16 +12,23 @@ import random
 
 import numpy as np
 
+from .obs_norm import make_obs_normalizer
 from .prioritized_replay_memory import _DeviceReplay
 
 
 class Replay(object):
-    def __init__(self, max_size, env, n_steps=1, gamma=0.99, obs_dim=None, act_dim=None, device=None):
+    def __init__(self, max_size, env, n_steps=1, gamma=0.99, obs_dim=None, act_dim=None, device=None, obs_norm=None):
         self.capacity = max_size
         self.env = env
         self.n_steps = n_steps
         self.gamma = gamma
-        self._store = _DeviceReplay(max_size, 1.0, False, obs_dim, act_dim, device)
+        # obs_norm: None / False, True, {"clip": c, "eps": e} or an ObsNormalizer that every insert updates (obs_norm.py)
+        self._store = _DeviceReplay(max_size, 1.0, False, obs_dim, act_dim, device,
+                                    make_obs_normalizer(obs_norm, obs_dim, device))
+
+    @property
+    def obs_normalizer(self):
+        return self._store.obs_norm
 
     def __len__(self):
         return len(self._store)

@@ -217,6 +217,30 @@ int32_t d4pg_her_relabel(int32_t T, int32_t obs_dim, int32_t goal_dim, int32_t a
                          float* out_s, float* out_a, double* out_r, float* out_s2, uint8_t* out_d,
                          d4pg_stream_t stream);
 
+/* Running per-feature observation normalizer (mean / variance over every stored row, with clipping).
+ *   stats  f64 [1 + 2*obs_dim] = {n, mean[S], M2[S]}      affine f32 [2*obs_dim] = {shift[S], scale[S]}
+ * Update: every row an insert stores contributes its s once, in insertion order (rows later overwritten by the ring
+ * still count), folded in with Welford's step, every fp64 operation rounded and not contracted:
+ *   n = n + 1;  d = x - mean;  mean = mean + d / n;  M2 = M2 + d * (x - mean)
+ * Affine, recomputed at the end of every update: n == 0 -> shift 0, scale 1; otherwise shift = f32(mean),
+ *   scale = f32(1 / sqrt(M2 / n + eps)) (fp64, correctly rounded, one cast at the end).
+ * Apply (fp32): y = min(max((x - shift) * scale, -clip), clip).  clip and eps: finite and > 0 (5.0 and 1e-8 are usual).
+ *
+ * d4pg_replay_set_obs_norm registers caller-owned device buffers with the replay and resets them to n = 0 on `stream`;
+ * from then on every insert (add, add_host, add_nstep) updates them on its own stream, right after its ring write.
+ * stats == NULL detaches.  The stored rows and every sample / gather of this section stay raw; only a learner created
+ * with obs_norm = 1 reads the affine.  d4pg_replay_obs_norm_refresh recomputes the affine from the stats after the
+ * caller wrote them (a state load).  Both bump the replay's generation, so a learner's prefetched batch is re-sampled.
+ * d4pg_obs_norm_update is the same fold + affine on caller rows [n, ld] (n == 0: the affine alone), without a replay;
+ * d4pg_obs_normalize applies the affine to x [n, obs_dim] into y and, when dydx is given, writes dy/dx: scale where the
+ * pre-clip value lies in [-clip, clip], else 0. */
+int32_t d4pg_replay_set_obs_norm(d4pg_replay_t* h, double* stats, float* affine, double clip, double eps, d4pg_stream_t stream);
+int32_t d4pg_replay_obs_norm_refresh(d4pg_replay_t* h, d4pg_stream_t stream);
+int32_t d4pg_obs_norm_update(double* stats, float* affine, int32_t obs_dim, const float* rows, int64_t n, int64_t ld,
+                             double eps, d4pg_stream_t stream);
+int32_t d4pg_obs_normalize(const float* affine, int32_t obs_dim, double clip, const float* x, int64_t n,
+                           float* y, float* dydx, d4pg_stream_t stream);
+
 /* _sample_proportional + IS weights + _encode_sample (:258-313,189-199).
  *   uniforms [B] f64 in [0,1): the reference's random.random() draws; NULL = device Philox
  *   (seed, counter) stream.  mass = u * sum(0,len-1) with the reference's association and
@@ -403,6 +427,11 @@ typedef struct {
    * weight_decay: 0 = off, otherwise finite and > 0 (L2 decay added to the gradient, not AdamW); any world size. */
   double  max_grad_norm_actor, max_grad_norm_critic;
   double  weight_decay_actor, weight_decay_critic;
+  int32_t obs_norm;           /* 1: s and s2 of every batch go through the replay's observation normalizer as they are
+                                 gathered (d4pg_replay_set_obs_norm, which must be registered before d4pg_learner_create
+                                 and stay registered, with the same buffers and clip, for the learner's lifetime).
+                                 0 = off.  Not supported with world_size > 1 (D4PG_EINVAL): each rank would normalize with
+                                 the statistics of its own shard */
 } d4pg_learner_config_t;
 
 /* Caller-owned device buffers.  P_a / P_c = d4pg_*_layout().total. */
