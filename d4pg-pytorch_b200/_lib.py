@@ -107,6 +107,10 @@ _PROTOS = {
     "d4pg_obs_normalize": (C.c_int32, [_P, C.c_int32, C.c_double, _P, C.c_int64, _P, _P, _P]),
     "d4pg_actor_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, _P]),
     "d4pg_critic_forward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, C.c_int32, _P]),
+    "d4pg_act_workspace_floats": (C.c_int64, [C.c_int32, C.c_int32]),
+    "d4pg_act": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_double, C.c_int32, _P,
+                             C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),
+    "d4pg_copy_rows_f32": (C.c_int32, [_P, C.c_int64, _P, C.c_int64, C.c_int64, C.c_int64, _P]),
     "d4pg_actor_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_critic_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P,
                                          _P, _P, _P, _P, C.c_int32, _P]),

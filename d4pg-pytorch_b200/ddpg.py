@@ -21,7 +21,7 @@ from . import _lib
 from .models import actor, critic
 from .obs_norm import make_obs_normalizer
 from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer
-from .random_process import GaussianNoise
+from .random_process import GaussianNoise, OrnsteinUhlenbeckProcess
 from .replay_memory import Replay
 from .shared_adam import SharedAdam, check_max_grad_norm
 from .utils import default_device
@@ -283,6 +283,11 @@ class DDPG:
         self.optimizer_global_critic = None
 
         self.noise = GaussianNoise(dimension=act_dim, num_epochs=5000)                       # ddpg.py:75
+        # act(): exploring calls so far (the Philox counter of the next one is 2^63 + this), the device OU state and the
+        # per-E workspace / pitch-4 input buffers
+        self._act_calls = 0
+        self._exploration_state = None
+        self._act_buffers = {}
 
         self.prioritized_replay = prioritized_replay
         if self.prioritized_replay:                                                          # ddpg.py:78-87
@@ -371,6 +376,133 @@ class DDPG:
         else:
             states, actions, rewards, next_states, terminates = self.replayBuffer.sample(self.batch_size)
         return states, actions, rewards, next_states, terminates, weights, batch_idxes
+
+    # ---- action selection -------------------------------------------------------------------
+    def act(self, state, explore=True, reset=None):
+        """The rollout's action, `np.clip(actor(s) + noise.sample(), -1, 1)` (main.py:145-146, 216-217, 279), for E
+        environments in one launch on the caller's stream.  `state`: numpy or tensor, host or device, [obs_dim] or
+        [E, obs_dim].  Returns an fp32 device tensor [E, act_dim] ([1, act_dim] for one row).
+
+        The actor runs at fp32 (precision 0) with this DDPG's observation normalizer, if any.  explore=False returns
+        actor(state) bit for bit.  explore=True adds the noise of `self.noise` -- GaussianNoise or
+        OrnsteinUhlenbeckProcess, whose epsilon / mu / var (theta / sigma / dt) are read at each call -- drawn on the
+        device from Philox (key philox_seed, counter 2^63 + the number of earlier exploring calls), and clips to
+        [-1, 1] in fp64.  OU noise keeps one state row per environment in `exploration_state`; `reset` (bool [E]) restarts
+        the rows of environments that began a new episode.  The arithmetic is in DESIGN.md §3 "Exploration"."""
+        mode, params = self._act_noise(explore)
+        x, E = self._act_rows(state)
+        if mode == 2:
+            st = self._exploration_state
+            if st is not None and st.shape[0] != E:
+                raise _lib.D4PGError("act: the Ornstein-Uhlenbeck state holds %d environments, this call has %d (assign "
+                                     "exploration_state = None to start over)" % (st.shape[0], E))
+            if reset is not None and tuple(np.shape(reset)) != (E,):
+                raise ValueError("act: reset must be a bool mask of shape (%d,), got %s" % (E, tuple(np.shape(reset))))
+        _lib.require_cuda()
+        L = _lib.lib()
+        S, A = self.obs_dim, self.act_dim
+        flat = self.actor.flat_params()
+        dev = flat.device
+        bufs = self._act_buffers.get(E)
+        if bufs is None or bufs[0].device != dev:
+            bufs = self._act_buffers[E] = [torch.empty(L.d4pg_act_workspace_floats(E, S), dtype=torch.float32, device=dev), None]
+        rows, lds = self._act_input(x, E, dev, bufs)
+        st = rmask = None
+        if mode == 2:
+            st = self._exploration_state
+            if st is None:
+                st = torch.from_numpy(np.zeros((E, A))).to(dev)          # a copy, not a fill kernel
+            rmask = self._act_reset(reset, dev) if reset is not None else None
+        norm = self.obs_normalizer
+        affine, clip = None, 0.0
+        if norm is not None:
+            norm._require()
+            norm._join()
+            affine, clip = _lib.ptr(norm.affine), norm.clip
+        out = torch.empty(E, A, dtype=torch.float32, device=dev)
+        p = (C.c_double * 5)(*params)
+        counter = (1 << 63) + self._act_calls
+        _lib.check(L.d4pg_act(_lib.ptr(flat), S, A, _lib.ptr(rows), lds, E, affine, clip, mode, p,
+                              int(self.philox_seed) & 0xFFFFFFFFFFFFFFFF, counter, _lib.ptr(st), _lib.ptr(rmask),
+                              _lib.ptr(out), _lib.ptr(bufs[0]), _lib.stream_ptr()), "d4pg_act")
+        if mode:
+            self._act_calls += 1
+        if mode == 2:
+            self._exploration_state = st
+        return out
+
+    @property
+    def exploration_state(self):
+        """The device Ornstein-Uhlenbeck state of act(): None until the first exploring call with OU noise, then fp64
+        [E, act_dim].  That call fixes E.  Assign None to drop it: the next call starts from zeros, with any E."""
+        return self._exploration_state
+
+    @exploration_state.setter
+    def exploration_state(self, value):
+        if value is not None:
+            raise ValueError("exploration_state can only be set to None")
+        self._exploration_state = None
+
+    def _act_noise(self, explore):
+        """(noise mode of d4pg_act, its parameters) for the current `self.noise`."""
+        if not explore:
+            return 0, ()
+        nz = self.noise
+        if isinstance(nz, GaussianNoise):
+            return 1, tuple(float(v) for v in (nz.epsilon, nz.mu, nz.var))
+        if isinstance(nz, OrnsteinUhlenbeckProcess):
+            return 2, tuple(float(v) for v in (nz.epsilon, nz.theta, nz.mu, nz.sigma, nz.dt))
+        raise _lib.D4PGError("act(explore=True) draws GaussianNoise or OrnsteinUhlenbeckProcess noise on the device; "
+                             "self.noise is a %s" % type(nz).__name__)
+
+    def _act_rows(self, state):
+        """(rows, E): `state` as [E, obs_dim], a tensor where it lives, anything else as float32 numpy."""
+        x = state.detach() if torch.is_tensor(state) else np.asarray(state, dtype=np.float32)
+        if x.ndim == 1:
+            x = x.reshape(1, -1)
+        if x.ndim != 2 or x.shape[1] != self.obs_dim:
+            raise ValueError("act: expected states of shape (%d,) or (E, %d), got %s"
+                             % (self.obs_dim, self.obs_dim, tuple(x.shape)))
+        E = int(x.shape[0])
+        if E < 1:
+            raise ValueError("act: no states (E = 0)")
+        if 2 * E * self.act_dim >= 2 ** 31:
+            raise ValueError("act: E = %d rows of %d actions exceed the noise draw index (2 * E * act_dim < 2^31)"
+                             % (E, self.act_dim))
+        return x, E
+
+    def _act_input(self, x, E, dev, bufs):
+        """(rows, pitch) as d4pg_act reads them.  A float32 tensor on `dev` with 16-B aligned rows is read in place;
+        anything else lands in the cached [E, pitch4(obs_dim)] buffer with one 2-D copy."""
+        S = self.obs_dim
+        if torch.is_tensor(x):
+            if x.device.type == "cpu":
+                x = x.to(torch.float32).contiguous().numpy()
+            elif x.device != dev or x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(0) < S:
+                x = x.to(device=dev, dtype=torch.float32).contiguous()
+        if torch.is_tensor(x) and x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0:
+            return x, x.stride(0)
+        if bufs[1] is None:
+            bufs[1] = torch.empty(E, (S + 3) & ~3, dtype=torch.float32, device=dev)
+        buf = bufs[1]
+        if torch.is_tensor(x):
+            src, lds = _lib.ptr(x), x.stride(0)
+        else:
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            src, lds = C.c_void_p(x.ctypes.data), S
+        _lib.check(_lib.lib().d4pg_copy_rows_f32(_lib.ptr(buf), buf.stride(0), src, lds, E, S, _lib.stream_ptr()),
+                   "d4pg_copy_rows_f32")
+        return buf, buf.stride(0)
+
+    @staticmethod
+    def _act_reset(reset, dev):
+        """The reset mask as a u8 device tensor (a bool / u8 device tensor is read in place)."""
+        if torch.is_tensor(reset):
+            r = reset.detach()
+            if r.device == dev and r.dtype in (torch.bool, torch.uint8) and r.is_contiguous():
+                return r.view(torch.uint8)
+            reset = r.cpu().numpy()
+        return torch.from_numpy(np.asarray(reset).astype(bool).astype(np.uint8)).to(dev)
 
     # ---- the hot path ----------------------------------------------------------------------
     def _drop_learner(self):

@@ -287,6 +287,35 @@ int32_t d4pg_critic_forward(const float* params, int32_t obs_dim, int32_t act_di
                             float* workspace, int32_t precision, d4pg_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Exploratory action selection (main.py:145-146,216-217,279: np.clip(actor(s) + noise.sample(), -1, 1)) in ONE launch:
+ * the actor at precision 0 as a 4-slot cluster chain, with the observation normalizer applied to the rows it reads,
+ * and the noise and the clip in fc3's epilogue.
+ *   s [E, obs_dim] f32 device rows with pitch lds (a multiple of 4 floats, 16-B aligned base; d4pg_copy_rows_f32
+ *     lands other layouts); 1 <= E and 2 * E * act_dim < 2^31;  action [E, act_dim] f32 device
+ *   norm_affine  {shift[obs_dim], scale[obs_dim]} of an observation normalizer (NULL = raw rows); then every s is
+ *     min(max((s - shift) * scale, -norm_clip), norm_clip) in fp32, as d4pg_obs_normalize computes it
+ *   noise  0: none -- action = actor(s), bit-identical to d4pg_actor_forward at precision 0
+ *          1: Gaussian, noise_params {eps, mu, var}:               n = eps * (mu + var * z)
+ *          2: Ornstein-Uhlenbeck, noise_params {eps, theta, mu, sigma, dt}; ou_state f64 [E, act_dim] device, updated in
+ *             place; rows with reset[row] != 0 (u8 [E] device, NULL = none) restart from 0 first:
+ *             x = (x + (theta * (mu - x)) * dt) + (sigma * sqrt(dt)) * z,  n = eps * x
+ *          with noise: action = f32(min(max(f64(actor(s)) + n, -1), 1)).  noise_params is host memory, read during the call.
+ *   z of element i = row * act_dim + j: u1 = Philox4x32-10 uniform53(seed, counter, 2i), u2 = (.., 2i + 1) (the device
+ *     sampler's construction), z = sqrt(-2 log(1 - u1)) * cos(2 pi u2); every fp64 operation rounded, none contracted.
+ *   workspace  d4pg_act_workspace_floats(E, obs_dim) floats of device scratch (-1: bad arguments)
+ * D4PG_ENOTSUP when the actor's fc1 does not fit one chain slot (obs_dim > 576).
+ * d4pg_copy_rows_f32: rows x width floats from src (pitch lds) to dst (pitch ldd), host or device, one 2-D copy on
+ * `stream` (no kernel).
+ * ------------------------------------------------------------------------------------- */
+int64_t d4pg_act_workspace_floats(int32_t E, int32_t obs_dim);
+int32_t d4pg_act(const float* actor_params, int32_t obs_dim, int32_t act_dim, const float* s, int64_t lds, int32_t E,
+                 const float* norm_affine, double norm_clip, int32_t noise, const double* noise_params, uint64_t seed,
+                 uint64_t counter, double* ou_state, const uint8_t* reset, float* action, float* workspace,
+                 d4pg_stream_t stream);
+int32_t d4pg_copy_rows_f32(float* dst, int64_t ldd, const float* src, int64_t lds, int64_t rows, int64_t width,
+                           d4pg_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Actor / critic backward: the autograd backward of the two forward calls above, for callers that own
  * the loss (ddpg.py:229-244 written against the modules, other losses, gradient checks).  Runs the same
  * per-layer GEMM kernels as the learner's one-launch-per-level plan at the same `precision` (3 rounds dZ and W
