@@ -20,6 +20,7 @@ from . import utils, random_process, models, obs_norm, prioritized_replay_memory
 from .ddpg import DDPG
 from .models import actor, critic, fanin_init
 from .obs_norm import ObsNormalizer
+from .random_process import AdaptiveParamNoiseSpec
 from .prioritized_replay_memory import (LinearSchedule, SegmentTree, SumSegmentTree, MinSegmentTree,
                                         ReplayBuffer, PrioritizedReplayBuffer)
 from .replay_memory import Replay

@@ -111,6 +111,8 @@ _PROTOS = {
     "d4pg_act": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_double, C.c_int32, _P,
                              C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),
     "d4pg_copy_rows_f32": (C.c_int32, [_P, C.c_int64, _P, C.c_int64, C.c_int64, C.c_int64, _P]),
+    "d4pg_actor_perturb": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_uint64, C.c_uint64, _P, _P]),
+    "d4pg_param_noise_adapt": (C.c_int32, [_P, _P, C.c_int64, C.c_double, C.c_double, _P, _P]),
     "d4pg_actor_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "d4pg_critic_backward": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P,
                                          _P, _P, _P, _P, C.c_int32, _P]),

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libd4pg_sm90.so")
 OBJ = os.path.join(HERE, "csrc", "_obj")
-SOURCES = ["abi.cu", "proj_loss.cu", "replay.cu", "obs_norm.cu", "gemm_ffma.cu", "gemm_tc.cu", "gemm_bf16.cu", "mlp_backward.cu", "mog_heads.cu", "qr_heads.cu", "adam.cu", "mlp_chain.cu", "mlp_tc_chain.cu", "learner.cu", "comm.cu", "act.cu"]
+SOURCES = ["abi.cu", "proj_loss.cu", "replay.cu", "obs_norm.cu", "gemm_ffma.cu", "gemm_tc.cu", "gemm_bf16.cu", "mlp_backward.cu", "mog_heads.cu", "qr_heads.cu", "adam.cu", "mlp_chain.cu", "mlp_tc_chain.cu", "learner.cu", "comm.cu", "act.cu", "param_noise.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off"]
 

@@ -21,10 +21,14 @@ from . import _lib
 from .models import actor, critic
 from .obs_norm import make_obs_normalizer
 from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer
-from .random_process import GaussianNoise, OrnsteinUhlenbeckProcess
+from .random_process import AdaptiveParamNoiseSpec, GaussianNoise, OrnsteinUhlenbeckProcess
 from .replay_memory import Replay
 from .shared_adam import SharedAdam, check_max_grad_norm
 from .utils import default_device
+
+# Philox counter of perturbation j (DDPG.perturb_actor / adapt_param_noise): 2^63 + 2^62 + j, apart from act()'s
+# 2^63 + k (k < 2^62) and from the learner sampler's step counter
+PERTURB_COUNTER_BASE = (1 << 63) + (1 << 62)
 
 
 class _Learner(object):
@@ -191,7 +195,11 @@ class DDPG:
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
                  importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None,
-                 obs_norm=None):
+                 obs_norm=None, param_noise=None):
+        # adaptive parameter-space exploration noise (random_process.AdaptiveParamNoiseSpec, DESIGN §3): None = off
+        if param_noise is not None and not isinstance(param_noise, AdaptiveParamNoiseSpec):
+            raise ValueError("param_noise must be None or an AdaptiveParamNoiseSpec, got %r" % (param_noise,))
+        self.param_noise = param_noise
         self.gamma = gamma
         self.n_steps = n_steps
         self.n_step_gamma = self.gamma ** self.n_steps
@@ -288,6 +296,12 @@ class DDPG:
         self._act_calls = 0
         self._exploration_state = None
         self._act_buffers = {}
+        # parameter noise: perturbations drawn so far (the Philox counter of the next is PERTURB_COUNTER_BASE + this),
+        # the device {sigma, last distance}, the rollout's perturbed actor and adapt_param_noise's own perturbed copy
+        self._perturbations = 0
+        self._param_noise_state = None
+        self._perturbed_actor = None
+        self._adaptive_flat = None
 
         self.prioritized_replay = prioritized_replay
         if self.prioritized_replay:                                                          # ddpg.py:78-87
@@ -388,7 +402,12 @@ class DDPG:
         OrnsteinUhlenbeckProcess, whose epsilon / mu / var (theta / sigma / dt) are read at each call -- drawn on the
         device from Philox (key philox_seed, counter 2^63 + the number of earlier exploring calls), and clips to
         [-1, 1] in fp64.  OU noise keeps one state row per environment in `exploration_state`; `reset` (bool [E]) restarts
-        the rows of environments that began a new episode.  The arithmetic is in DESIGN.md §3 "Exploration"."""
+        the rows of environments that began a new episode.  The arithmetic is in DESIGN.md §3 "Exploration".
+
+        With DDPG(param_noise=...), explore=True runs `perturbed_actor` instead of the actor (drawing perturbation 0
+        first if none was drawn yet) and adds the noise of `self.noise` to it; self.noise = None is parameter noise
+        alone.  explore=False still runs the actor itself.  `reset` never re-perturbs (DESIGN.md §3 "Parameter-space
+        noise")."""
         mode, params = self._act_noise(explore)
         x, E = self._act_rows(state)
         if mode == 2:
@@ -403,9 +422,12 @@ class DDPG:
         S, A = self.obs_dim, self.act_dim
         flat = self.actor.flat_params()
         dev = flat.device
-        bufs = self._act_buffers.get(E)
-        if bufs is None or bufs[0].device != dev:
-            bufs = self._act_buffers[E] = [torch.empty(L.d4pg_act_workspace_floats(E, S), dtype=torch.float32, device=dev), None]
+        if explore and self.param_noise is not None:
+            pa = self._perturbed_actor
+            if pa is None or pa.flat_params().device != dev:
+                pa = self.perturb_actor()
+            flat = pa.flat_params()
+        bufs = self._act_workspace(E, dev)
         rows, lds = self._act_input(x, E, dev, bufs)
         st = rmask = None
         if mode == 2:
@@ -413,12 +435,7 @@ class DDPG:
             if st is None:
                 st = torch.from_numpy(np.zeros((E, A))).to(dev)          # a copy, not a fill kernel
             rmask = self._act_reset(reset, dev) if reset is not None else None
-        norm = self.obs_normalizer
-        affine, clip = None, 0.0
-        if norm is not None:
-            norm._require()
-            norm._join()
-            affine, clip = _lib.ptr(norm.affine), norm.clip
+        affine, clip = self._act_affine()
         out = torch.empty(E, A, dtype=torch.float32, device=dev)
         p = (C.c_double * 5)(*params)
         counter = (1 << 63) + self._act_calls
@@ -448,12 +465,31 @@ class DDPG:
         if not explore:
             return 0, ()
         nz = self.noise
+        if self._param_noise_args() is not None and nz is None:
+            return 0, ()                                  # parameter noise alone
         if isinstance(nz, GaussianNoise):
             return 1, tuple(float(v) for v in (nz.epsilon, nz.mu, nz.var))
         if isinstance(nz, OrnsteinUhlenbeckProcess):
             return 2, tuple(float(v) for v in (nz.epsilon, nz.theta, nz.mu, nz.sigma, nz.dt))
         raise _lib.D4PGError("act(explore=True) draws GaussianNoise or OrnsteinUhlenbeckProcess noise on the device; "
                              "self.noise is a %s" % type(nz).__name__)
+
+    def _act_workspace(self, E, dev):
+        """[d4pg_act workspace, pitch-4 input buffer or None] cached per E."""
+        bufs = self._act_buffers.get(E)
+        if bufs is None or bufs[0].device != dev:
+            ws = torch.empty(_lib.lib().d4pg_act_workspace_floats(E, self.obs_dim), dtype=torch.float32, device=dev)
+            bufs = self._act_buffers[E] = [ws, None]
+        return bufs
+
+    def _act_affine(self):
+        """(affine pointer, clip) of the observation normalizer for d4pg_act, (None, 0.0) without one."""
+        norm = self.obs_normalizer
+        if norm is None:
+            return None, 0.0
+        norm._require()
+        norm._join()
+        return _lib.ptr(norm.affine), norm.clip
 
     def _act_rows(self, state):
         """(rows, E): `state` as [E, obs_dim], a tensor where it lives, anything else as float32 numpy."""
@@ -503,6 +539,106 @@ class DDPG:
                 return r.view(torch.uint8)
             reset = r.cpu().numpy()
         return torch.from_numpy(np.asarray(reset).astype(bool).astype(np.uint8)).to(dev)
+
+    # ---- parameter-space noise ----------------------------------------------------------------
+    def _param_noise_args(self):
+        """`self.param_noise.check()` -- (initial_stddev, desired_action_stddev, adoption_coefficient) -- or None when
+        parameter noise is off.  Raises ValueError for anything else, before any device work."""
+        spec = self.param_noise
+        if spec is None:
+            return None
+        if not isinstance(spec, AdaptiveParamNoiseSpec):
+            raise ValueError("param_noise must be None or an AdaptiveParamNoiseSpec, got %r" % (spec,))
+        return spec.check()
+
+    def _require_param_noise(self, what):
+        args = self._param_noise_args()
+        if args is None:
+            raise _lib.D4PGError("%s needs DDPG(param_noise=AdaptiveParamNoiseSpec(...))" % what)
+        return args
+
+    def _noise_state(self, dev, initial_stddev):
+        st = self._param_noise_state
+        if st is None or st.device != dev:
+            st = torch.tensor([initial_stddev, float("nan")], dtype=torch.float64).to(dev)     # a copy, not a fill kernel
+            self._param_noise_state = st
+        return st
+
+    def _perturb(self, src, dst, initial_stddev):
+        """dst = src + sigma * N(0, 1) per logical parameter: perturbation j = self._perturbations (one launch)."""
+        st = self._noise_state(src.device, initial_stddev)
+        _lib.check(_lib.lib().d4pg_actor_perturb(_lib.ptr(src), self.obs_dim, self.act_dim, _lib.ptr(st),
+                                                 int(self.philox_seed) & 0xFFFFFFFFFFFFFFFF,
+                                                 PERTURB_COUNTER_BASE + self._perturbations, _lib.ptr(dst),
+                                                 _lib.stream_ptr()), "d4pg_actor_perturb")
+        self._perturbations += 1
+
+    def perturb_actor(self):
+        """Draw the next parameter perturbation of the actor into `perturbed_actor` (one launch on the caller's stream)
+        and return that module.  Baselines' perturb_policy: call it at the start of every episode.  Reads the actor's
+        current parameters and the device sigma of `param_noise_state`; the result is a snapshot that later train()
+        steps do not change.  Perturbation j (j counts this DDPG's perturbations, including adapt_param_noise's, from 0)
+        adds sigma * z to logical parameter i, z from Philox (key philox_seed, counter 2^63 + 2^62 + j, lanes 2i / 2i + 1);
+        DESIGN.md §3 "Parameter-space noise"."""
+        initial, _, _ = self._require_param_noise("perturb_actor")
+        _lib.require_cuda()
+        src = self.actor.flat_params()
+        pa = self._perturbed_actor
+        if pa is None or pa.flat_params().device != src.device:
+            pa = actor.unfilled(self.obs_dim, self.act_dim, device=src.device)
+            if self.obs_normalizer is not None:
+                pa.obs_normalizer = self.obs_normalizer
+            self._perturbed_actor = pa
+        self._perturb(src, pa.flat_params(), initial)
+        return pa
+
+    def adapt_param_noise(self, states):
+        """Adapt sigma to the policy distance on `states` ([B, obs_dim] raw observations, host or device; act()'s limits
+        on B): perturb an adaptive copy of the actor with the current sigma (perturbation j), run the actor and the copy
+        on the states without action noise, d = sqrt(mean((a_perturbed - a)^2)) in fp64, then sigma = sigma /
+        adoption_coefficient if d > desired_action_stddev else sigma * adoption_coefficient.  Four launches on the
+        caller's stream; returns d as a 0-d fp64 device tensor (a view of param_noise_state), without synchronising.
+        `perturbed_actor` is not touched.  Baselines calls this every ~50 training steps on a replay batch."""
+        initial, desired, coef = self._require_param_noise("adapt_param_noise")
+        x, E = self._act_rows(states)
+        _lib.require_cuda()
+        L = _lib.lib()
+        S, A = self.obs_dim, self.act_dim
+        src = self.actor.flat_params()
+        dev = src.device
+        ad = self._adaptive_flat
+        if ad is None or ad.device != dev:
+            ad = self._adaptive_flat = torch.empty(self.actor._total, dtype=torch.float32, device=dev)
+        bufs = self._act_workspace(E, dev)
+        rows, lds = self._act_input(x, E, dev, bufs)
+        affine, clip = self._act_affine()
+        self._perturb(src, ad, initial)
+        out = torch.empty(2, E, A, dtype=torch.float32, device=dev)
+        for k, flat in enumerate((src, ad)):
+            _lib.check(L.d4pg_act(_lib.ptr(flat), S, A, _lib.ptr(rows), lds, E, affine, clip, 0, None, 0, 0, None, None,
+                                  _lib.ptr(out[k]), _lib.ptr(bufs[0]), _lib.stream_ptr()), "d4pg_act")
+        st = self._param_noise_state
+        _lib.check(L.d4pg_param_noise_adapt(_lib.ptr(out[0]), _lib.ptr(out[1]), E * A, desired, coef, _lib.ptr(st),
+                                            _lib.stream_ptr()), "d4pg_param_noise_adapt")
+        return st[1]
+
+    @property
+    def perturbed_actor(self):
+        """The actor with the most recent perturb_actor() draw (an `actor` module: same dimensions and device, this
+        DDPG's observation normalizer, precision 0), or None before the first.  Never part of the learner."""
+        return self._perturbed_actor
+
+    @property
+    def param_noise_state(self):
+        """fp64 [2] device tensor {sigma, last distance}: None until the first perturbation or adaptation, which
+        creates it as {initial_stddev, NaN}.  Assign None to drop it: the next use starts again from initial_stddev."""
+        return self._param_noise_state
+
+    @param_noise_state.setter
+    def param_noise_state(self, value):
+        if value is not None:
+            raise ValueError("param_noise_state can only be set to None")
+        self._param_noise_state = None
 
     # ---- the hot path ----------------------------------------------------------------------
     def _drop_learner(self):

@@ -63,12 +63,13 @@ class _FlatNet(nn.Module):
     # attaches its normalizer to all four networks); the critic's action input is never normalized
     obs_normalizer = None
 
-    def __init__(self, dims, device=None):
+    def __init__(self, dims, device=None, empty=False):
         super().__init__()
         self._dims = list(dims)
         self._offsets, self._sizes, self._total, self._pitch = _layout_py(self._dims)
         self._device = torch.device(device) if device is not None else default_device()
-        self._flat = torch.zeros(self._total, dtype=torch.float32, device=self._device)
+        # empty=True: the buffer is left unwritten for a kernel that writes every float of it, pads included
+        self._flat = (torch.empty if empty else torch.zeros)(self._total, dtype=torch.float32, device=self._device)
         self._flat_grad = None
         for name, (fin, fout) in zip(_LAYER_NAMES, self._dims):
             setattr(self, name, _LinearView(fin, fout))
@@ -249,6 +250,16 @@ class actor(_FlatNet):
         super().__init__([(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)], device)
         self.differentiable = bool(differentiable)
         self.init_weights()
+
+    @classmethod
+    def unfilled(cls, input_size, output_size, device=None):
+        """An actor whose flat buffer is allocated but not written: no RNG draw and no kernel.  For a buffer a kernel
+        fills completely (DDPG.perturbed_actor)."""
+        net = cls.__new__(cls)
+        net.input_size, net.output_size = input_size, output_size
+        _FlatNet.__init__(net, [(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)], device,
+                          empty=True)
+        return net
 
     def init_weights(self, init_w=10e-3):
         # same CPU-RNG consumption as the reference: 4 nn.Linear ctors, 3 fan-in normals, fc3 normal

@@ -316,6 +316,30 @@ int32_t d4pg_copy_rows_f32(float* dst, int64_t ldd, const float* src, int64_t ld
                            d4pg_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Adaptive parameter-space exploration noise (Plappert et al. 2018, "Parameter Space Noise for Exploration"; the
+ * baselines DDPG's AdaptiveParamNoiseSpec).  The reference has none; these semantics are the library's own.
+ *   noise_state  f64 [2] device {sigma, last distance}; sigma is read on the device, so both calls can be captured
+ *
+ * d4pg_actor_perturb: out = the actor `params` (d4pg_actor_layout(obs_dim, act_dim) order) with Gaussian noise of std
+ *   dev sigma added to every parameter, in one launch.  Logical element i is the i-th float of the unpadded
+ *   concatenation fc1.weight, fc1.bias, ..., fc3.bias (nn.Module parameter order, row-major weights):
+ *     u1 = Philox4x32-10 uniform53(seed, counter, 2i), u2 = (.., 2i + 1), z = sqrt(-2 log(1 - u1)) * cos(2 pi u2),
+ *     out_i = f32(f64(p_i) + sigma * z), every fp64 operation rounded, none contracted (d4pg_act's construction).
+ *   Every padding float of out (row pitch columns, tensor alignment gaps) is written as 0.  params and out: 16-B
+ *   aligned, both d4pg_actor_layout().total floats; count = the logical parameter count, 2 * count < 2^32.
+ * d4pg_param_noise_adapt: the policy distance of two action planes a, a_perturbed [n] f32 (n >= 1, usually the actor's
+ *   and the perturbed actor's d4pg_act outputs on the same states):
+ *     d = sqrt(sum_i (f64(a_perturbed_i) - f64(a_i))^2 / n) in fp64 (one CTA, fixed summation order, no atomics),
+ *     sigma = d > desired_stddev ? sigma / coefficient : sigma * coefficient;  noise_state = {sigma, d}.
+ *   desired_stddev finite and > 0, coefficient finite and > 1.
+ * Bad arguments fail with D4PG_EINVAL before any device work.
+ * ------------------------------------------------------------------------------------- */
+int32_t d4pg_actor_perturb(const float* params, int32_t obs_dim, int32_t act_dim, const double* noise_state,
+                           uint64_t seed, uint64_t counter, float* out, d4pg_stream_t stream);
+int32_t d4pg_param_noise_adapt(const float* a, const float* a_perturbed, int64_t n, double desired_stddev,
+                               double coefficient, double* noise_state, d4pg_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Actor / critic backward: the autograd backward of the two forward calls above, for callers that own
  * the loss (ddpg.py:229-244 written against the modules, other losses, gradient checks).  Runs the same
  * per-layer GEMM kernels as the learner's one-launch-per-level plan at the same `precision` (3 rounds dZ and W
