@@ -15,6 +15,7 @@ PROJ_TARGET_IS_PROBS, PROJ_Q_IS_PROBS = 1, 2
 HIDDEN = 256
 MAX_ATOMS = 128
 MAX_COMPONENTS = 32
+STEPS_MAX_N = 64          # D4PG_STEPS_MAX_N: the longest n-step window of d4pg_replay_add_steps
 
 c_float_p = C.POINTER(C.c_float)
 c_double_p = C.POINTER(C.c_double)
@@ -98,6 +99,9 @@ _PROTOS = {
     "d4pg_replay_set_leaves": (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P]),
     "d4pg_nstep_returns": (C.c_int32, [_P, C.c_int64, C.c_int32, C.c_double, _P, _P]),
     "d4pg_replay_add_nstep": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int32, _P]),
+    "d4pg_replay_steps_window_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
+    "d4pg_replay_add_steps": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int64,
+                                          C.c_int32, _P]),
     "d4pg_her_relabel": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                      C.c_double, C.c_int32, _P, _P, _P, _P, _P, _P]),
     "d4pg_replay_set_len": (C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int32, _P]),

@@ -466,15 +466,116 @@ extern "C" int32_t d4pg_replay_set_staging(d4pg_replay_t* h, void* pinned_host, 
 // Transition i of an episode of T steps: (s_i, a_i, sum_{k<n} gamma^k r_{i+k}, s'_{i+n-1}, done_{i+n-1}).  Only the
 // reward needs arithmetic -- s'/done are the same arrays shifted by n-1 rows -- and it is the reference's own
 // left-to-right f64 loop (`cum += exp_gamma * r; exp_gamma *= gamma`) with explicit _rn ops (no FMA contraction).
+// nstep_return is that loop over n consecutive rewards; the episode kernel and the streaming windows both call it.
+__device__ __forceinline__ double nstep_return(const double* __restrict__ r, int n, double gamma) {
+  double cum = 0.0, eg = 1.0;
+  for (int k = 0; k < n; ++k) {
+    cum = __dadd_rn(cum, __dmul_rn(eg, r[k]));
+    eg = __dmul_rn(eg, gamma);
+  }
+  return cum;
+}
+
 __global__ void nstep_returns_kernel(const double* __restrict__ rew, int64_t T, int n, double gamma, double* __restrict__ out) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i + n > T) return;
-  double cum = 0.0, eg = 1.0;
-  for (int k = 0; k < n; ++k) {
-    cum = __dadd_rn(cum, __dmul_rn(eg, rew[i + k]));
-    eg = __dmul_rn(eg, gamma);
+  out[i] = nstep_return(rew + i, n, gamma);
+}
+
+// ---- device-side ingest: streaming n-step windows of E environments (DESIGN.md §3 "Streaming n-step insert") ------
+// One call = one vector step.  Environment e appends (s, a, r) to its window; once the window holds n steps of the
+// current episode it emits (s_{t-n+1}, a_{t-n+1}, R, s'_t, terminated_t), R = nstep_return over the window's rewards;
+// then an episode end clears the window.  Emitting environments take consecutive ring rows in ascending e.
+//
+// Window state (caller-owned, zero-filled before the first call; d4pg_replay_steps_window_bytes):
+//   rec u64 [E]      {bits 0-31: id of the last call, 32-39: fill before it, 40-47: fill after it}
+//   wr  f64 [E, 2n]  reward of step u at u % n AND u % n + n, so the last n rewards are contiguous from (fill+1) % n
+//   ws  f32 [E, n, S], wa f32 [E, n, A]: s / a of step u at u % n (not written for n = 1)
+// fill counts the steps of the current episode, kept in [0, 2n) by subtracting n (u % n is all that is used).
+// The emit decision of e needs the fill BEFORE this call; a CTA counts the emitters below its first environment from
+// the other CTAs' records, which may or may not have been rewritten yet: a record carrying this call's id holds the
+// old fill in bits 32-39.  Every record carries the same call id between calls, because every call steps all E.
+constexpr int STEPS_THREADS = 256, STEPS_WARPS = STEPS_THREADS / 32;
+struct StepsArgs {
+  const float* obs; const float* act; const double* rew; const float* obs2; const uint8_t* term; const uint8_t* end;
+  int64_t E, chunk; int S, A, n; double gamma;
+  unsigned long long* rec; double* wr; float* ws; float* wa;
+  float* r_obs; float* r_act; double* r_rew; float* r_obs2; uint8_t* r_done;
+  int64_t size, start, n_rows, new_len, new_next; ReplayState* state;
+};
+
+__device__ __forceinline__ int steps_fill_before(unsigned long long rec, unsigned kprev) {
+  return int(((unsigned)rec == kprev ? rec >> 40 : rec >> 32) & 0xff);
+}
+
+__global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const StepsArgs a) {
+  __shared__ int red[STEPS_WARPS];
+  __shared__ int fill_s[STEPS_THREADS], rank_s[STEPS_THREADS];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5, n = a.n, S = a.S, A = a.A;
+  const int64_t e0 = int64_t(blockIdx.x) * a.chunk, e1 = min(a.E, e0 + a.chunk);
+  if (blockIdx.x == 0 && t == 0) { a.state->len = a.new_len; a.state->next_idx = a.new_next; }
+  // this CTA rewrites its own records only after the barriers below, so rec[e0] still has the previous call's id
+  const unsigned kprev = (unsigned)__ldcg(a.rec + e0);
+  // emitting environments in [0, e0)
+  int c = 0;
+  for (int64_t e = t; e < e0; e += STEPS_THREADS) c += steps_fill_before(__ldcg(a.rec + e), kprev) >= n - 1;
+  c = __reduce_add_sync(0xffffffffu, c);
+  if (lane == 0) red[w] = c;
+  __syncthreads();
+  int64_t base = 0;
+  for (int i = 0; i < STEPS_WARPS; ++i) base += red[i];
+  for (int64_t tile = e0; tile < e1; tile += STEPS_THREADS) {
+    // exclusive rank of this tile's emitters
+    const int64_t e = tile + t;
+    const int fill = e < e1 ? steps_fill_before(__ldcg(a.rec + e), kprev) : 0;
+    const bool emit = e < e1 && fill >= n - 1;
+    const unsigned bal = __ballot_sync(0xffffffffu, emit);
+    __syncthreads();                                   // red[] of the previous tile / the prefix count is consumed
+    if (lane == 0) red[w] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int i = 0; i < STEPS_WARPS; ++i) { before += i < w ? red[i] : 0; total += red[i]; }
+    fill_s[t] = fill;
+    rank_s[t] = before + __popc(bal & ((1u << lane) - 1u));
+    __syncthreads();
+    const int cnt = int(min(int64_t(STEPS_THREADS), e1 - tile));
+    for (int j = w; j < cnt; j += STEPS_WARPS) {
+      const int64_t ee = tile + j;
+      const int f = fill_s[j], slot = f % n, old = (f + 1) % n;
+      const int64_t rank = base + rank_s[j];
+      const bool write = f >= n - 1 && rank < a.n_rows;       // never outside [start, start + n_rows)
+      const int64_t p = (a.start + rank) % a.size;
+      const float* s_in = a.obs + ee * S;
+      float* ws = a.ws + ee * n * S;
+      for (int k = lane; k < S; k += 32) {
+        const float v = s_in[k];
+        if (n > 1) ws[slot * S + k] = v;
+        if (write) {
+          a.r_obs[p * S + k] = n > 1 ? ws[old * S + k] : v;
+          a.r_obs2[p * S + k] = a.obs2[ee * S + k];
+        }
+      }
+      const float* a_in = a.act + ee * A;
+      float* wa = a.wa + ee * n * A;
+      for (int k = lane; k < A; k += 32) {
+        const float v = a_in[k];
+        if (n > 1) wa[slot * A + k] = v;
+        if (write) a.r_act[p * A + k] = n > 1 ? wa[old * A + k] : v;
+      }
+      if (lane == 0) {
+        double* wr = a.wr + ee * 2 * n;
+        if (n > 1) { const double r = a.rew[ee]; wr[slot] = r; wr[slot + n] = r; }
+        const bool term = a.term[ee] != 0, ended = term || (a.end && a.end[ee] != 0);
+        if (write) {
+          a.r_rew[p] = nstep_return(n > 1 ? wr + old : a.rew + ee, n, a.gamma);
+          a.r_done[p] = term ? 1 : 0;
+        }
+        const int nf = ended ? 0 : (f + 1 >= 2 * n ? f + 1 - n : f + 1);
+        a.rec[ee] = (unsigned long long)(kprev + 1u) | ((unsigned long long)f << 32) | ((unsigned long long)nf << 40);
+      }
+    }
+    base += total;
   }
-  out[i] = cum;
 }
 
 extern "C" int32_t d4pg_nstep_returns(const double* rew, int64_t T, int32_t n_steps, double gamma, double* out,
@@ -674,26 +775,21 @@ extern "C" int32_t d4pg_replay_obs_norm_refresh(d4pg_replay_t* h, d4pg_stream_t 
   return launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, nullptr, 0, h->obs_dim, h->norm_eps, as_stream(stream));
 }
 
-extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs, const float* act,
-                                   const double* rew, const float* obs2, const uint8_t* done,
-                                   int32_t prioritized, d4pg_stream_t stream) {
-  if (h) ++h->gen;
-  D4PG_REQUIRE(h && obs && act && rew && obs2 && done, D4PG_EINVAL, "d4pg_replay_add: null argument");
-  D4PG_REQUIRE(n > 0 && n <= h->size, D4PG_EINVAL, "d4pg_replay_add: need 0 < n <= size (n=%lld)", (long long)n);
-  cudaStream_t st = as_stream(stream);
-  const int64_t start = h->next_idx;
-  const int64_t new_len = std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n));
-  const int64_t new_next = (start + n) % h->size;
-  const int blocks = int(std::min<int64_t>(4 * device_sm_count(), (n * h->obs_dim + 255) / 256));   // grid-stride
-  ring_write_kernel<<<blocks, 256, 0, st>>>(h->obs, h->act, h->rew, h->obs2, h->done, obs, act, rew, obs2, done,
-                                             n, h->obs_dim, h->act_dim, h->size, start,
-                                             reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
-  D4PG_LAUNCH_OK();
+namespace {
+// What every insert runs after its ring write of n rows at [start, start + n) (mod size): the normalizer's fold over
+// the same rows in insertion order (rows1 [n1, obs_dim], then rows2 [n - n1, obs_dim]), then, prioritized, the ingest
+// gate and the tree add of the new leaves; last, the host mirror of len / next_idx.
+int replay_insert_tail(d4pg_replay* h, int64_t n, int64_t start, int64_t new_len, int64_t new_next,
+                       const float* rows1, int64_t n1, const float* rows2, int32_t prioritized, cudaStream_t st) {
   if (h->norm_stats) {
     // the normalizer's statistics: the same rows, in the same order.  Before the ingest gate and the tree kernels, so
     // the host pipeline's tree add stays the kernel the presample is programmatically dependent on
-    int nrc = launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, obs, n, h->obs_dim, h->norm_eps, st);
+    int nrc = launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, rows1, n1, h->obs_dim, h->norm_eps, st);
     if (nrc) return nrc;
+    if (n1 < n) {
+      nrc = launch_obs_stats(h->norm_stats, h->norm_affine, h->obs_dim, rows2, n - n1, h->obs_dim, h->norm_eps, st);
+      if (nrc) return nrc;
+    }
   }
   if (prioritized) {
     // ingest gate (host pipeline): the rows above only had to follow the previous gather (stream order); the trees wait for
@@ -739,6 +835,78 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
   h->len = new_len;
   h->next_idx = new_next;
   return D4PG_OK;
+}
+
+struct StepsLayout { int64_t rec, wr, ws, wa, total; };
+StepsLayout steps_layout(int64_t E, int64_t S, int64_t A, int64_t n) {
+  auto up = [](int64_t b) { return (b + 15) & ~int64_t(15); };
+  StepsLayout l;
+  l.rec = 0;
+  l.wr = up(l.rec + E * 8);
+  l.ws = up(l.wr + E * 2 * n * 8);
+  l.wa = up(l.ws + E * n * S * 4);
+  l.total = up(l.wa + E * n * A * 4);
+  return l;
+}
+}  // namespace
+
+extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs, const float* act,
+                                   const double* rew, const float* obs2, const uint8_t* done,
+                                   int32_t prioritized, d4pg_stream_t stream) {
+  if (h) ++h->gen;
+  D4PG_REQUIRE(h && obs && act && rew && obs2 && done, D4PG_EINVAL, "d4pg_replay_add: null argument");
+  D4PG_REQUIRE(n > 0 && n <= h->size, D4PG_EINVAL, "d4pg_replay_add: need 0 < n <= size (n=%lld)", (long long)n);
+  cudaStream_t st = as_stream(stream);
+  const int64_t start = h->next_idx;
+  const int64_t new_len = std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n));
+  const int64_t new_next = (start + n) % h->size;
+  const int blocks = int(std::min<int64_t>(4 * device_sm_count(), (n * h->obs_dim + 255) / 256));   // grid-stride
+  ring_write_kernel<<<blocks, 256, 0, st>>>(h->obs, h->act, h->rew, h->obs2, h->done, obs, act, rew, obs2, done,
+                                             n, h->obs_dim, h->act_dim, h->size, start,
+                                             reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
+  D4PG_LAUNCH_OK();
+  return replay_insert_tail(h, n, start, new_len, new_next, obs, n, nullptr, prioritized, st);
+}
+
+extern "C" int64_t d4pg_replay_steps_window_bytes(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps) {
+  if (E <= 0 || obs_dim <= 0 || act_dim <= 0 || n_steps < 1 || n_steps > D4PG_STEPS_MAX_N) return -1;
+  return steps_layout(E, obs_dim, act_dim, n_steps).total;
+}
+
+extern "C" int32_t d4pg_replay_add_steps(d4pg_replay_t* h, int64_t E, const float* obs, const float* act, const double* rew,
+                                         const float* obs2, const uint8_t* terminated, const uint8_t* episode_end,
+                                         int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t prioritized,
+                                         d4pg_stream_t stream) {
+  if (h && n_rows > 0) ++h->gen;          // a call that inserts no row leaves the store, and a prefetched batch, valid
+  D4PG_REQUIRE(h && obs && act && rew && obs2 && terminated && window, D4PG_EINVAL, "d4pg_replay_add_steps: null argument");
+  D4PG_REQUIRE(E > 0 && E <= h->size, D4PG_EINVAL, "d4pg_replay_add_steps: need 0 < E <= size (E=%lld)", (long long)E);
+  D4PG_REQUIRE(n_steps >= 1 && n_steps <= D4PG_STEPS_MAX_N, D4PG_EINVAL, "d4pg_replay_add_steps: need 1 <= n_steps <= %d (got %d)",
+               D4PG_STEPS_MAX_N, n_steps);
+  D4PG_REQUIRE(n_rows >= 0 && n_rows <= E, D4PG_EINVAL, "d4pg_replay_add_steps: need 0 <= n_rows <= E (n_rows=%lld)",
+               (long long)n_rows);
+  cudaStream_t st = as_stream(stream);
+  const int64_t start = h->next_idx;
+  const int64_t new_len = n_rows ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n_rows)) : h->len;
+  const int64_t new_next = (start + n_rows) % h->size;
+  const StepsLayout l = steps_layout(E, h->obs_dim, h->act_dim, n_steps);
+  uint8_t* wb = static_cast<uint8_t*>(window);
+  StepsArgs a{};
+  a.obs = obs; a.act = act; a.rew = rew; a.obs2 = obs2; a.term = terminated; a.end = episode_end;
+  a.E = E; a.S = h->obs_dim; a.A = h->act_dim; a.n = n_steps; a.gamma = gamma;
+  a.rec = reinterpret_cast<unsigned long long*>(wb + l.rec); a.wr = reinterpret_cast<double*>(wb + l.wr);
+  a.ws = reinterpret_cast<float*>(wb + l.ws); a.wa = reinterpret_cast<float*>(wb + l.wa);
+  a.r_obs = h->obs; a.r_act = h->act; a.r_rew = h->rew; a.r_obs2 = h->obs2; a.r_done = h->done;
+  a.size = h->size; a.start = start; a.n_rows = n_rows; a.new_len = new_len; a.new_next = new_next;
+  a.state = reinterpret_cast<ReplayState*>(h->state);
+  // a CTA takes a contiguous chunk of environments, one warp per environment; the grid is at most 4 CTAs per SM
+  const int64_t blocks = std::min<int64_t>((E + STEPS_WARPS - 1) / STEPS_WARPS, 4 * device_sm_count());
+  a.chunk = (E + blocks - 1) / blocks;
+  replay_add_steps_kernel<<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
+  D4PG_LAUNCH_OK();
+  if (n_rows == 0) return D4PG_OK;
+  // the rows just written, read back from the ring in insertion order: [start, size) then [0, ...)
+  const int64_t n1 = std::min<int64_t>(n_rows, h->size - start);
+  return replay_insert_tail(h, n_rows, start, new_len, new_next, h->obs + start * h->obs_dim, n1, h->obs, prioritized, st);
 }
 
 extern "C" int32_t d4pg_replay_sample(d4pg_replay_t* h, int32_t B, const double* uniforms,

@@ -391,6 +391,15 @@ class DDPG:
             states, actions, rewards, next_states, terminates = self.replayBuffer.sample(self.batch_size)
         return states, actions, rewards, next_states, terminates, weights, batch_idxes
 
+    # ---- storing transitions -----------------------------------------------------------------
+    def observe(self, s, a, r, s2, terminated, truncated=None):
+        """Store one vector step of E environments: `replayBuffer.add_steps(..., n_steps=self.n_steps, gamma=self.gamma)`,
+        the n-step windows kept on the device (DESIGN.md §3 "Streaming n-step insert").  s / s2 [E, obs_dim] (s2 the
+        true next or final observation), a [E, act_dim] (e.g. what act() returned), r [E], terminated / truncated bool
+        [E]; numpy, CPU or CUDA tensors.  With `a = ddpg.act(s)` and device-resident environments the rollout step
+        stays on the device.  Returns the number of rows inserted."""
+        return self.replayBuffer.add_steps(s, a, r, s2, terminated, truncated, n_steps=self.n_steps, gamma=self.gamma)
+
     # ---- action selection -------------------------------------------------------------------
     def act(self, state, explore=True, reset=None):
         """The rollout's action, `np.clip(actor(s) + noise.sample(), -1, 1)` (main.py:145-146, 216-217, 279), for E

@@ -41,6 +41,31 @@ class LinearSchedule(object):
         return self.initial_p + fraction * (self.final_p - self.initial_p)
 
 
+class StepsMirror(object):
+    """add_steps' pending n-step windows: the fixed (E, n, gamma), the host mirror of each window's fill (steps of the
+    current episode, capped at n - 1, which is all the emit decision needs) and the device state (window bytes, the
+    pinned slot the end flags of a call with CUDA flags are copied back into, and that copy's event).  Environment e
+    emits a row at a call iff fill[e] == n - 1 before it, so the count is exact before the call without a device read."""
+
+    def __init__(self, E, n, gamma):
+        self.E, self.n, self.gamma = int(E), int(n), float(gamma)
+        self.fill = np.zeros(self.E, dtype=np.int64)
+        self.window = self.ends = self.event = None
+        self.pending = False
+
+    def rows(self):
+        """Rows the next call inserts."""
+        return int(np.count_nonzero(self.fill >= self.n - 1))
+
+    def advance(self):
+        """Every environment took one step."""
+        np.minimum(self.fill + 1, self.n - 1, out=self.fill)
+
+    def end(self, ended):
+        """Clear the windows of the environments whose episode ended (bool [E])."""
+        self.fill[np.asarray(ended, dtype=bool)] = 0
+
+
 class _DeviceReplay(object):
     """Device storage + trees + the C handle.  Allocated lazily on the first add (the
     reference constructors do not know obs/act dims)."""
@@ -58,6 +83,7 @@ class _DeviceReplay(object):
         self._n_staged = 0
         self._len = 0
         self._next_idx = 0
+        self._steps = None               # add_steps: the device windows and the host mirror of their fills
         # host pipeline (a learner's ingest stream, ddpg.py): add_batch_host is issued there; every other device
         # operation runs on the caller's stream -- the two are kept in program order by events, only when they interleave
         self._ingest_stream = None
@@ -325,6 +351,92 @@ class _DeviceReplay(object):
         self._add_device(n_out, outs)
         return n_out
 
+    # -- streaming n-step insert (DESIGN.md §3 "Streaming n-step insert") ------------------------------------------
+    def _check_steps(self, obs, action, reward, obs_next, terminated, truncated, n_steps, gamma):
+        """Shapes and the fixed (E, n_steps, gamma) of the pending windows, before any device work -> (E, S, A)."""
+        if isinstance(n_steps, bool) or int(n_steps) != n_steps or not 1 <= int(n_steps) <= _lib.STEPS_MAX_N:
+            raise ValueError("add_steps: n_steps must be an integer in [1, %d], got %r" % (_lib.STEPS_MAX_N, n_steps))
+        shape = lambda x: tuple(x.shape) if hasattr(x, "shape") else np.shape(x)
+        so, sa = shape(obs), shape(action)
+        if len(so) != 2 or len(sa) != 2 or so[0] < 1:
+            raise ValueError("add_steps: obs and action must be [E, obs_dim] / [E, act_dim], got %s / %s" % (so, sa))
+        E, S, A = so[0], so[1], sa[1]
+        if sa[0] != E or shape(obs_next) != (E, S) or shape(reward) != (E,) or shape(terminated) != (E,) \
+                or (truncated is not None and shape(truncated) != (E,)):
+            raise ValueError("add_steps: shapes must be obs / obs_next [E, obs_dim], action [E, act_dim], reward / "
+                             "terminated / truncated [E]; got %s %s %s %s %s %s" % (so, sa, shape(reward), shape(obs_next),
+                                                                                 shape(terminated), shape(truncated)))
+        if self.obs_dim is not None and (S, A) != (self.obs_dim, self.act_dim):
+            raise ValueError("add_steps: rows of (%d, %d) into a buffer of (%d, %d)" % (S, A, self.obs_dim, self.act_dim))
+        if E > self.size:
+            raise ValueError("add_steps: E = %d environments exceed the buffer size %d" % (E, self.size))
+        w = self._steps
+        if w is not None and (w.E, w.n, w.gamma) != (E, int(n_steps), float(gamma)):
+            raise ValueError("add_steps: the pending windows hold E=%d, n_steps=%d, gamma=%r; this call has E=%d, "
+                             "n_steps=%d, gamma=%r (drop_steps() discards them)" % (w.E, w.n, w.gamma, E,
+                                                                                    int(n_steps), float(gamma)))
+        return E, S, A
+
+    def add_steps(self, obs, action, reward, obs_next, terminated, truncated=None, n_steps=1, gamma=0.99):
+        """One vector step of E environments into per-environment n-step windows on the device; the rows of the windows
+        that are full go straight into the ring in one launch.  Returns the number of rows inserted, known on the host
+        without a device read (a mirror of the window fills).  See ReplayBuffer.add_steps."""
+        E, S, A = self._check_steps(obs, action, reward, obs_next, terminated, truncated, n_steps, gamma)
+        n, gamma = int(n_steps), float(gamma)
+        if self.handle is None:
+            self._allocate(S, A)
+        self.flush()
+        dev = self.device
+        w = self._steps
+        if w is None:
+            w = self._steps = StepsMirror(E, n, gamma)
+        if w.window is None:
+            nbytes = int(_lib.lib().d4pg_replay_steps_window_bytes(E, S, A, n))
+            w.window = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+            w.ends = torch.zeros(2, E, dtype=torch.uint8, pin_memory=True)
+            w.event = torch.cuda.Event()
+        if w.pending:                             # the end flags of the previous call, copied back asynchronously
+            w.event.synchronize()
+            e = w.ends.numpy()
+            w.end((e[0] | e[1]) != 0)
+            w.pending = False
+        n_rows = w.rows()
+
+        def dev_flags(x):
+            x = torch.as_tensor(x, device=dev).reshape(E)
+            return (x if x.dtype == torch.bool else x != 0).contiguous().view(torch.uint8)
+        on_dev = (torch.is_tensor(terminated) and terminated.is_cuda) or (torch.is_tensor(truncated) and truncated.is_cuda)
+        term = dev_flags(terminated)
+        trunc = dev_flags(truncated) if truncated is not None else None
+        args = [torch.as_tensor(obs, dtype=torch.float32).to(dev).contiguous(),
+                torch.as_tensor(action, dtype=torch.float32).to(dev).contiguous(),
+                torch.as_tensor(reward, dtype=torch.float64).to(dev).contiguous(),
+                torch.as_tensor(obs_next, dtype=torch.float32).to(dev).contiguous(), term, trunc]
+        _lib.check(_lib.lib().d4pg_replay_add_steps(self.handle, E, *[_lib.ptr(t) for t in args], n, gamma,
+                                                    _lib.ptr(w.window), n_rows, 1 if self.prioritized else 0,
+                                                    _lib.stream_ptr()), "d4pg_replay_add_steps")
+        w.advance()
+        if on_dev:                                # the episode ends are applied at the next call
+            w.ends[0].copy_(term, non_blocking=True)
+            if trunc is not None:
+                w.ends[1].copy_(trunc, non_blocking=True)
+            else:
+                w.ends[1].zero_()                 # host memory: no copy into it is in flight (waited for above)
+            w.event.record()
+            w.pending = True
+        else:
+            ended = np.asarray(terminated).reshape(E).astype(bool)
+            if truncated is not None:
+                ended = ended | np.asarray(truncated).reshape(E).astype(bool)
+            w.end(ended)
+        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
+        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+        return n_rows
+
+    def drop_steps(self):
+        """Discard the pending n-step windows; the next add_steps may use another E, n_steps or gamma."""
+        self._steps = None
+
     def _add_device(self, n, tensors):
         _lib.check(_lib.lib().d4pg_replay_add(self.handle, n, *[_lib.ptr(t) for t in tensors],
                                               1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add")
@@ -543,6 +655,29 @@ class ReplayBuffer(object):
     def add_her_episode(self, obs, obs_next, goal, achieved_goal_next, action, reward, done, **kw):
         """Hindsight relabelling on the device (main.py:154-184); see _DeviceReplay.add_her_episode."""
         return self._store.add_her_episode(obs, obs_next, goal, achieved_goal_next, action, reward, done, **kw)
+
+    def add_steps(self, obs, action, reward, obs_next, terminated, truncated=None, n_steps=1, gamma=0.99):
+        """One vector step of E environments, with the n-step windows kept on the device (DESIGN.md §3 "Streaming
+        n-step insert").  obs / obs_next [E, obs_dim] (obs_next: the true next or final observation, not an auto-reset
+        one), action [E, act_dim], reward [E], terminated / truncated bool [E] (truncated=None: no truncation); numpy,
+        CPU or CUDA tensors.  Returns the number of rows inserted.
+
+        Environment e appends (s, a, r) to its window; once the window holds n_steps steps of the current episode, the
+        row (s_{t-n+1}, a_{t-n+1}, R, obs_next_t, terminated_t) is inserted with R the reference's left-to-right f64
+        return (replay_memory.py:38-45, as add_episode); then terminated or truncated clears the window.  Windows that
+        never fill are dropped.  The stored action is the window's oldest, as replay_memory.py:44 stores it, not the
+        episode's last action that main.py:233 stores.  The rows of one call go in ascending e, which fixes their ring
+        positions, their leaves and the normalizer's fold; with n_steps=1 a call stores what add_batch stores (a reward
+        of -0.0 becomes +0.0, as in the reference's loop).
+
+        The first call fixes E, n_steps and gamma; a call that changes one raises ValueError until drop_steps().  CUDA
+        terminated / truncated are read back asynchronously and waited for at the next call.  The pending windows are
+        not part of any checkpoint."""
+        return self._store.add_steps(obs, action, reward, obs_next, terminated, truncated, n_steps, gamma)
+
+    def drop_steps(self):
+        """Discard the pending n-step windows of add_steps."""
+        self._store.drop_steps()
 
     def _encode_sample(self, idxes):
         return _to_host_batch(self._store.gather(idxes))

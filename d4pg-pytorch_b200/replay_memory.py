@@ -51,6 +51,19 @@ class Replay(object):
         at insert -- the arithmetic of initialize() below / replay_memory.py:38-45."""
         return self._store.add_episode_nstep(states, actions, rewards, next_states, dones, self.n_steps, self.gamma)
 
+    def add_steps(self, states, actions, rewards, next_states, terminated, truncated=None, n_steps=None, gamma=None):
+        """One vector step of E environments with the n-step windows on the device, at this Replay's n_steps / gamma
+        (ReplayBuffer.add_steps has the semantics).  n_steps / gamma, when given, must equal the Replay's.  Returns the
+        number of rows inserted."""
+        if (n_steps is not None and n_steps != self.n_steps) or (gamma is not None and float(gamma) != float(self.gamma)):
+            raise ValueError("Replay.add_steps: this Replay forms %d-step returns at gamma=%r, got n_steps=%r, gamma=%r"
+                             % (self.n_steps, self.gamma, n_steps, gamma))
+        return self._store.add_steps(states, actions, rewards, next_states, terminated, truncated, self.n_steps, self.gamma)
+
+    def drop_steps(self):
+        """Discard the pending n-step windows of add_steps."""
+        self._store.drop_steps()
+
     def initialize(self, init_length):
         """Random-policy filler with n-step return accumulation at insert time (replay_memory.py:21-59).  Needs a
         gym-style `env`.  The rollout is host glue; every finished (or cut-off) episode goes to the device in one

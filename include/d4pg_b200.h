@@ -200,6 +200,33 @@ int32_t d4pg_replay_add_nstep(d4pg_replay_t* h, int64_t T, const float* obs, con
                               const float* obs2, const uint8_t* done, int32_t n_steps, double gamma,
                               double* rew_scratch, int32_t prioritized, d4pg_stream_t stream);
 
+/* Streaming n-step insert: one vector step of E environments per call, the n-step windows kept on the device.
+ *   obs, obs2 f32 [E, obs_dim]   act f32 [E, act_dim]   rew f64 [E]   terminated u8 [E]   episode_end u8 [E] or NULL
+ * Environment e appends (obs_e, act_e, rew_e) to its window.  With f = the steps of e's current episode before this
+ * call, e emits when f + 1 >= n: the row (s_{f-n+1}, a_{f-n+1}, R, obs2_e, terminated_e != 0), with
+ *   R = sum_{k<n} gamma^k r_{f-n+1+k}, the left-to-right f64 loop of d4pg_nstep_returns, bit for bit.
+ * Then the window is cleared when terminated_e != 0 or episode_end_e != 0 (pass truncated, or terminated | truncated;
+ * NULL = terminated only).  Windows that never fill are dropped, like replay_memory.py:38 before step n-1.
+ * The emitting environments take ring rows next_idx, next_idx + 1, ... in ascending e; the leaves, the normalizer's
+ * fold and len / next_idx follow as for d4pg_replay_add of those rows in that order (n_steps = 1 stores what
+ * d4pg_replay_add of the E rows stores, except that R = 0.0 + 1.0 * r turns a reward of -0.0 into +0.0).
+ *   n_rows: the number of emitting environments, which the caller counts from the episode ends of earlier calls (a
+ *           host mirror of the fills, no device read).  The kernel writes no ring row outside [next_idx, next_idx + n_rows).
+ *   window: caller-owned device memory of d4pg_replay_steps_window_bytes(E, obs_dim, act_dim, n_steps) bytes (-1 on
+ *           bad arguments), zero-filled before the first call.  It holds the per-environment state: a u64 record
+ *           {call id, fill before, fill after} [E], rewards f64 [E, 2n] (each stored twice, so the last n are
+ *           contiguous), states f32 [E, n, obs_dim] and actions f32 [E, n, act_dim].  Zero-filling it again discards
+ *           the pending windows.  E, n_steps and gamma must stay the same between zero-fills.
+ * One kernel per call, plus the d4pg_replay_add tail when n_rows > 0 (the normalizer's fold, split at the ring's
+ * wrap; the tree add).  Stream-ordered, no allocation.  D4PG_EINVAL: null pointers, E outside (0, size], n_steps
+ * outside [1, D4PG_STEPS_MAX_N], n_rows outside [0, E]. */
+#define D4PG_STEPS_MAX_N 64
+int64_t d4pg_replay_steps_window_bytes(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps);
+int32_t d4pg_replay_add_steps(d4pg_replay_t* h, int64_t E, const float* obs, const float* act, const double* rew,
+                              const float* obs2, const uint8_t* terminated, const uint8_t* episode_end,
+                              int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t prioritized,
+                              d4pg_stream_t stream);
+
 /* Hindsight-experience relabelling on the device (main.py:154-184, "future" strategy) as a gather kernel that produces
  * the rows d4pg_replay_add then inserts.  Episode of T goal-conditioned steps: obs / obs_next f32 [T, obs_dim], goal
  * f64 [T, goal_dim] (desired goal of every step), ag_next f64 [T, goal_dim] (achieved goal of the next state), act f32
@@ -227,7 +254,7 @@ int32_t d4pg_her_relabel(int32_t T, int32_t obs_dim, int32_t goal_dim, int32_t a
  * Apply (fp32): y = min(max((x - shift) * scale, -clip), clip).  clip and eps: finite and > 0 (5.0 and 1e-8 are usual).
  *
  * d4pg_replay_set_obs_norm registers caller-owned device buffers with the replay and resets them to n = 0 on `stream`;
- * from then on every insert (add, add_host, add_nstep) updates them on its own stream, right after its ring write.
+ * from then on every insert (add, add_host, add_nstep, add_steps) updates them on its own stream, right after its ring write.
  * stats == NULL detaches.  The stored rows and every sample / gather of this section stay raw; only a learner created
  * with obs_norm = 1 reads the affine.  d4pg_replay_obs_norm_refresh recomputes the affine from the stats after the
  * caller wrote them (a state load).  Both bump the replay's generation, so a learner's prefetched batch is re-sampled.
