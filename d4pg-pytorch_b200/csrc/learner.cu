@@ -57,15 +57,42 @@ struct Workspace {
 //   PLAN_CHAIN     cluster-fused chains of mlp_chain.cu: exact FFMA tiles at fp32, mma.sync 3xTF32 / TF32 tiles otherwise;
 //   PLAN_TC_CHAIN  cluster-fused wgmma chains of mlp_tc_chain.cu, with pre-packed hi/lo weight images.
 // The chain plans pay off while the batch fits one wave of clusters (a 64-row cluster chain is a latency design; 128-row
-// level tiles suit larger batches), so batches above CHAIN_MAX_BATCH rows always run the level plan.
+// level tiles suit larger batches), so batches above CHAIN_MAX_BATCH rows always run the level plan.  PLAN_CHAIN also
+// needs every slot of its forward and dX launches to fit one chain CTA (chain_plan_fits): a wide observation or action
+// runs the level plan.
 enum StepPlan { PLAN_LEVELS, PLAN_CHAIN, PLAN_TC_CHAIN };
 constexpr int CHAIN_MAX_BATCH = 512;
+// pre-layers (a narrow layer computed inside the slot that consumes it): fp32 tile, |a| <= 8
+static bool chain_pre_ok(const d4pg_learner_config_t& c) { return c.precision == 0 && c.act_dim <= 8; }
+// chain_fits (mlp_chain.cu) of the PLAN_CHAIN launches, on slots of the shapes chain_build_actor_critic, forward_chain
+// and backward_chain add: fc1 is |s| deep, critic fc2 H + |a|, actor fc3 and the d-action layer |a| wide, critic fc3
+// as wide as the head.  Sizes only: no launch is built from these slots.
+static bool chain_plan_fits(const d4pg_learner_config_t& c) {
+  const int H = D4PG_HIDDEN, S = c.obs_dim, A = c.act_dim, N = c.n_atoms;
+  ChainArgs f, b;
+  chain_args_begin(f, c.batch, nullptr, c.precision);
+  chain_add(f, 0, chain_fwd(nullptr, 0, nullptr, H, S, EPI_BIAS_RELU, nullptr, 0, 1));             // fc1
+  chain_add(f, 0, chain_fwd(nullptr, 0, nullptr, H, H, EPI_BIAS_RELU, nullptr, 0, 1));             // actor fc2, fc2_2
+  ChainSlot fc2 = chain_fwd(nullptr, 0, nullptr, H, H + A, EPI_BIAS_RELU, nullptr, 0, 1);           // critic fc2
+  if (chain_pre_ok(c)) chain_pre_layer(fc2, nullptr, 0, nullptr, nullptr, 0, A, H, EPI_BIAS_TANH, nullptr, 0, 0, H, false);
+  else chain_add(f, 0, chain_fwd(nullptr, 0, nullptr, A, H, EPI_BIAS_TANH, nullptr, 0, 1));       // actor fc3
+  chain_add(f, 0, fc2);
+  chain_add(f, 0, chain_fwd(nullptr, 0, nullptr, N, H, EPI_BIAS, nullptr, 0, 0));                  // critic fc3
+  chain_args_begin(b, c.batch, nullptr, c.precision);
+  chain_add(b, 0, chain_dx(nullptr, 0, H, N, EPI_RELU_MASK, nullptr, 0, nullptr, 0, 1));           // critic fc3
+  chain_add(b, 0, chain_dx(nullptr, 0, H, H, EPI_RELU_MASK, nullptr, 0, nullptr, 0, 1));           // the H x H layers
+  ChainSlot fc3 = chain_dx(nullptr, 0, H, A, EPI_RELU_MASK, nullptr, 0, nullptr, 0, 1);             // actor fc3
+  if (chain_pre_ok(c)) chain_pre_layer(fc3, nullptr, 0, nullptr, nullptr, 0, A, H, EPI_TANH_MASK, nullptr, 0, 0, H, true);
+  else chain_add(b, 0, chain_dx(nullptr, 0, A, H, EPI_TANH_MASK, nullptr, 0, nullptr, 0, 1));      // d action
+  chain_add(b, 0, fc3);
+  return chain_fits(f) && chain_fits(b);
+}
 static StepPlan step_plan(const d4pg_learner_config_t& c) {
   if (c.batch > CHAIN_MAX_BATCH || c.chain != 1) return PLAN_LEVELS;
   if (c.precision == 3) return PLAN_LEVELS;             // bf16: the level kernel only (no bf16 chain tiles)
   // the wgmma chains need |s| <= 32 (one resident input chunk), |a| <= 32 (one K-tail chunk) and <= 256 atoms
   if (c.precision >= 1 && c.obs_dim <= 32 && c.act_dim <= 32 && c.n_atoms <= 256) return PLAN_TC_CHAIN;
-  return PLAN_CHAIN;
+  return chain_plan_fits(c) ? PLAN_CHAIN : PLAN_LEVELS;
 }
 // The mixture-of-Gaussians critic (dist_type 1) has a raw head of 3K columns: it takes the place of n_atoms wherever a
 // plane or a layer is sized (carve, critic_dims, step_plan, tcc_setup), so the learner keeps the config with n_atoms = 3K
@@ -418,8 +445,6 @@ static ChainSlot chain_layer(const Step& x, Net net, int l, float* C, int ldc, i
   const Layer y = layer(x.L, net, l);
   return chain_fwd(y.W, y.ldw, y.bias, y.n_out, y.k_in, y.epi, C, ldc, publish);
 }
-// pre-layers (a narrow layer computed inside the slot that consumes it): fp32 tile, |a| <= 8
-static bool chain_pre_ok(const Step& x) { return x.c.precision == 0 && x.A <= 8; }
 // actor `an` on `s`, then critic `cn` on (s, that action), as chain `ci`: T (the targets on s') and P (the online nets on
 // s).  ka / kc: the activation sets they write; c_h1: where the critic's h1 goes (nullptr: exchange only)
 static void chain_build_actor_critic(const Step& x, ChainArgs& ca, int ci, Net an, Net cn, const float* s, int ka,
@@ -432,10 +457,10 @@ static void chain_build_actor_critic(const Step& x, ChainArgs& ca, int ci, Net a
   sl = chain_layer(x, an, 2, w.h3[ka], H, 1); chain_src_plane(sl, t); const int a22 = chain_add(ca, ci, sl);
   // the 6-wide actor fc3 is a PRE-LAYER of the critic's fc2 slot (every CTA computes it for its 32 rows) instead of
   // a slot of its own, when it fits; otherwise it is a slot that publishes 8 plane rows
-  if (!chain_pre_ok(x)) { sl = chain_layer(x, an, 3, w.out[ka], x.Ap, 1); chain_src_plane(sl, a22); a3 = chain_add(ca, ci, sl); }
+  if (!chain_pre_ok(x.c)) { sl = chain_layer(x, an, 3, w.out[ka], x.Ap, 1); chain_src_plane(sl, a22); a3 = chain_add(ca, ci, sl); }
   sl = chain_layer(x, cn, 0, c_h1, H, 1); chain_src_global(sl, s, x.Sp); t = chain_add(ca, ci, sl);
   sl = chain_layer(x, cn, 1, w.h2[kc], H, 1); chain_src_plane(sl, t);
-  if (chain_pre_ok(x)) {
+  if (chain_pre_ok(x.c)) {
     const Layer y = layer(x.L, an, 3);
     chain_pre_layer(sl, y.W, y.ldw, y.bias, nullptr, 0, y.n_out, y.k_in, y.epi, w.out[ka], x.Ap, a22, H, false);
   } else chain_src2_plane(sl, H, a3);
@@ -657,7 +682,7 @@ static int backward_chain(Step& x) {
   sl = chain_layer_dx(layer_dx(L, CRITIC, 3), EPI_RELU_MASK, w.h3[4], H, w.p_dz22, H, 1); chain_src_global(sl, w.dlogits_pi, Np); t = chain_add(cb, 1, sl);
   sl = chain_layer_dx(layer_dx(L, CRITIC, 2), EPI_RELU_MASK, w.h2[4], H, w.p_dz2, H, 1); chain_src_plane(sl, t); t = chain_add(cb, 1, sl);
   const LayerDx da = critic_fc2_action_dx(L);
-  if (chain_pre_ok(x)) {      // d action (6 wide) as a pre-layer of the step through actor fc3
+  if (chain_pre_ok(x.c)) {      // d action (6 wide) as a pre-layer of the step through actor fc3
     sl = chain_layer_dx(layer_dx(L, ACTOR, 3), EPI_RELU_MASK, w.h3[3], H, w.a_dz22, H, 1);
     chain_pre_layer(sl, da.W, da.ldw, nullptr, w.out[3], Ap, da.n_in, da.k_out, EPI_TANH_MASK, w.a_dz3, Ap, t, H, true);
     t = chain_add(cb, 1, sl);

@@ -253,6 +253,13 @@ int chain_add(ChainArgs& a, int c, const ChainSlot& s) {
   if (wf > a.w_floats) a.w_floats = wf;
   return l;
 }
+size_t chain_smem_bytes(const ChainArgs& a) { return size_t(a.a_floats + 2 * a.w_floats) * sizeof(float); }
+bool chain_fits(const ChainArgs& a) {
+  for (int c = 0; c < a.nchains; ++c)
+    for (int l = 0; l < a.nslots[c]; ++l)
+      if (a.slot[c][l].N > CHAIN_CLUSTER * BN) return false;
+  return chain_smem_bytes(a) <= CHAIN_SMEM_MAX;
+}
 ChainSlot chain_fwd(const float* W, int ldw, const float* bias, int N, int K, int epi, float* C, int ldc, int publish) {
   ChainSlot s{};
   s.W = W; s.ldw = ldw; s.bias = bias; s.N = N; s.K = K; s.K1 = K; s.epi = epi; s.C = C; s.ldc = ldc;
@@ -284,7 +291,7 @@ int launch_mlp_chain(ChainArgs& a, cudaStream_t st) {
     D4PG_REQUIRE(a.nslots[c] > 0 && a.nslots[c] <= CHAIN_MAX_SLOTS, D4PG_EINVAL, "launch_mlp_chain: chain %d has %d slots", c, a.nslots[c]);
     for (int l = 0; l < a.nslots[c]; ++l) {
       const ChainSlot& s = a.slot[c][l];
-      D4PG_REQUIRE(s.N > 0 && s.N <= CHAIN_CLUSTER * BN, D4PG_ENOTSUP, "launch_mlp_chain: layer width %d > %d", s.N, CHAIN_CLUSTER * BN);
+      D4PG_REQUIRE(s.N > 0, D4PG_EINVAL, "launch_mlp_chain: slot %d has no columns", l);
       D4PG_REQUIRE(s.ldw % 4 == 0 && (reinterpret_cast<uintptr_t>(s.W) & 15) == 0, D4PG_EINVAL, "launch_mlp_chain: weights must be 16-B pitched");
       D4PG_REQUIRE(s.src < l && s.src2 < l, D4PG_EINVAL, "launch_mlp_chain: slot %d reads a later plane", l);
       D4PG_REQUIRE(s.src >= 0 || s.src == -2 || (s.Ag && s.ldag % 4 == 0 && s.ldag >= s.K1), D4PG_EINVAL, "launch_mlp_chain: bad global A source");
@@ -300,10 +307,11 @@ int launch_mlp_chain(ChainArgs& a, cudaStream_t st) {
       D4PG_REQUIRE(s.K == s.K1 || s.src2 < 0 || (a.slot[c][s.src2].publish && a.slot[c][s.src2].N >= s.K - s.K1), D4PG_EINVAL, "launch_mlp_chain: slot %d reads an unpublished plane", l);
     }
   }
-  const size_t smem = size_t(a.a_floats + 2 * a.w_floats) * sizeof(float);
+  const size_t smem = chain_smem_bytes(a);
   // NOT padded to force one CTA per SM: 16 clusters of 8 at one CTA per SM need two free 8-SM groups in every
   // GPC; a single foreign CTA (the concurrent tree update) pushes clusters into a second wave.
-  D4PG_REQUIRE(smem <= 220 * 1024, D4PG_ENOTSUP, "launch_mlp_chain: %zu B of shared memory needed", smem);
+  D4PG_REQUIRE(chain_fits(a), D4PG_ENOTSUP, "launch_mlp_chain: %zu B of shared memory needed (at most %zu) or a layer wider than %d",
+               smem, CHAIN_SMEM_MAX, CHAIN_CLUSTER * BN);
   D4PG_REQUIRE(a.precision >= 0 && a.precision <= 2, D4PG_EINVAL, "launch_mlp_chain: precision %d", a.precision);
   static size_t smem_set[3] = {0, 0, 0};
   void (*kern)(ChainArgs) = a.precision == 0 ? mlp_chain_kernel<0> : a.precision == 1 ? mlp_chain_kernel<1> : mlp_chain_kernel<2>;

@@ -61,6 +61,13 @@ void chain_src2_global(ChainSlot& s, int K1, const float* A2g, int lda2g);
 void chain_src2_plane(ChainSlot& s, int K1, int slot);
 void chain_pre_layer(ChainSlot& s, const float* W, int ldw, const float* bias, const float* aux, int ldaux, int N, int K, int epi,
                      float* C, int ldc, int src_slot, int pre_row, bool whole_operand);
+// One CTA holds the largest A plane and two of the largest weight slices of the slots chain_add was given, in at most
+// CHAIN_SMEM_MAX bytes, and each of a layer's CHAIN_CLUSTER ranks owns one BN-column slice of it.  chain_fits is what
+// launch_mlp_chain requires of a launch; a caller that may have a layer too wide or too deep asks it before choosing
+// the chain (learner.cu step_plan).
+constexpr size_t CHAIN_SMEM_MAX = 220 * 1024;
+size_t chain_smem_bytes(const ChainArgs& a);
+bool chain_fits(const ChainArgs& a);
 int launch_mlp_chain(ChainArgs& a, cudaStream_t st);
 
 // dW level of the whole step in one launch (up to 12 problems, no TMA descriptors in the parameters)

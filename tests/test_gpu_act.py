@@ -11,7 +11,9 @@ from tests import act_oracle as AO
 pytestmark = pytest.mark.gpu
 
 INFO = {"type": "categorical", "v_min": -50.0, "v_max": 0.0, "n_atoms": 51}
-DIMS = [(1, 1), (3, 1), (17, 6), (17, 9), (376, 17)]
+# (17, 33) / (17, 256): actor fc3 has output tiles on 2 / all 8 cluster ranks; (545, 6): chain_wpitch steps to the next
+# 32 floats; (576, 17): the largest fc1 slot that fits the chain's shared memory
+DIMS = [(1, 1), (3, 1), (17, 6), (17, 9), (376, 17), (17, 33), (17, 256), (545, 6), (576, 17)]
 ES = (1, 31, 32, 33, 256, 4097)
 
 

@@ -1,8 +1,8 @@
 """Every layer of one learner step at the shapes where the step's kernels branch, against the teacher-forced float64
 restatement and componentwise bound of tests/step_check.py.
 
-The edges: the step plan (csrc/learner.cu step_plan) switches at batch 512 / 513, |s| or |a| 32 / 33 and precision; the
-fp32 cluster chain folds the actor's fc3 into the next slot for |a| <= 8; the level plan's dW runs split-K from batch
+The edges: the step plan (csrc/learner.cu step_plan) switches at batch 512 / 513, |s| or |a| 32 / 33, precision, and
+where the cluster chain no longer fits one CTA (|s| 576 / 577, |a| 256 / 257); the fp32 cluster chain folds the actor's fc3 into the next slot for |a| <= 8; the level plan's dW runs split-K from batch
 1024 (csrc/gemm_ffma.cu prepare_problem: 1025 rows give three slices, the last of 257 rows; 3585 rows eight slices, the
 last of ONE row); chain clusters own 64 rows and level tiles 128, so 65 and 513 rows leave a 1-row cluster / tile.
 """
@@ -168,6 +168,17 @@ CASES = [
     ("chain", "fp32", 65, 17, 8, _cat(51), {}),                         # |a| = 8: actor fc3 as a pre-layer
     ("chain", "fp32", 65, 17, 9, _cat(51), {}),                         # |a| = 9: actor fc3 as a slot of its own
     ("chain", "fp32", 512, 376, 17, _cat(128), {}),                     # batch limit, config 3 widths, max atoms
+    # the chain's shared-memory and width limits (csrc/mlp_chain.cu chain_fits): fc1 holds all |s| columns, 222,208 B
+    # at |s| = 576; a layer is at most 256 wide
+    ("chain", "fp32", 512, 576, 6, _cat(51), {}),                       # the largest fc1 slot, pre-layer fc3
+    ("chain", "tf32x3", 256, 576, 17, _cat(101), {}),
+    ("chain", "fp32", 128, 17, 256, _cat(51), {}),                      # |a| = 256: actor fc3 on all 8 cluster ranks
+    # one past them: the level plan
+    ("levels", "fp32", 256, 577, 6, _cat(51), {}),                      # 230,528 B
+    ("levels", "tf32x3", 256, 577, 17, _cat(51), {}),
+    ("levels", "fp32", 64, 17, 257, _cat(51), {}),                      # actor fc3 257 wide
+    ("levels", "tf32x3", 512, 700, 6, _qr(51), {}),                     # quantile head
+    ("levels", "fp32", 1025, 2053, 6, _cat(51), {}),                    # split-K dW with fc1 K = 2053, not a multiple of 4
 ]
 for _p in ("fp32", "tf32x3"):
     CASES += [
