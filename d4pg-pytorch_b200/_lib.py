@@ -51,6 +51,7 @@ class LearnerConfig(C.Structure):
         ("max_grad_norm_actor", C.c_double), ("max_grad_norm_critic", C.c_double),
         ("weight_decay_actor", C.c_double), ("weight_decay_critic", C.c_double),
         ("obs_norm", C.c_int32),
+        ("nstep_tails", C.c_int32),
     ]
 
 
@@ -102,6 +103,10 @@ _PROTOS = {
     "d4pg_replay_steps_window_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "d4pg_replay_add_steps": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int64,
                                           C.c_int32, _P]),
+    "d4pg_replay_set_horizons": (C.c_int32, [_P, _P, _P]),
+    "d4pg_replay_steps_window_bytes_ex": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "d4pg_replay_add_steps_ex": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int64,
+                                             C.c_int32, C.c_int32, _P]),
     "d4pg_her_relabel": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                      C.c_double, C.c_int32, _P, _P, _P, _P, _P, _P]),
     "d4pg_replay_set_len": (C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int32, _P]),

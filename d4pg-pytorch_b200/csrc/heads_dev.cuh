@@ -118,6 +118,7 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
     }
   } else {
     // per-atom bins and weights in fp64 (ddpg.py:155-158 / ddpg.py:129-134)
+    const double disc = MODE == 0 ? a.h.discount : head_discount(a.h, row);
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
       int j = lane + 32 * t;
@@ -125,7 +126,7 @@ __device__ __forceinline__ void heads_row(const HeadsArgs& a, int row, int lane,
         double zj = __dadd_rn(a.v_min, __dmul_rn(double(j), a.delta));
         double c;
         if (MODE == 0) c = __dmul_rn(zj, a.h.discount);                        // (v_min+j*delta)*gamma
-        else c = __dmul_rn(__dmul_rn(a.h.discount, done ? 0.0 : 1.0), zj);      // gamma^n*(1-d)*z_j
+        else c = __dmul_rn(__dmul_rn(disc, done ? 0.0 : 1.0), zj);              // gamma^n*(1-d)*z_j (gamma^k: tail row)
         double tz = fmin(a.v_max, fmax(a.v_min, __dadd_rn(r, c)));
         double b = __ddiv_rn(__dsub_rn(tz, a.v_min), a.delta);
         double lf = floor(b), uf = ceil(b);

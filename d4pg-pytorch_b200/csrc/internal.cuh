@@ -22,7 +22,16 @@ struct HeadCommon {
   unsigned long long* trace;
   int only_policy;               // 1: only the policy head (pi_rows, dpi) -- the second loss launch of the post-update-critic plan
   LearnerClock* sampler_clock;   // prefetch pipeline: thread 0 advances the sampler's counters (after sample(k), before sample(k+1))
+  // episode tails (DESIGN.md §3 "Episode tails"): the batch's per-row horizon k (0 = `discount`) and gtab[k] = gamma^k;
+  // both null without them.  Read from the batch, never from the ring, which a later add may already overwrite
+  const uint8_t* horizon; const double* gtab;
 };
+
+// bootstrap discount of batch row `row` that is not done: gamma^k of its horizon, `discount` for a full row
+__device__ __forceinline__ double head_discount(const HeadCommon& h, int row) {
+  const int k = h.horizon ? int(h.horizon[row]) : 0;
+  return k ? h.gtab[k] : h.discount;
+}
 
 // categorical head (proj_loss.cu): N atoms on [v_min, v_max]
 struct HeadsArgs {
@@ -58,7 +67,7 @@ constexpr int SAMPLE_ROWS = 32;      // batch rows per CTA of the sample + gathe
 // sample for the learner: per-step scalars come from device memory (graph replay safe)
 int learner_sample(d4pg_replay* h, int B, int prioritized, const double* uniforms, const int32_t* positions,
                    uint64_t seed, LearnerClock* clock, const ClockParams& cp,
-                   int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d,
+                   int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d, uint8_t* hz,
                    int ld_obs, int ld_act, const float* norm, float norm_clip, int pipe_slot, cudaStream_t st,
                    bool dependent = false, unsigned long long* done_epoch = nullptr);
 // gate != nullptr: *gate is bumped (release) once the trees are complete -- by the update kernel itself when it can
@@ -66,6 +75,8 @@ int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* p
 int64_t replay_generation(const d4pg_replay* h);
 // the replay's observation normalizer: its affine (nullptr when none is registered) and clip
 const float* replay_obs_norm(const d4pg_replay* h, double* clip);
+// the replay's per-row horizon column (d4pg_replay_set_horizons; nullptr when none is registered)
+const uint8_t* replay_horizons(const d4pg_replay* h);
 // ingest gate (host pipeline): every gated learner step bumps the buffer's flag once (launch_gate_signal) and arms the
 // gate after its launch; the next add / presample on the ingest stream first waits for flag >= number of armed steps
 unsigned long long* replay_gate_flag(d4pg_replay* h);

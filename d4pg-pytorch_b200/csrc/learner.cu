@@ -33,7 +33,7 @@
 namespace d4pg {
 
 // One half of the double-buffered batch: the rows the sample kernel gathers, the indices and IS weights it draws
-struct Batch { float *s, *a, *s2; double* r; uint8_t* done; int32_t* idx; float* wts; };
+struct Batch { float *s, *a, *s2; double* r; uint8_t* done; int32_t* idx; float* wts; uint8_t* hz; };   // hz: nstep_tails only
 
 struct Workspace {
   // batch[1] exists under the prefetch / host pipelines only; without them batch[0].idx / .wts are the caller's
@@ -107,7 +107,7 @@ static_assert((CHAIN_MAX_BATCH + SAMPLE_ROWS - 1) / SAMPLE_ROWS <= TCC_THREADS, 
 
 // Every 2-D plane has a row pitch that is a multiple of 4 floats (16-B rows): |s|=17 -> 20,
 // |a|=6 -> 8, N=51 -> 52.  That makes every GEMM operand TMA- and float4-addressable.
-static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, bool prefetch, bool clip) {
+static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, bool prefetch, bool clip, bool tails) {
   Workspace w{};
   int64_t off = 0;
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += align4(n); return p; };
@@ -139,6 +139,9 @@ static Workspace carve(float* base, int B, int S, int A, int N, StepPlan plan, b
     for (int k = 0; k < 2; ++k) { w.batch[k].idx = reinterpret_cast<int32_t*>(take(B)); w.batch[k].wts = take(B); }
   }
   if (clip) w.sq_partials = reinterpret_cast<double*>(take(2 * GRAD_NORM_CTAS * 2));
+  // the batch's horizons (nstep_tails), last so that every other plane keeps its offset
+  if (tails)
+    for (int k = 0; k < (prefetch ? 2 : 1); ++k) w.batch[k].hz = reinterpret_cast<uint8_t*>(take((B + 3) / 4));
   w.total = off;
   return w;
 }
@@ -188,6 +191,7 @@ struct d4pg_learner {
   bool images_dirty;               // parameters were written outside the library since the forward weight images were last current
   // cfg.obs_norm: the replay's observation normalizer, applied to s / s2 by every sample launch of the step
   const float* norm_affine; float norm_clip;
+  double* gtab;                    // cfg.nstep_tails: gamma^k for k < D4PG_STEPS_MAX_N (device), the tail rows' discounts
   bool profiling;
   std::vector<cudaEvent_t> ev;
   std::vector<std::string> ev_name;
@@ -358,7 +362,7 @@ static int sample_batch(Step& x) {
       learner_sample(x.L->replay, x.B, c.prioritized, c.sample_mode == 0 ? x.b.uniforms : nullptr,
                      (c.sample_mode == 0 && !c.prioritized) ? x.b.positions : nullptr,
                      c.philox_seed, x.w.clock, x.L->clock_params,
-                     x.bt.idx, x.bt.wts, x.bt.s, x.bt.a, x.bt.r, x.bt.s2, x.bt.done, x.Sp, x.Ap, x.L->norm_affine,
+                     x.bt.idx, x.bt.wts, x.bt.s, x.bt.a, x.bt.r, x.bt.s2, x.bt.done, x.bt.hz, x.Sp, x.Ap, x.L->norm_affine,
                      x.L->norm_clip, x.pf ? x.par : -1, x.st));
   return D4PG_OK;
 }
@@ -542,6 +546,7 @@ static HeadCommon head_common(const Step& x, bool only_policy) {
   h.is_weights = ((c.loss_flags & 1) && c.prioritized) ? x.bt.wts : nullptr;
   h.only_policy = only_policy ? 1 : 0;
   h.sampler_clock = (x.pf && !only_policy) ? w.clock : nullptr;    // sample(t) is done, sample(t+1) not yet launched
+  h.horizon = x.bt.hz; h.gtab = x.L->gtab;                           // episode tails: this batch's horizons
   return h;
 }
 static int launch_step_heads(Step& x, bool only_policy) {
@@ -585,7 +590,7 @@ static int side_branch(Step& x) {
     const Batch& o = x.w.batch[q];
     RUN("learner_sample", false,
         learner_sample(L->replay, x.B, c.prioritized, nullptr, nullptr, c.philox_seed, x.w.clock, L->clock_params,
-                       o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, x.Sp, x.Ap, L->norm_affine, L->norm_clip, q, L->side));
+                       o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, o.hz, x.Sp, x.Ap, L->norm_affine, L->norm_clip, q, L->side));
   }
   if (x.pf) {                           // the caller-visible copies of this step's indices / IS weights (off the
     // path to the next batch: after the write-back and the prefetch)
@@ -910,7 +915,8 @@ static int enqueue_step(d4pg_learner* L, cudaStream_t st, int par, bool cold, bo
 extern "C" int64_t d4pg_learner_workspace_floats(const d4pg_learner_config_t* cfg) {
   if (!cfg) return -1;
   const d4pg_learner_config_t ec = with_head_width(*cfg);
-  return carve(nullptr, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, step_plan(ec), piped(ec), clipping(ec)).total;
+  return carve(nullptr, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, step_plan(ec), piped(ec), clipping(ec),
+               ec.nstep_tails != 0).total;
 }
 
 extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d4pg_learner_buffers_t* buf,
@@ -948,6 +954,12 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   const float* norm_affine = cfg->obs_norm ? replay_obs_norm(replay, &norm_clip) : nullptr;
   D4PG_REQUIRE(!cfg->obs_norm || norm_affine, D4PG_EINVAL,
                "d4pg_learner_create: obs_norm needs a replay with an observation normalizer (d4pg_replay_set_obs_norm)");
+  D4PG_REQUIRE(cfg->nstep_tails == 0 || cfg->nstep_tails == 1, D4PG_EINVAL, "d4pg_learner_create: nstep_tails must be 0 or 1");
+  D4PG_REQUIRE(!cfg->nstep_tails || cfg->proj_mode == 1 || cfg->n_steps <= 1, D4PG_EINVAL,
+               "d4pg_learner_create: nstep_tails with proj_mode 0 (gamma for every row) and n_steps > 1: a per-row horizon "
+               "has no meaning there");
+  D4PG_REQUIRE(!cfg->nstep_tails || replay_horizons(replay), D4PG_EINVAL,
+               "d4pg_learner_create: nstep_tails needs a replay with a horizon column (d4pg_replay_set_horizons)");
   D4PG_REQUIRE(cfg->world_size <= 1 || comm, D4PG_EINVAL, "d4pg_learner_create: world_size>1 needs a communicator");
   D4PG_REQUIRE(cfg->chain == 0 || cfg->chain == 1, D4PG_EINVAL, "d4pg_learner_create: chain must be 0 or 1");
   for (double mn : {cfg->max_grad_norm_actor, cfg->max_grad_norm_critic})
@@ -971,7 +983,8 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
     set_error("d4pg_learner_create: grad_critic must equal grad_actor + P_a (one flat gradient buffer)");
     delete L; return D4PG_EINVAL;
   }
-  L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec), clipping(ec));
+  L->ws = carve(buf->workspace, ec.batch, ec.obs_dim, ec.act_dim, ec.n_atoms, L->plan, piped(ec), clipping(ec),
+                ec.nstep_tails != 0);
   if (!piped(ec)) { L->ws.batch[0].idx = buf->idx; L->ws.batch[0].wts = buf->weights; }   // sampled straight into the caller's buffers
   L->clock_params = ClockParams{ec.lr_actor, ec.lr_critic, ec.beta1, ec.beta2, ec.per_beta0, ec.per_beta_final,
                                 ec.per_beta_iters > 0 ? ec.per_beta_iters : 1};
@@ -989,6 +1002,16 @@ extern "C" int32_t d4pg_learner_create(const d4pg_learner_config_t* cfg, const d
   L->loss_steps = 0;
   L->ing = nullptr; L->ev_ing = nullptr; L->gate_flag = nullptr; L->images_dirty = true;
   L->norm_affine = norm_affine; L->norm_clip = float(norm_clip);
+  L->gtab = nullptr;
+  if (cfg->nstep_tails) {
+    // the same pow as head_common's gamma^n_steps; uploaded once, so graph capture never sees the copy
+    double g[D4PG_STEPS_MAX_N];
+    for (int k = 0; k < D4PG_STEPS_MAX_N; ++k) g[k] = pow(cfg->gamma, double(k));
+    if (cudaMalloc(reinterpret_cast<void**>(&L->gtab), sizeof(g)) != cudaSuccess ||
+        cudaMemcpy(L->gtab, g, sizeof(g), cudaMemcpyHostToDevice) != cudaSuccess) {
+      set_error("d4pg_learner_create: horizon table upload failed"); delete L; return D4PG_ECUDA;
+    }
+  }
   if (host_pipe(*cfg)) {
     L->gate_flag = replay_gate_flag(replay);
     const bool ok = L->gate_flag && cudaStreamCreateWithFlags(&L->ing, cudaStreamNonBlocking) == cudaSuccess &&
@@ -1033,6 +1056,7 @@ extern "C" int32_t d4pg_learner_destroy(d4pg_learner_t* L) {
   cudaEventDestroy(L->ev_fork); cudaEventDestroy(L->ev_join); cudaEventDestroy(L->ev_fork2); cudaEventDestroy(L->ev_join2);
   cudaStreamDestroy(L->side);
   if (L->tcc_images) cudaFree(L->tcc_images);
+  if (L->gtab) cudaFree(L->gtab);
   if (L->ing) { cudaStreamSynchronize(L->ing); cudaStreamDestroy(L->ing); }
   if (L->ev_ing) cudaEventDestroy(L->ev_ing);
   if (L->ev_in) cudaEventDestroy(L->ev_in);
@@ -1128,7 +1152,7 @@ extern "C" int32_t d4pg_learner_step(d4pg_learner_t* L, d4pg_stream_t stream) {
 static int presample(d4pg_learner* L, int par, const double* uniforms, const int32_t* positions, cudaStream_t st) {
   const d4pg_learner_config_t& c = L->cfg; const Workspace& w = L->ws; const Batch& o = w.batch[par];
   return learner_sample(L->replay, c.batch, c.prioritized, uniforms, !c.prioritized ? positions : nullptr, c.philox_seed,
-                        w.clock, L->clock_params, o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, pitch4(c.obs_dim),
+                        w.clock, L->clock_params, o.idx, o.wts, o.s, o.a, o.r, o.s2, o.done, o.hz, pitch4(c.obs_dim),
                         pitch4(c.act_dim), L->norm_affine, L->norm_clip, par, st, /*dependent=*/true, w.pipe_epoch);
 }
 
@@ -1326,6 +1350,7 @@ extern "C" int32_t d4pg_learner_tensor(d4pg_learner_t* L, const char* name, void
   struct E { const char* n; void* p; int64_t c; int ld; };
   const E table[] = {
       {"s", bt.s, B * Sp, Sp}, {"a", bt.a, B * Ap, Ap}, {"r", bt.r, B, 1}, {"s2", bt.s2, B * Sp, Sp}, {"done", bt.done, B, 1},
+      {"h", bt.hz, bt.hz ? B : 0, 1},
       {"target_logits", w.out[1], B * Np, Np}, {"q_logits", w.out[2], B * Np, Np}, {"pi_logits", w.out[4], B * Np, Np},
       {"m", w.m, B * Np, Np}, {"q_probs", w.q_probs, B * Np, Np}, {"target_probs", w.target_probs, B * Np, Np},
       {"dlogits_q", w.dlogits_q, B * Np, Np}, {"dlogits_pi", w.dlogits_pi, B * Np, Np},
@@ -1341,7 +1366,7 @@ extern "C" int32_t d4pg_learner_tensor(d4pg_learner_t* L, const char* name, void
       {"a_dz3", w.a_dz3, B * Ap, Ap}, {"a_dz22", w.a_dz22, B * 256, 256}, {"a_dh2", w.a_dh2, B * 256, 256},
       {"a_dz1", w.a_dz1, B * 256, 256}};
   for (const E& e : table)
-    if (strcmp(e.n, name) == 0) { *ptr = e.p; *count = e.c; *ld = e.ld; return D4PG_OK; }
+    if (e.p && strcmp(e.n, name) == 0) { *ptr = e.p; *count = e.c; *ld = e.ld; return D4PG_OK; }
   set_error("d4pg_learner_tensor: unknown tensor '%s'", name);
   return D4PG_EINVAL;
 }

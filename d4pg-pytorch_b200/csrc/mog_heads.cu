@@ -62,7 +62,7 @@ __device__ __forceinline__ MogComp mog_comp(const float* __restrict__ raw, int K
 // Lane j holds online component j; the 8K quadrature points are spread over the lanes (point p = 8k + q on lane p % 32,
 // NT = ceil(8K / 32) per lane), so the per-point logsumexp over the components runs in registers and only the K
 // per-component gradient sums need warp reductions.
-template <int NT>
+template <int NT, bool HZ>
 __device__ __forceinline__ void mog_critic_row(const MogArgs& a, int row, int lane) {
   const int K = a.K;
   const size_t ro = size_t(row) * a.h.ld;
@@ -70,7 +70,7 @@ __device__ __forceinline__ void mog_critic_row(const MogArgs& a, int row, int la
   const MogComp t = mog_comp(a.h.target + ro, K, lane);
   const MogComp q = mog_comp(a.h.q + ro, K, lane);
   const double r = a.h.rewards[row];
-  const double c = a.h.dones[row] ? 0.0 : a.h.discount;
+  const double c = a.h.dones[row] ? 0.0 : (HZ ? head_discount(a.h, row) : a.h.discount);
   const float isw = a.h.is_weights ? __ldg(a.h.is_weights + row) : 1.f;
   const double LOG_2PI = 1.8378770664093453, SQRT2 = 1.4142135623730951, INV_SQRTPI = 0.5641895835477563;
   const double inv_sig = 1.0 / q.sigma;
@@ -155,8 +155,9 @@ __device__ __forceinline__ void mog_policy_row(const MogArgs& a, int row, int la
 // warps [0, B): critic part of row g; [B, 2B): policy part of row g - B (only_policy: warps [0, B) run the policy part).
 // Also does what heads_kernel does for the step besides the maths: PDL wait / trigger, the step stamps and the
 // sampler-clock advance of the prefetch / host pipelines.
-// __maxnreg__(255): without it ptxas aims at 64-96 registers and spills the per-point arrays (blocks are 128 threads)
-template <int NT>
+// __maxnreg__(255): without it ptxas aims at 64-96 registers and spills the per-point arrays (blocks are 128 threads).
+// HZ: the batch carries per-row horizons (episode tails); a separate instantiation, so the plain one keeps its registers
+template <int NT, bool HZ>
 __global__ void __maxnreg__(255) mog_heads_kernel(const MogArgs a) {
   pdl_trigger(a.h.pdl);
   pdl_wait();
@@ -164,7 +165,7 @@ __global__ void __maxnreg__(255) mog_heads_kernel(const MogArgs a) {
   const int g = blockIdx.x * MOG_WARPS + warp;
   step_stamp(a.h.trace, 2);
   if (a.h.only_policy) { if (g < a.h.B) mog_policy_row(a, g, lane); }
-  else if (g < a.h.B) mog_critic_row<NT>(a, g, lane);
+  else if (g < a.h.B) mog_critic_row<NT, HZ>(a, g, lane);
   else if (g < 2 * a.h.B) mog_policy_row(a, g - a.h.B, lane);
   step_stamp(a.h.trace, 2 + 16);
   if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
@@ -173,19 +174,25 @@ __global__ void __maxnreg__(255) mog_heads_kernel(const MogArgs a) {
   pdl_trigger_end(a.h.pdl);
 }
 
+template <bool HZ>
+static int launch_mog_heads_nt(const MogArgs& a, dim3 grid, dim3 block, cudaStream_t st) {
+  D4PG_MAX_CARVEOUT((mog_heads_kernel<1, HZ>)); D4PG_MAX_CARVEOUT((mog_heads_kernel<2, HZ>));
+  D4PG_MAX_CARVEOUT((mog_heads_kernel<4, HZ>)); D4PG_MAX_CARVEOUT((mog_heads_kernel<8, HZ>));
+  // NT = quadrature points per lane: 8K points over 32 lanes
+  if (a.K <= 4) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<1, HZ>, grid, block, 0, st, a));
+  else if (a.K <= 8) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<2, HZ>, grid, block, 0, st, a));
+  else if (a.K <= 16) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<4, HZ>, grid, block, 0, st, a));
+  else D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<8, HZ>, grid, block, 0, st, a));
+  return D4PG_OK;
+}
+
 int launch_mog_heads(const MogArgs& a_in, cudaStream_t st) {
   MogArgs a = a_in;
   a.h.pdl = pdl_mode();
   a.h.trace = (a.h.sampler_clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
   dim3 grid(cdiv(((a.h.pi && !a.h.only_policy) ? 2 : 1) * a.h.B, MOG_WARPS)), block(MOG_WARPS * 32);
-  D4PG_MAX_CARVEOUT(mog_heads_kernel<1>); D4PG_MAX_CARVEOUT(mog_heads_kernel<2>);
-  D4PG_MAX_CARVEOUT(mog_heads_kernel<4>); D4PG_MAX_CARVEOUT(mog_heads_kernel<8>);
-  // NT = quadrature points per lane: 8K points over 32 lanes
-  if (a.K <= 4) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<1>, grid, block, 0, st, a));
-  else if (a.K <= 8) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<2>, grid, block, 0, st, a));
-  else if (a.K <= 16) D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<4>, grid, block, 0, st, a));
-  else D4PG_CUDA_OK(launch_pdl(mog_heads_kernel<8>, grid, block, 0, st, a));
-  return D4PG_OK;
+  if (a.h.horizon) return launch_mog_heads_nt<true>(a, grid, block, st);
+  return launch_mog_heads_nt<false>(a, grid, block, st);
 }
 
 // raw head [B, ldr] -> w, mu, sigma [B, K] (dense), one warp per row

@@ -31,7 +31,7 @@ __device__ __forceinline__ void qr_critic_row(const QrArgs& a, int row, int lane
   const int N = a.N;
   const size_t ro = size_t(row) * a.h.ld;
   const double r = a.h.rewards[row];
-  const double c = a.h.dones[row] ? 0.0 : a.h.discount;
+  const double c = a.h.dones[row] ? 0.0 : head_discount(a.h, row);
   const float isw = a.h.is_weights ? __ldg(a.h.is_weights + row) : 1.f;
   const double kap = a.kappa;
   double th[NT], tau[NT], g[NT], ls[NT];

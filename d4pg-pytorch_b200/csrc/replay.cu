@@ -37,6 +37,8 @@ struct d4pg_replay {
   cudaEvent_t order_ev;
   // observation normalizer (d4pg_replay_set_obs_norm): caller-owned stats / affine, updated by every insert
   double* norm_stats; float* norm_affine; double norm_clip, norm_eps;
+  // per-row horizon column (d4pg_replay_set_horizons): k of an episode-tail row, 0 for every other row
+  uint8_t* horizon;
 };
 
 namespace d4pg {
@@ -44,15 +46,16 @@ namespace d4pg {
 static unsigned long long* step_trace() { unsigned long long* p = debug_trace_buffer(); return p ? p + STEP_TRACE_BASE : nullptr; }
 
 
-// NORM: the learner's batch goes through the observation normalizer as it is gathered (sample_body<true>).  The two
-// instantiations are separate non-template kernels so that the plain one compiles to what it was before the option.
-template <bool NORM>
+// NORM: the learner's batch goes through the observation normalizer as it is gathered (sample_body<true, .>); HZ: the
+// rows' horizons are gathered too (episode tails).  The instantiations are separate non-template kernels so that the
+// plain one compiles to what it was before either option.
+template <bool NORM, bool HZ>
 __device__ __forceinline__ void sample_gather_body(const SampleArgs& a) {
   __shared__ SampleSmem sm;
   pdl_trigger(a.pdl);
   pdl_wait();
   step_stamp(a.trace, a.trace_slot);
-  sample_body<NORM>(a, blockIdx.x, sm);
+  sample_body<NORM, HZ>(a, blockIdx.x, sm);
   if (a.done_epoch) {                          // the forward chains of the step poll these instead of a stream event
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -64,8 +67,10 @@ __device__ __forceinline__ void sample_gather_body(const SampleArgs& a) {
   step_stamp(a.trace, a.trace_slot + 16);
   pdl_trigger_end(a.pdl);
 }
-__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_kernel(const SampleArgs a) { sample_gather_body<false>(a); }
-__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_norm_kernel(const SampleArgs a) { sample_gather_body<true>(a); }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_kernel(const SampleArgs a) { sample_gather_body<false, false>(a); }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_norm_kernel(const SampleArgs a) { sample_gather_body<true, false>(a); }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_hz_kernel(const SampleArgs a) { sample_gather_body<false, true>(a); }
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_gather_norm_hz_kernel(const SampleArgs a) { sample_gather_body<true, true>(a); }
 
 template <int MODE>
 __global__ void __launch_bounds__(TREE_THREADS) tree_write_kernel(const TreeArgs a) {
@@ -297,9 +302,15 @@ int launch_sample(const d4pg_replay* h, SampleArgs& a, cudaStream_t st, bool dep
   a.pdl = pdl_mode();
   a.trace = (a.clock && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
   a.trace_slot = a.pipe_slot >= 0 && a.uniforms == nullptr && st_is_side(st) ? 4 : 0;
-  // a.norm (learner with an observation normalizer): s / s2 are normalized as they are gathered
-  void (*kernel)(const SampleArgs) = a.norm ? sample_gather_norm_kernel : sample_gather_kernel;
-  if (a.norm) D4PG_MAX_CARVEOUT(sample_gather_norm_kernel);
+  // a.norm (learner with an observation normalizer): s / s2 are normalized as they are gathered; a.hz (learner with
+  // episode tails): the rows' horizons are gathered from the ring's column
+  a.horizon = a.hz ? h->horizon : nullptr;
+  void (*kernel)(const SampleArgs) = a.hz ? (a.norm ? sample_gather_norm_hz_kernel : sample_gather_hz_kernel)
+                                          : (a.norm ? sample_gather_norm_kernel : sample_gather_kernel);
+  if (a.hz) {
+    if (a.norm) D4PG_MAX_CARVEOUT(sample_gather_norm_hz_kernel);
+    else D4PG_MAX_CARVEOUT(sample_gather_hz_kernel);
+  } else if (a.norm) D4PG_MAX_CARVEOUT(sample_gather_norm_kernel);
   else D4PG_MAX_CARVEOUT(sample_gather_kernel);
   if (dependent) {
     // programmatic dependent launch behind the previous kernel of the stream (the host pipeline's tree add): the grid is
@@ -319,11 +330,11 @@ int launch_sample(const d4pg_replay* h, SampleArgs& a, cudaStream_t st, bool dep
 
 int learner_sample(d4pg_replay* h, int B, int prioritized, const double* uniforms, const int32_t* positions,
                    uint64_t seed, LearnerClock* clock, const ClockParams& cp,
-                   int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d,
+                   int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d, uint8_t* hz,
                    int ld_obs, int ld_act, const float* norm, float norm_clip, int pipe_slot, cudaStream_t st, bool dependent,
                    unsigned long long* done_epoch) {
   SampleArgs sa{};
-  sa.done_epoch = done_epoch;
+  sa.done_epoch = done_epoch; sa.hz = hz;
   sa.norm = norm; sa.norm_clip = norm_clip;
   sa.ld_obs = ld_obs; sa.ld_act = ld_act; sa.pipe_slot = pipe_slot;
   sa.uniforms = uniforms; sa.seed = seed; sa.counter = 0; sa.clock = clock; sa.clock_params = cp;
@@ -357,6 +368,7 @@ void tree_update_args(d4pg_replay* h, int B, const int32_t* idx, const float* pr
 
 int64_t replay_generation(const d4pg_replay* h) { return h->gen; }
 const float* replay_obs_norm(const d4pg_replay* h, double* clip) { if (clip) *clip = h->norm_clip; return h->norm_affine; }
+const uint8_t* replay_horizons(const d4pg_replay* h) { return h->horizon; }
 
 int launch_gate_signal(unsigned long long* flag, cudaStream_t st);
 int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* prio, cudaStream_t st, unsigned long long* gate) {
@@ -415,6 +427,7 @@ extern "C" int32_t d4pg_replay_create(int64_t size, int32_t obs_dim, int32_t act
   for (int i = 0; i < 2; ++i) { h->stage_ev[i] = nullptr; h->stage_busy[i] = false; }
   h->gate_flag = nullptr; h->gate_target = 0; h->gate_pending = false; h->order_ev = nullptr;
   h->norm_stats = nullptr; h->norm_affine = nullptr; h->norm_clip = 0.0; h->norm_eps = 0.0;
+  h->horizon = nullptr;
   tree_init_kernel<<<2 * device_sm_count(), 256, 0, as_stream(stream)>>>(h->sum, h->mn, h->scratch,
                                                         reinterpret_cast<ReplayState*>(h->state), h->cap);
   cudaError_t e = cudaGetLastError();
@@ -495,6 +508,13 @@ __global__ void nstep_returns_kernel(const double* __restrict__ rew, int64_t T, 
 // The emit decision of e needs the fill BEFORE this call; a CTA counts the emitters below its first environment from
 // the other CTAs' records, which may or may not have been rewritten yet: a record carrying this call's id holds the
 // old fill in bits 32-39.  Every record carries the same call id between calls, because every call steps all E.
+//
+// TAILS (DESIGN.md §3 "Episode tails"): an episode that ends at a call with fill f leaves P = min(f + 1, n - 1) pending
+// tail rows, which environment e emits first thing at its next call, before it appends that call's step: start
+// u = f + 1 - P + i (i < P) gives (s_u, a_u, nstep_return over its k = P - i remaining rewards, obs_next and terminated
+// of the ending step) with horizon k.  The window also keeps that obs_next (wo f32 [E, S], after wa), and the record
+// {bits 48-53: P, 54: terminated, 55-60: (f + 1) % n}; a rewritten record holds the ROWS its call emitted in bits 32-39
+// (P, or 1 for a full row), which is what the other CTAs count.  Every row writes its horizon: k, or 0 for a full row.
 constexpr int STEPS_THREADS = 256, STEPS_WARPS = STEPS_THREADS / 32;
 struct StepsArgs {
   const float* obs; const float* act; const double* rew; const float* obs2; const uint8_t* term; const uint8_t* end;
@@ -502,12 +522,19 @@ struct StepsArgs {
   unsigned long long* rec; double* wr; float* ws; float* wa;
   float* r_obs; float* r_act; double* r_rew; float* r_obs2; uint8_t* r_done;
   int64_t size, start, n_rows, new_len, new_next; ReplayState* state;
+  float* wo; uint8_t* r_hz;          // TAILS only
 };
 
 __device__ __forceinline__ int steps_fill_before(unsigned long long rec, unsigned kprev) {
   return int(((unsigned)rec == kprev ? rec >> 40 : rec >> 32) & 0xff);
 }
+// TAILS: the rows environment `rec` emits at this call (a full row, or its pending tails)
+__device__ __forceinline__ int steps_rows(unsigned long long rec, unsigned kprev, int n) {
+  if ((unsigned)rec != kprev) return int((rec >> 32) & 0xff);
+  return int(((rec >> 40) & 0xff) >= unsigned(n - 1)) + int((rec >> 48) & 0x3f);
+}
 
+template <bool TAILS>
 __global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const StepsArgs a) {
   __shared__ int red[STEPS_WARPS];
   __shared__ int fill_s[STEPS_THREADS], rank_s[STEPS_THREADS];
@@ -518,25 +545,40 @@ __global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const S
   const unsigned kprev = (unsigned)__ldcg(a.rec + e0);
   // emitting environments in [0, e0)
   int c = 0;
-  for (int64_t e = t; e < e0; e += STEPS_THREADS) c += steps_fill_before(__ldcg(a.rec + e), kprev) >= n - 1;
+  for (int64_t e = t; e < e0; e += STEPS_THREADS)
+    c += TAILS ? steps_rows(__ldcg(a.rec + e), kprev, n) : steps_fill_before(__ldcg(a.rec + e), kprev) >= n - 1;
   c = __reduce_add_sync(0xffffffffu, c);
   if (lane == 0) red[w] = c;
   __syncthreads();
   int64_t base = 0;
   for (int i = 0; i < STEPS_WARPS; ++i) base += red[i];
   for (int64_t tile = e0; tile < e1; tile += STEPS_THREADS) {
-    // exclusive rank of this tile's emitters
+    // exclusive rank of this tile's emitters (TAILS: of their first rows, by a warp scan of the row counts)
     const int64_t e = tile + t;
-    const int fill = e < e1 ? steps_fill_before(__ldcg(a.rec + e), kprev) : 0;
-    const bool emit = e < e1 && fill >= n - 1;
-    const unsigned bal = __ballot_sync(0xffffffffu, emit);
-    __syncthreads();                                   // red[] of the previous tile / the prefix count is consumed
-    if (lane == 0) red[w] = __popc(bal);
+    int fill, within = 0;
+    unsigned bal = 0u;
+    if (TAILS) {
+      const unsigned long long rc = e < e1 ? __ldcg(a.rec + e) : 0ull;
+      fill = e < e1 ? steps_fill_before(rc, kprev) : 0;
+      const int rows = e < e1 ? steps_rows(rc, kprev, n) : 0;
+      int incl = rows;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+      __syncthreads();                                 // red[] of the previous tile / the prefix count is consumed
+      if (lane == 31) red[w] = incl;
+      within = incl - rows;
+    } else {
+      fill = e < e1 ? steps_fill_before(__ldcg(a.rec + e), kprev) : 0;
+      const bool emit = e < e1 && fill >= n - 1;
+      bal = __ballot_sync(0xffffffffu, emit);
+      __syncthreads();                                 // red[] of the previous tile / the prefix count is consumed
+      if (lane == 0) red[w] = __popc(bal);
+    }
     __syncthreads();
     int before = 0, total = 0;
     for (int i = 0; i < STEPS_WARPS; ++i) { before += i < w ? red[i] : 0; total += red[i]; }
     fill_s[t] = fill;
-    rank_s[t] = before + __popc(bal & ((1u << lane) - 1u));
+    rank_s[t] = before + (TAILS ? within : __popc(bal & ((1u << lane) - 1u)));
     __syncthreads();
     const int cnt = int(min(int64_t(STEPS_THREADS), e1 - tile));
     for (int j = w; j < cnt; j += STEPS_WARPS) {
@@ -545,6 +587,30 @@ __global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const S
       const int64_t rank = base + rank_s[j];
       const bool write = f >= n - 1 && rank < a.n_rows;       // never outside [start, start + n_rows)
       const int64_t p = (a.start + rank) % a.size;
+      int P = 0;                                              // TAILS: pending tail rows, emitted before the append
+      if (TAILS) {
+        const unsigned long long rc = __ldcg(a.rec + ee);    // not rewritten yet (lane 0 does that after a __syncwarp)
+        P = int((rc >> 48) & 0x3f);
+        const uint8_t tterm = uint8_t((rc >> 54) & 1);
+        const int endm = int((rc >> 55) & 0x3f);
+        const float* tws = a.ws + ee * n * S;
+        const float* twa = a.wa + ee * n * A;
+        const float* two = a.wo + ee * S;
+        int64_t q = p;                                        // ring slot and window slot of tail i, stepped
+        int us = (endm - P + n) % n;
+        for (int i = 0; i < P && rank + i < a.n_rows; ++i, q = q + 1 == a.size ? 0 : q + 1, us = us + 1 == n ? 0 : us + 1) {
+          const int k = P - i;
+          for (int c = lane; c < S; c += 32) { a.r_obs[q * S + c] = tws[us * S + c]; a.r_obs2[q * S + c] = two[c]; }
+          for (int c = lane; c < A; c += 32) a.r_act[q * A + c] = twa[us * A + c];
+          if (lane == 0) {
+            a.r_rew[q] = nstep_return(a.wr + ee * 2 * n + us, k, a.gamma);
+            a.r_done[q] = tterm;
+            a.r_hz[q] = uint8_t(k);
+          }
+        }
+        if (a.term[ee] != 0 || (a.end && a.end[ee] != 0))   // this step ends the episode: keep its obs_next
+          for (int c = lane; c < S; c += 32) a.wo[ee * S + c] = a.obs2[ee * S + c];
+      }
       const float* s_in = a.obs + ee * S;
       float* ws = a.ws + ee * n * S;
       for (int k = lane; k < S; k += 32) {
@@ -562,6 +628,7 @@ __global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const S
         if (n > 1) wa[slot * A + k] = v;
         if (write) a.r_act[p * A + k] = n > 1 ? wa[old * A + k] : v;
       }
+      if (TAILS) __syncwarp();                                // every lane has read the record
       if (lane == 0) {
         double* wr = a.wr + ee * 2 * n;
         if (n > 1) { const double r = a.rew[ee]; wr[slot] = r; wr[slot + n] = r; }
@@ -569,9 +636,17 @@ __global__ void __launch_bounds__(STEPS_THREADS) replay_add_steps_kernel(const S
         if (write) {
           a.r_rew[p] = nstep_return(n > 1 ? wr + old : a.rew + ee, n, a.gamma);
           a.r_done[p] = term ? 1 : 0;
+          if (TAILS) a.r_hz[p] = 0;
         }
         const int nf = ended ? 0 : (f + 1 >= 2 * n ? f + 1 - n : f + 1);
-        a.rec[ee] = (unsigned long long)(kprev + 1u) | ((unsigned long long)f << 32) | ((unsigned long long)nf << 40);
+        if (TAILS) {
+          const int pn = ended ? min(f + 1, n - 1) : 0, rows = P + (f >= n - 1 ? 1 : 0);
+          a.rec[ee] = (unsigned long long)(kprev + 1u) | ((unsigned long long)rows << 32) | ((unsigned long long)nf << 40) |
+                      ((unsigned long long)pn << 48) | ((unsigned long long)(term ? 1 : 0) << 54) |
+                      ((unsigned long long)((f + 1) % n) << 55);
+        } else {
+          a.rec[ee] = (unsigned long long)(kprev + 1u) | ((unsigned long long)f << 32) | ((unsigned long long)nf << 40);
+        }
       }
     }
     base += total;
@@ -837,16 +912,27 @@ int replay_insert_tail(d4pg_replay* h, int64_t n, int64_t start, int64_t new_len
   return D4PG_OK;
 }
 
-struct StepsLayout { int64_t rec, wr, ws, wa, total; };
-StepsLayout steps_layout(int64_t E, int64_t S, int64_t A, int64_t n) {
+struct StepsLayout { int64_t rec, wr, ws, wa, wo, total; };
+StepsLayout steps_layout(int64_t E, int64_t S, int64_t A, int64_t n, bool tails) {
   auto up = [](int64_t b) { return (b + 15) & ~int64_t(15); };
   StepsLayout l;
   l.rec = 0;
   l.wr = up(l.rec + E * 8);
   l.ws = up(l.wr + E * 2 * n * 8);
   l.wa = up(l.ws + E * n * S * 4);
-  l.total = up(l.wa + E * n * A * 4);
+  l.wo = up(l.wa + E * n * A * 4);
+  l.total = up(l.wo + (tails ? E * S * 4 : 0));
   return l;
+}
+
+// Every insert path but the episode-tails add_steps stores rows of horizon 0: clear the column over [start, start + n)
+// (mod size), on the stream of the insert's ring write, so a slot that held a tail row does not keep its horizon
+int zero_horizons(d4pg_replay* h, int64_t start, int64_t n, cudaStream_t st) {
+  if (!h->horizon || n == 0) return D4PG_OK;
+  const int64_t n1 = std::min<int64_t>(n, h->size - start);
+  D4PG_CUDA_OK(cudaMemsetAsync(h->horizon + start, 0, size_t(n1), st));
+  if (n1 < n) D4PG_CUDA_OK(cudaMemsetAsync(h->horizon, 0, size_t(n - n1), st));
+  return D4PG_OK;
 }
 }  // namespace
 
@@ -861,6 +947,7 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
   const int64_t new_len = std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n));
   const int64_t new_next = (start + n) % h->size;
   const int blocks = int(std::min<int64_t>(4 * device_sm_count(), (n * h->obs_dim + 255) / 256));   // grid-stride
+  if (int rc = zero_horizons(h, start, n, st)) return rc;
   ring_write_kernel<<<blocks, 256, 0, st>>>(h->obs, h->act, h->rew, h->obs2, h->done, obs, act, rew, obs2, done,
                                              n, h->obs_dim, h->act_dim, h->size, start,
                                              reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
@@ -869,26 +956,51 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
 }
 
 extern "C" int64_t d4pg_replay_steps_window_bytes(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps) {
-  if (E <= 0 || obs_dim <= 0 || act_dim <= 0 || n_steps < 1 || n_steps > D4PG_STEPS_MAX_N) return -1;
-  return steps_layout(E, obs_dim, act_dim, n_steps).total;
+  return d4pg_replay_steps_window_bytes_ex(E, obs_dim, act_dim, n_steps, 0);
+}
+
+extern "C" int64_t d4pg_replay_steps_window_bytes_ex(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps, int32_t tails) {
+  if (E <= 0 || obs_dim <= 0 || act_dim <= 0 || n_steps < 1 || n_steps > D4PG_STEPS_MAX_N || (tails != 0 && tails != 1)) return -1;
+  return steps_layout(E, obs_dim, act_dim, n_steps, tails != 0).total;
+}
+
+extern "C" int32_t d4pg_replay_set_horizons(d4pg_replay_t* h, uint8_t* horizon, d4pg_stream_t stream) {
+  if (h) ++h->gen;
+  D4PG_REQUIRE(h, D4PG_EINVAL, "d4pg_replay_set_horizons: null handle");
+  if (horizon) D4PG_CUDA_OK(cudaMemsetAsync(horizon, 0, size_t(h->size), as_stream(stream)));
+  h->horizon = horizon;
+  return D4PG_OK;
 }
 
 extern "C" int32_t d4pg_replay_add_steps(d4pg_replay_t* h, int64_t E, const float* obs, const float* act, const double* rew,
                                          const float* obs2, const uint8_t* terminated, const uint8_t* episode_end,
                                          int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t prioritized,
                                          d4pg_stream_t stream) {
+  return d4pg_replay_add_steps_ex(h, E, obs, act, rew, obs2, terminated, episode_end, n_steps, gamma, window, n_rows, 0,
+                                  prioritized, stream);
+}
+
+extern "C" int32_t d4pg_replay_add_steps_ex(d4pg_replay_t* h, int64_t E, const float* obs, const float* act, const double* rew,
+                                            const float* obs2, const uint8_t* terminated, const uint8_t* episode_end,
+                                            int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t tails,
+                                            int32_t prioritized, d4pg_stream_t stream) {
   if (h && n_rows > 0) ++h->gen;          // a call that inserts no row leaves the store, and a prefetched batch, valid
   D4PG_REQUIRE(h && obs && act && rew && obs2 && terminated && window, D4PG_EINVAL, "d4pg_replay_add_steps: null argument");
   D4PG_REQUIRE(E > 0 && E <= h->size, D4PG_EINVAL, "d4pg_replay_add_steps: need 0 < E <= size (E=%lld)", (long long)E);
   D4PG_REQUIRE(n_steps >= 1 && n_steps <= D4PG_STEPS_MAX_N, D4PG_EINVAL, "d4pg_replay_add_steps: need 1 <= n_steps <= %d (got %d)",
                D4PG_STEPS_MAX_N, n_steps);
-  D4PG_REQUIRE(n_rows >= 0 && n_rows <= E, D4PG_EINVAL, "d4pg_replay_add_steps: need 0 <= n_rows <= E (n_rows=%lld)",
-               (long long)n_rows);
+  D4PG_REQUIRE(tails == 0 || tails == 1, D4PG_EINVAL, "d4pg_replay_add_steps: tails must be 0 or 1 (got %d)", tails);
+  D4PG_REQUIRE(!tails || h->horizon, D4PG_ESTATE, "d4pg_replay_add_steps: episode tails need a horizon column (d4pg_replay_set_horizons)");
+  // with tails an environment emits up to n - 1 rows per call
+  const int64_t max_rows = tails ? E * std::max(1, n_steps - 1) : E;
+  D4PG_REQUIRE(n_rows >= 0 && n_rows <= max_rows && n_rows <= h->size, D4PG_EINVAL,
+               "d4pg_replay_add_steps: need 0 <= n_rows <= %s (%lld) and <= size (n_rows=%lld)",
+               tails ? "E * max(1, n_steps - 1)" : "E", (long long)max_rows, (long long)n_rows);
   cudaStream_t st = as_stream(stream);
   const int64_t start = h->next_idx;
   const int64_t new_len = n_rows ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n_rows)) : h->len;
   const int64_t new_next = (start + n_rows) % h->size;
-  const StepsLayout l = steps_layout(E, h->obs_dim, h->act_dim, n_steps);
+  const StepsLayout l = steps_layout(E, h->obs_dim, h->act_dim, n_steps, tails != 0);
   uint8_t* wb = static_cast<uint8_t*>(window);
   StepsArgs a{};
   a.obs = obs; a.act = act; a.rew = rew; a.obs2 = obs2; a.term = terminated; a.end = episode_end;
@@ -896,12 +1008,17 @@ extern "C" int32_t d4pg_replay_add_steps(d4pg_replay_t* h, int64_t E, const floa
   a.rec = reinterpret_cast<unsigned long long*>(wb + l.rec); a.wr = reinterpret_cast<double*>(wb + l.wr);
   a.ws = reinterpret_cast<float*>(wb + l.ws); a.wa = reinterpret_cast<float*>(wb + l.wa);
   a.r_obs = h->obs; a.r_act = h->act; a.r_rew = h->rew; a.r_obs2 = h->obs2; a.r_done = h->done;
+  if (tails) { a.wo = reinterpret_cast<float*>(wb + l.wo); a.r_hz = h->horizon; }
   a.size = h->size; a.start = start; a.n_rows = n_rows; a.new_len = new_len; a.new_next = new_next;
   a.state = reinterpret_cast<ReplayState*>(h->state);
   // a CTA takes a contiguous chunk of environments, one warp per environment; the grid is at most 4 CTAs per SM
   const int64_t blocks = std::min<int64_t>((E + STEPS_WARPS - 1) / STEPS_WARPS, 4 * device_sm_count());
   a.chunk = (E + blocks - 1) / blocks;
-  replay_add_steps_kernel<<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
+  if (tails) replay_add_steps_kernel<true><<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
+  else {
+    if (int rc = zero_horizons(h, start, n_rows, st)) return rc;
+    replay_add_steps_kernel<false><<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
+  }
   D4PG_LAUNCH_OK();
   if (n_rows == 0) return D4PG_OK;
   // the rows just written, read back from the ring in insertion order: [start, size) then [0, ...)

@@ -73,8 +73,10 @@ struct SampleArgs {
   int pipe_slot;                    // >= 0 (prefetch pipeline): use the sampler's own counters, derive into this slot
   unsigned long long* trace; int trace_slot;
   unsigned long long* done_epoch;   // host pipeline: CTA b publishes (release) s_steps_done + 1 in [b] when its rows are gathered
-  const float* norm;                // observation normalizer affine {shift[S], scale[S]} (sample_body<true> only)
+  const float* norm;                // observation normalizer affine {shift[S], scale[S]} (sample_body<true, .> only)
   float norm_clip;
+  const uint8_t* horizon;           // the ring's per-row horizon column and the batch plane it is gathered into (HZ only)
+  uint8_t* hz;
 };
 
 constexpr int SAMPLE_THREADS = 256;
@@ -107,8 +109,9 @@ struct SampleSmem {
   float total;
 };
 // rows [bid*32, bid*32+32) of the batch, executed by one 256-thread CTA.  NORM: s and s2 are written through the
-// observation normalizer's affine (obs_norm.cuh) -- before the CTA's rows count as gathered.
-template <bool NORM>
+// observation normalizer's affine (obs_norm.cuh) -- before the CTA's rows count as gathered.  HZ: the rows' horizons
+// (episode tails) are gathered into a.hz.
+template <bool NORM, bool HZ>
 __device__ __forceinline__ void sample_body(const SampleArgs& a, int bid, SampleSmem& sm) {
   int32_t* idx_s = sm.idx;
   float* top_s = sm.top;
@@ -213,6 +216,7 @@ __device__ __forceinline__ void sample_body(const SampleArgs& a, int bid, Sample
     if (a.idx) a.idx[row] = leaf_idx;
     if (a.r) a.r[row] = a.rew[leaf_idx];
     if (a.d) a.d[row] = a.done[leaf_idx];
+    if (HZ) a.hz[row] = a.horizon[leaf_idx];
   }
   __syncthreads();
   // coalesced row gathers: consecutive threads walk consecutive features of one transition

@@ -94,6 +94,7 @@ class _Learner(object):
         cfg.max_grad_norm_actor, cfg.max_grad_norm_critic = ddpg.max_grad_norm
         cfg.weight_decay_actor, cfg.weight_decay_critic = opt_a.weight_decay(), opt_c.weight_decay()
         cfg.obs_norm = 1 if ddpg.obs_normalizer is not None else 0
+        cfg.nstep_tails = 1 if ddpg.nstep_tails else 0
         if cfg.obs_norm and cfg.world_size > 1:
             raise _lib.D4PGError("obs_norm is not supported with a communicator of world size > 1")
         if any(ddpg.max_grad_norm) and cfg.world_size > 1:
@@ -195,7 +196,7 @@ class DDPG:
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
                  importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None,
-                 obs_norm=None, param_noise=None):
+                 obs_norm=None, param_noise=None, nstep_tails=False):
         # adaptive parameter-space exploration noise (random_process.AdaptiveParamNoiseSpec, DESIGN §3): None = off
         if param_noise is not None and not isinstance(param_noise, AdaptiveParamNoiseSpec):
             raise ValueError("param_noise must be None or an AdaptiveParamNoiseSpec, got %r" % (param_noise,))
@@ -213,6 +214,13 @@ class DDPG:
         # "bf16": every MLP GEMM operand rounded to bf16, fp32 accumulate; runs the "levels" plan whatever `chain` says
         assert precision in ("fp32", "tf32x3", "tf32", "bf16")
         self.sampling, self.projection, self.precision = sampling, projection, precision
+        # episode tails (DESIGN.md §3 "Episode tails"): observe() also stores the last n_steps - 1 starts of every episode
+        # as shorter rows, each bootstrapped with gamma^k of its own horizon k.  Fixed here: the buffer and the learner
+        # both depend on it.  The reference projection discounts every row with gamma, so a horizon means nothing there
+        self.nstep_tails = bool(nstep_tails)
+        if self.nstep_tails and projection == "reference" and n_steps > 1:
+            raise ValueError('nstep_tails=True with n_steps > 1 needs projection="nstep": the reference projection '
+                             'discounts every row with gamma (no per-row horizon)')
         self.use_graph, self.philox_seed, self.comm = use_graph, philox_seed, comm
         # step plan of the MLP passes: "cluster" (default) cluster-fused layer chains (exact FFMA tiles for fp32,
         # wgmma tiles for tf32x3 / tf32), "levels" one launch per dependency level
@@ -306,12 +314,14 @@ class DDPG:
         self.prioritized_replay = prioritized_replay
         if self.prioritized_replay:                                                          # ddpg.py:78-87
             self.replayBuffer = PrioritizedReplayBuffer(self.memory_size, alpha=0.6, obs_dim=obs_dim,
-                                                        act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer)
+                                                        act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer,
+                                                        nstep_tails=self.nstep_tails)
             self.beta_schedule = LinearSchedule(100000, initial_p=0.4, final_p=1.0)
             self.prioritized_replay_eps = 1e-6
         else:
             self.replayBuffer = Replay(self.memory_size, self.env, n_steps=self.n_steps, gamma=self.gamma,
-                                       obs_dim=obs_dim, act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer)
+                                       obs_dim=obs_dim, act_dim=act_dim, device=self.device, obs_norm=self.obs_normalizer,
+                                       nstep_tails=self.nstep_tails)
         self._learner = None
 
     # ---- reference plumbing methods ------------------------------------------------------
@@ -397,7 +407,8 @@ class DDPG:
         the n-step windows kept on the device (DESIGN.md §3 "Streaming n-step insert").  s / s2 [E, obs_dim] (s2 the
         true next or final observation), a [E, act_dim] (e.g. what act() returned), r [E], terminated / truncated bool
         [E]; numpy, CPU or CUDA tensors.  With `a = ddpg.act(s)` and device-resident environments the rollout step
-        stays on the device.  Returns the number of rows inserted."""
+        stays on the device.  Returns the number of rows inserted.  With DDPG(nstep_tails=True) the last n_steps - 1
+        starts of every episode are stored too, at the next call (DESIGN.md §3 "Episode tails")."""
         return self.replayBuffer.add_steps(s, a, r, s2, terminated, truncated, n_steps=self.n_steps, gamma=self.gamma)
 
     # ---- action selection -------------------------------------------------------------------

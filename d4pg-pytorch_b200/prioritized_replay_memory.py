@@ -45,25 +45,35 @@ class StepsMirror(object):
     """add_steps' pending n-step windows: the fixed (E, n, gamma), the host mirror of each window's fill (steps of the
     current episode, capped at n - 1, which is all the emit decision needs) and the device state (window bytes, the
     pinned slot the end flags of a call with CUDA flags are copied back into, and that copy's event).  Environment e
-    emits a row at a call iff fill[e] == n - 1 before it, so the count is exact before the call without a device read."""
+    emits a row at a call iff fill[e] == n - 1 before it, so the count is exact before the call without a device read.
+    With episode tails (`tails`), an episode that ended also leaves tails[e] = min(its length, n - 1) rows, which e
+    emits at its next call."""
 
-    def __init__(self, E, n, gamma):
+    def __init__(self, E, n, gamma, tails=False):
         self.E, self.n, self.gamma = int(E), int(n), float(gamma)
         self.fill = np.zeros(self.E, dtype=np.int64)
+        self.tails = np.zeros(self.E, dtype=np.int64) if tails else None
         self.window = self.ends = self.event = None
         self.pending = False
 
     def rows(self):
         """Rows the next call inserts."""
-        return int(np.count_nonzero(self.fill >= self.n - 1))
+        full = int(np.count_nonzero(self.fill >= self.n - 1))
+        return full if self.tails is None else full + int(self.tails.sum())
 
     def advance(self):
-        """Every environment took one step."""
+        """Every environment took one step (and emitted its pending tails first)."""
         np.minimum(self.fill + 1, self.n - 1, out=self.fill)
+        if self.tails is not None:
+            self.tails[:] = 0
 
     def end(self, ended):
-        """Clear the windows of the environments whose episode ended (bool [E])."""
-        self.fill[np.asarray(ended, dtype=bool)] = 0
+        """Clear the windows of the environments whose episode ended (bool [E]); with tails, their last
+        min(length, n - 1) starts become pending."""
+        ended = np.asarray(ended, dtype=bool)
+        if self.tails is not None:
+            self.tails[ended] = self.fill[ended]          # fill = min(length, n - 1) after advance()
+        self.fill[ended] = 0
 
 
 class _DeviceReplay(object):
@@ -72,8 +82,12 @@ class _DeviceReplay(object):
 
     STAGE_ROWS = 4096
 
-    def __init__(self, size, alpha, prioritized, obs_dim=None, act_dim=None, device=None, obs_norm=None):
+    def __init__(self, size, alpha, prioritized, obs_dim=None, act_dim=None, device=None, obs_norm=None,
+                 nstep_tails=False):
         self.size = int(size)
+        # episode tails of add_steps (DESIGN.md §3 "Episode tails"): a u8 horizon column beside `done`, fixed at construction
+        self.nstep_tails = bool(nstep_tails)
+        self.horizon = None
         self.obs_norm = obs_norm         # ObsNormalizer (obs_norm.py): registered when the store is allocated
         self.alpha = float(alpha)
         self.prioritized = bool(prioritized)
@@ -119,6 +133,10 @@ class _DeviceReplay(object):
                                                  _lib.ptr(self.state), _lib.stream_ptr(), C.byref(h)),
                    "d4pg_replay_create")
         self.handle = h
+        if self.nstep_tails:
+            self.horizon = torch.zeros(n, dtype=torch.uint8, device=dev)
+            _lib.check(_lib.lib().d4pg_replay_set_horizons(h, _lib.ptr(self.horizon), _lib.stream_ptr()),
+                       "d4pg_replay_set_horizons")
         if self.obs_norm is not None:
             self.obs_norm._bind(self)
         R = self.STAGE_ROWS
@@ -370,6 +388,9 @@ class _DeviceReplay(object):
             raise ValueError("add_steps: rows of (%d, %d) into a buffer of (%d, %d)" % (S, A, self.obs_dim, self.act_dim))
         if E > self.size:
             raise ValueError("add_steps: E = %d environments exceed the buffer size %d" % (E, self.size))
+        if self.nstep_tails and E * max(1, int(n_steps) - 1) > self.size:
+            raise ValueError("add_steps: with nstep_tails one call can insert E * (n_steps - 1) = %d rows, more than the "
+                             "buffer size %d" % (E * (int(n_steps) - 1), self.size))
         w = self._steps
         if w is not None and (w.E, w.n, w.gamma) != (E, int(n_steps), float(gamma)):
             raise ValueError("add_steps: the pending windows hold E=%d, n_steps=%d, gamma=%r; this call has E=%d, "
@@ -389,9 +410,9 @@ class _DeviceReplay(object):
         dev = self.device
         w = self._steps
         if w is None:
-            w = self._steps = StepsMirror(E, n, gamma)
+            w = self._steps = StepsMirror(E, n, gamma, self.nstep_tails)
         if w.window is None:
-            nbytes = int(_lib.lib().d4pg_replay_steps_window_bytes(E, S, A, n))
+            nbytes = int(_lib.lib().d4pg_replay_steps_window_bytes_ex(E, S, A, n, 1 if self.nstep_tails else 0))
             w.window = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
             w.ends = torch.zeros(2, E, dtype=torch.uint8, pin_memory=True)
             w.event = torch.cuda.Event()
@@ -412,9 +433,10 @@ class _DeviceReplay(object):
                 torch.as_tensor(action, dtype=torch.float32).to(dev).contiguous(),
                 torch.as_tensor(reward, dtype=torch.float64).to(dev).contiguous(),
                 torch.as_tensor(obs_next, dtype=torch.float32).to(dev).contiguous(), term, trunc]
-        _lib.check(_lib.lib().d4pg_replay_add_steps(self.handle, E, *[_lib.ptr(t) for t in args], n, gamma,
-                                                    _lib.ptr(w.window), n_rows, 1 if self.prioritized else 0,
-                                                    _lib.stream_ptr()), "d4pg_replay_add_steps")
+        _lib.check(_lib.lib().d4pg_replay_add_steps_ex(self.handle, E, *[_lib.ptr(t) for t in args], n, gamma,
+                                                       _lib.ptr(w.window), n_rows, 1 if self.nstep_tails else 0,
+                                                       1 if self.prioritized else 0, _lib.stream_ptr()),
+                   "d4pg_replay_add_steps_ex")
         w.advance()
         if on_dev:                                # the episode ends are applied at the next call
             w.ends[0].copy_(term, non_blocking=True)
@@ -434,7 +456,8 @@ class _DeviceReplay(object):
         return n_rows
 
     def drop_steps(self):
-        """Discard the pending n-step windows; the next add_steps may use another E, n_steps or gamma."""
+        """Discard the pending n-step windows (and pending episode tails); the next add_steps may use another E, n_steps
+        or gamma."""
         self._steps = None
 
     def _add_device(self, n, tensors):
@@ -620,10 +643,10 @@ class ReplayBuffer(object):
 
     _prioritized = False
 
-    def __init__(self, size, obs_dim=None, act_dim=None, device=None, _alpha=1.0, obs_norm=None):
+    def __init__(self, size, obs_dim=None, act_dim=None, device=None, _alpha=1.0, obs_norm=None, nstep_tails=False):
         self._maxsize = size
         self._store = _DeviceReplay(size, _alpha, self._prioritized, obs_dim, act_dim, device,
-                                    make_obs_normalizer(obs_norm, obs_dim, device))
+                                    make_obs_normalizer(obs_norm, obs_dim, device), nstep_tails)
 
     @property
     def obs_normalizer(self):
@@ -672,7 +695,14 @@ class ReplayBuffer(object):
 
         The first call fixes E, n_steps and gamma; a call that changes one raises ValueError until drop_steps().  CUDA
         terminated / truncated are read back asynchronously and waited for at the next call.  The pending windows are
-        not part of any checkpoint."""
+        not part of any checkpoint.
+
+        With nstep_tails=True (DESIGN.md §3 "Episode tails") an episode of L steps that ends -- terminated or
+        truncated -- also stores its last min(L, n_steps - 1) starts u as shorter rows (s_u, a_u, R over the k = L - u
+        remaining rewards, the final obs_next, terminated) with horizon k in `_store.horizon` (0 for every full row), so
+        a learner bootstraps them with gamma^k.  They are inserted by the NEXT call, ahead of that call's own rows, and
+        are lost by drop_steps(); nothing flushes them when the stream stops.  One call may then insert up to
+        E * (n_steps - 1) rows, which must not exceed the buffer size."""
         return self._store.add_steps(obs, action, reward, obs_next, terminated, truncated, n_steps, gamma)
 
     def drop_steps(self):
@@ -692,10 +722,11 @@ class PrioritizedReplayBuffer(ReplayBuffer):
 
     _prioritized = True
 
-    def __init__(self, size, alpha, obs_dim=None, act_dim=None, device=None, obs_norm=None):
+    def __init__(self, size, alpha, obs_dim=None, act_dim=None, device=None, obs_norm=None, nstep_tails=False):
         assert alpha >= 0                                                                    # :240
         self._alpha = alpha
-        super(PrioritizedReplayBuffer, self).__init__(size, obs_dim, act_dim, device, _alpha=alpha, obs_norm=obs_norm)
+        super(PrioritizedReplayBuffer, self).__init__(size, obs_dim, act_dim, device, _alpha=alpha, obs_norm=obs_norm,
+                                                      nstep_tails=nstep_tails)
         self._it_sum = _TreeView(self._store, 0)
         self._it_min = _TreeView(self._store, 1)
 

@@ -17,14 +17,16 @@ from .prioritized_replay_memory import _DeviceReplay
 
 
 class Replay(object):
-    def __init__(self, max_size, env, n_steps=1, gamma=0.99, obs_dim=None, act_dim=None, device=None, obs_norm=None):
+    def __init__(self, max_size, env, n_steps=1, gamma=0.99, obs_dim=None, act_dim=None, device=None, obs_norm=None,
+                 nstep_tails=False):
         self.capacity = max_size
         self.env = env
         self.n_steps = n_steps
         self.gamma = gamma
-        # obs_norm: None / False, True, {"clip": c, "eps": e} or an ObsNormalizer that every insert updates (obs_norm.py)
+        # obs_norm: None / False, True, {"clip": c, "eps": e} or an ObsNormalizer that every insert updates (obs_norm.py);
+        # nstep_tails: add_steps also stores the last n_steps - 1 starts of every episode (ReplayBuffer.add_steps)
         self._store = _DeviceReplay(max_size, 1.0, False, obs_dim, act_dim, device,
-                                    make_obs_normalizer(obs_norm, obs_dim, device))
+                                    make_obs_normalizer(obs_norm, obs_dim, device), nstep_tails)
 
     @property
     def obs_normalizer(self):

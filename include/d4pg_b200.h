@@ -227,6 +227,24 @@ int32_t d4pg_replay_add_steps(d4pg_replay_t* h, int64_t E, const float* obs, con
                               int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t prioritized,
                               d4pg_stream_t stream);
 
+/* Episode tails of the streaming insert (DESIGN.md §3 "Episode tails").  d4pg_replay_set_horizons registers a
+ * caller-owned device column horizon u8 [size] with the replay and zero-fills it on `stream` (NULL unregisters): every
+ * row then carries its bootstrap horizon, 0 for a full-horizon row.  Every insert path clears the horizons of the slots
+ * it writes (a cudaMemsetAsync on the stream of its ring write), except d4pg_replay_add_steps_ex with tails = 1.
+ * d4pg_replay_add_steps_ex with tails = 0 is d4pg_replay_add_steps.  With tails = 1 (needs the column; D4PG_ESTATE
+ * otherwise) an episode of L steps that ends at call k -- terminated or truncated -- also yields, at call k+1 and before
+ * that call's own step, one tail row per start u in [max(0, L-n+1), L-1]: (s_u, a_u, the f64 n-step return over its
+ * k = L-u remaining rewards, obs_next and terminated of step L-1) with horizon k; full rows get horizon 0.  Rows of one
+ * call go in ascending environment, then ascending u.  n_rows counts tail rows too: at most E * max(1, n_steps-1) and
+ * at most size.  The window of a tails call is d4pg_replay_steps_window_bytes_ex(E, obs_dim, act_dim, n_steps, 1)
+ * bytes (it also keeps the ending step's obs_next); a window is used with one tails setting only. */
+int32_t d4pg_replay_set_horizons(d4pg_replay_t* h, uint8_t* horizon, d4pg_stream_t stream);
+int64_t d4pg_replay_steps_window_bytes_ex(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps, int32_t tails);
+int32_t d4pg_replay_add_steps_ex(d4pg_replay_t* h, int64_t E, const float* obs, const float* act, const double* rew,
+                                 const float* obs2, const uint8_t* terminated, const uint8_t* episode_end,
+                                 int32_t n_steps, double gamma, void* window, int64_t n_rows, int32_t tails,
+                                 int32_t prioritized, d4pg_stream_t stream);
+
 /* Hindsight-experience relabelling on the device (main.py:154-184, "future" strategy) as a gather kernel that produces
  * the rows d4pg_replay_add then inserts.  Episode of T goal-conditioned steps: obs / obs_next f32 [T, obs_dim], goal
  * f64 [T, goal_dim] (desired goal of every step), ag_next f64 [T, goal_dim] (achieved goal of the next state), act f32
@@ -512,6 +530,12 @@ typedef struct {
                                  and stay registered, with the same buffers and clip, for the learner's lifetime).
                                  0 = off.  Not supported with world_size > 1 (D4PG_EINVAL): each rank would normalize with
                                  the statistics of its own shard */
+  int32_t nstep_tails;        /* 1: batches carry per-row horizons (d4pg_replay_set_horizons, registered before
+                                 d4pg_learner_create and kept for the learner's lifetime): a row of horizon k > 0 that is
+                                 not done bootstraps with gamma^k, computed on the host with pow(gamma, k) like the
+                                 gamma^n_steps of full rows; every critic type.  D4PG_EINVAL with proj_mode 0 and
+                                 n_steps > 1 (its gamma-for-every-row rule has no horizon) or without a horizon column.
+                                 0 = off */
 } d4pg_learner_config_t;
 
 /* Caller-owned device buffers.  P_a / P_c = d4pg_*_layout().total. */
