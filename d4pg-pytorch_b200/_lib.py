@@ -16,6 +16,7 @@ HIDDEN = 256
 MAX_ATOMS = 128
 MAX_COMPONENTS = 32
 STEPS_MAX_N = 64          # D4PG_STEPS_MAX_N: the longest n-step window of d4pg_replay_add_steps
+GOAL_MAX_STEPS = 65536    # D4PG_GOAL_MAX_STEPS: the longest episode window of d4pg_replay_add_goal_steps
 
 c_float_p = C.POINTER(C.c_float)
 c_double_p = C.POINTER(C.c_double)
@@ -107,6 +108,10 @@ _PROTOS = {
     "d4pg_replay_steps_window_bytes_ex": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "d4pg_replay_add_steps_ex": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int64,
                                              C.c_int32, C.c_int32, _P]),
+    "d4pg_replay_goal_window_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "d4pg_replay_add_goal_steps": (C.c_int32, [_P, C.c_int64, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                               C.c_int32, _P, _P, C.c_int64, C.c_int64, C.c_double, C.c_int32, C.c_int32,
+                                               C.c_int32, _P]),
     "d4pg_her_relabel": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                      C.c_double, C.c_int32, _P, _P, _P, _P, _P, _P]),
     "d4pg_replay_set_len": (C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int32, _P]),

@@ -75,7 +75,7 @@ __global__ void softmax_rows_kernel(const float* logits, float* probs, int B, in
 using namespace d4pg;
 
 extern "C" const char* d4pg_last_error(void) { return g_err; }
-extern "C" int32_t d4pg_version(void) { return 1100; }   /* 0.11.0 */
+extern "C" int32_t d4pg_version(void) { return 1200; }   /* 0.12.0 */
 /* sizeof of the structs that cross the ABI by pointer: a binding whose mirror has another size is out of date */
 extern "C" int32_t d4pg_struct_size(int32_t which) {
   switch (which) {

@@ -691,6 +691,18 @@ struct HerArgs {
   int T, So, G, A, action_mode; double threshold;
   float* o_s; float* o_a; double* o_r; float* o_s2; uint8_t* o_d;
 };
+// The relabelled copy's reward: -(||ag[t] - ag[f]||_2 > a.threshold) in f64, ag the achieved goals [*, a.G] of an
+// episode (ag[t] after the step, ag[f] after its future step: the new goal), the sum of squares left to right.
+// her_relabel_kernel (HerArgs) and the streaming relabel (replay_add_goal_steps_kernel, GoalArgs) both call it.
+template <class Args>
+__device__ __forceinline__ double her_reward(const Args& a, const double* ag, int t, int f) {
+  double ss = 0.0;
+  for (int j = 0; j < a.G; ++j) {
+    const double d = __dsub_rn(ag[size_t(t) * a.G + j], ag[size_t(f) * a.G + j]);
+    ss = __dadd_rn(ss, __dmul_rn(d, d));
+  }
+  return (__dsqrt_rn(ss) > a.threshold) ? -1.0 : -0.0;     // -(d > threshold), as gym-robotics returns it
+}
 __global__ void her_relabel_kernel(const HerArgs a) {
   const int t = blockIdx.x;
   if (t >= a.T) return;
@@ -717,12 +729,7 @@ __global__ void her_relabel_kernel(const HerArgs a) {
     a.o_r[row] = a.rew[t];
     a.o_d[row] = a.done[t];
     if (sel) {
-      double ss = 0.0;
-      for (int j = 0; j < a.G; ++j) {
-        const double d = __dsub_rn(a.ag_next[size_t(t) * a.G + j], a.ag_next[size_t(f) * a.G + j]);
-        ss = __dadd_rn(ss, __dmul_rn(d, d));
-      }
-      const double r = (__dsqrt_rn(ss) > a.threshold) ? -1.0 : -0.0;     // -(d > threshold), as gym-robotics returns it
+      const double r = her_reward(a, a.ag_next, t, f);
       a.o_r[row + 1] = r;
       a.o_d[row + 1] = (r == 0.0) ? 1 : 0;
     }
@@ -1022,6 +1029,175 @@ extern "C" int32_t d4pg_replay_add_steps_ex(d4pg_replay_t* h, int64_t E, const f
   D4PG_LAUNCH_OK();
   if (n_rows == 0) return D4PG_OK;
   // the rows just written, read back from the ring in insertion order: [start, size) then [0, ...)
+  const int64_t n1 = std::min<int64_t>(n_rows, h->size - start);
+  return replay_insert_tail(h, n_rows, start, new_len, new_next, h->obs + start * h->obs_dim, n1, h->obs, prioritized, st);
+}
+
+// ---- device-side ingest: streaming hindsight relabelling (DESIGN.md §3 "Streaming hindsight relabelling") ----------
+// One call = one vector step of E goal-conditioned environments.  Environment e appends step t of its current episode
+// to its window; an episode that ended at the previous call (its record's end bit) is emitted first, then the window
+// restarts with this call's step.  One warp per environment does both, in that order, so the step that starts the new
+// episode overwrites slot 0 only after every lane has read the emitted episode (a __syncwarp between them): one
+// episode slot per environment is enough, and the emitted rows need no second launch.
+//
+// Window (caller-owned, zero-filled before the first call; d4pg_replay_goal_window_bytes), M = max_episode_steps:
+//   rec u32 [E]        bits 0-30: steps of the current episode, bit 31: it ended at the last call
+//   obs, obs2 f32 [E, M, So]   act f32 [E, M, A]   goal, ag f64 [E, M, G]   rew f64 [E, M]   term u8 [E, M]
+// Plan (the host's draws, uploaded with one copy; NULL when no episode is emitted), i32:
+//   step_off [E]       first draw of e's emitted episode (read only for an environment that emits)
+//   future [n_draws]   future step of the relabelled copy of (e, t), -1 = no copy
+//   dst [n_draws]      rank of the original row of (e, t) in this call; its copy takes dst + 1
+constexpr int GOAL_THREADS = 256, GOAL_WARPS = GOAL_THREADS / 32;
+struct GoalArgs {
+  const float* obs; const double* goal; const float* act; const double* rew; const float* obs2; const double* ag2;
+  const uint8_t* term; const uint8_t* end;
+  int64_t E; int So, G, A, M, action_mode, no_step; double threshold;
+  uint32_t* rec; float* w_obs; float* w_obs2; float* w_act; double* w_goal; double* w_ag; double* w_rew; uint8_t* w_term;
+  const int32_t* step_off; const int32_t* future; const int32_t* dst; int64_t n_draws;
+  float* r_obs; float* r_act; double* r_rew; float* r_obs2; uint8_t* r_done;
+  int64_t size, start, n_rows, new_len, new_next; ReplayState* state;
+};
+
+__global__ void __launch_bounds__(GOAL_THREADS) replay_add_goal_steps_kernel(const GoalArgs a) {
+  const int lane = threadIdx.x & 31, So = a.So, G = a.G, A = a.A, M = a.M, S = So + G;
+  const int64_t e = int64_t(blockIdx.x) * GOAL_WARPS + (threadIdx.x >> 5);
+  if (blockIdx.x == 0 && threadIdx.x == 0) { a.state->len = a.new_len; a.state->next_idx = a.new_next; }
+  if (e >= a.E) return;
+  const uint32_t rc = a.rec[e];
+  const bool ended = (rc >> 31) != 0;
+  int fill = int(rc & 0x7fffffffu);
+  const int64_t w0 = e * M;                                   // window row of step 0
+  if (ended && a.step_off) {
+    // emit the ended episode of L steps: the original row of t at dst, its relabelled copy (if any) at dst + 1
+    const int L = fill;
+    const int64_t d0 = a.step_off[e];
+    const float* last_act = a.w_act + (w0 + L - 1) * A;
+    for (int t = 0; t < L && d0 + t < a.n_draws; ++t) {
+      const int64_t rank = a.dst[d0 + t];
+      const int f = a.future[d0 + t];
+      const float* so = a.w_obs + (w0 + t) * So;
+      const float* sn = a.w_obs2 + (w0 + t) * So;
+      const float* at = a.w_act + (w0 + t) * A;
+      if (rank < a.n_rows) {                                  // never outside [start, start + n_rows)
+        int64_t p = a.start + rank;                            // start < size and rank < n_rows <= size
+        if (p >= a.size) p -= a.size;
+        const double* g = a.w_goal + (w0 + t) * G;
+        for (int j = lane; j < So; j += 32) { a.r_obs[p * S + j] = so[j]; a.r_obs2[p * S + j] = sn[j]; }
+        for (int j = lane; j < G; j += 32) { const float v = float(g[j]); a.r_obs[p * S + So + j] = v; a.r_obs2[p * S + So + j] = v; }
+        for (int j = lane; j < A; j += 32) a.r_act[p * A + j] = at[j];
+        if (lane == 0) { a.r_rew[p] = a.w_rew[w0 + t]; a.r_done[p] = a.w_term[w0 + t]; }
+      }
+      if (f >= t && f < L && rank + 1 < a.n_rows) {
+        int64_t q = a.start + rank + 1;
+        if (q >= a.size) q -= a.size;
+        const double* g2 = a.w_ag + (w0 + f) * G;             // goal' = the achieved goal after step f
+        const float* ac = a.action_mode ? at : last_act;
+        for (int j = lane; j < So; j += 32) { a.r_obs[q * S + j] = so[j]; a.r_obs2[q * S + j] = sn[j]; }
+        for (int j = lane; j < G; j += 32) { const float v = float(g2[j]); a.r_obs[q * S + So + j] = v; a.r_obs2[q * S + So + j] = v; }
+        for (int j = lane; j < A; j += 32) a.r_act[q * A + j] = ac[j];
+        if (lane == 0) {
+          const double r = her_reward(a, a.w_ag, int(w0 + t), int(w0 + f));   // E * M < size
+          a.r_rew[q] = r;
+          a.r_done[q] = (r == 0.0) ? 1 : 0;
+        }
+      }
+    }
+  }
+  if (ended) fill = 0;
+  __syncwarp();                                               // every lane has read the record and the emitted episode
+  if (a.no_step) {                                            // flush: emit only; running episodes keep their windows
+    if (ended && lane == 0) a.rec[e] = 0u;
+    return;
+  }
+  const int slot = fill;
+  if (slot < M) {                                             // the host never lets an episode outgrow its window
+    const int64_t w = w0 + slot;
+    for (int j = lane; j < So; j += 32) { a.w_obs[w * So + j] = a.obs[e * So + j]; a.w_obs2[w * So + j] = a.obs2[e * So + j]; }
+    for (int j = lane; j < G; j += 32) { a.w_goal[w * G + j] = a.goal[e * G + j]; a.w_ag[w * G + j] = a.ag2[e * G + j]; }
+    for (int j = lane; j < A; j += 32) a.w_act[w * A + j] = a.act[e * A + j];
+  }
+  if (lane == 0) {
+    const bool term = a.term[e] != 0, end_now = term || (a.end && a.end[e] != 0);
+    if (slot < M) { a.w_rew[w0 + slot] = a.rew[e]; a.w_term[w0 + slot] = term ? 1 : 0; }
+    a.rec[e] = uint32_t(min(slot + 1, M)) | (end_now ? 0x80000000u : 0u);
+  }
+}
+
+namespace {
+struct GoalLayout { int64_t rec, obs, obs2, act, goal, ag, rew, term, total; };
+GoalLayout goal_layout(int64_t E, int64_t So, int64_t G, int64_t A, int64_t M) {
+  auto up = [](int64_t b) { return (b + 15) & ~int64_t(15); };
+  GoalLayout l;
+  l.rec = 0;
+  l.obs = up(l.rec + E * 4);
+  l.obs2 = up(l.obs + E * M * So * 4);
+  l.act = up(l.obs2 + E * M * So * 4);
+  l.goal = up(l.act + E * M * A * 4);
+  l.ag = up(l.goal + E * M * G * 8);
+  l.rew = up(l.ag + E * M * G * 8);
+  l.term = up(l.rew + E * M * 8);
+  l.total = up(l.term + E * M);
+  return l;
+}
+}  // namespace
+
+extern "C" int64_t d4pg_replay_goal_window_bytes(int64_t E, int32_t obs_dim, int32_t goal_dim, int32_t act_dim,
+                                                 int32_t max_episode_steps) {
+  if (E <= 0 || obs_dim <= 0 || goal_dim <= 0 || act_dim <= 0 || max_episode_steps < 1 ||
+      max_episode_steps > D4PG_GOAL_MAX_STEPS) return -1;
+  return goal_layout(E, obs_dim, goal_dim, act_dim, max_episode_steps).total;
+}
+
+extern "C" int32_t d4pg_replay_add_goal_steps(d4pg_replay_t* h, int64_t E, int32_t obs_dim, int32_t goal_dim,
+                                              const float* obs, const double* goal, const float* act, const double* rew,
+                                              const float* obs2, const double* ag2, const uint8_t* terminated,
+                                              const uint8_t* episode_end, int32_t max_episode_steps, void* window,
+                                              const int32_t* plan, int64_t n_draws, int64_t n_rows, double threshold,
+                                              int32_t her_action_mode, int32_t no_step, int32_t prioritized,
+                                              d4pg_stream_t stream) {
+  if (h && n_rows > 0) ++h->gen;          // a call that inserts no row leaves the store, and a prefetched batch, valid
+  D4PG_REQUIRE(h && window, D4PG_EINVAL, "d4pg_replay_add_goal_steps: null argument");
+  D4PG_REQUIRE(no_step == 0 || no_step == 1, D4PG_EINVAL, "d4pg_replay_add_goal_steps: no_step must be 0 or 1 (got %d)", no_step);
+  D4PG_REQUIRE(no_step || (obs && goal && act && rew && obs2 && ag2 && terminated), D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: null step input");
+  D4PG_REQUIRE(E > 0 && E <= h->size, D4PG_EINVAL, "d4pg_replay_add_goal_steps: need 0 < E <= size (E=%lld)", (long long)E);
+  D4PG_REQUIRE(obs_dim > 0 && goal_dim > 0 && int64_t(obs_dim) + goal_dim == h->obs_dim, D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: obs_dim + goal_dim must equal the replay's obs_dim %d (got %d + %d)",
+               h->obs_dim, obs_dim, goal_dim);
+  D4PG_REQUIRE(max_episode_steps >= 1 && max_episode_steps <= D4PG_GOAL_MAX_STEPS, D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: need 1 <= max_episode_steps <= %d (got %d)", D4PG_GOAL_MAX_STEPS, max_episode_steps);
+  D4PG_REQUIRE(std::isfinite(threshold) && threshold >= 0.0, D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: threshold must be finite and >= 0 (got %g)", threshold);
+  D4PG_REQUIRE(her_action_mode == 0 || her_action_mode == 1, D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: her_action_mode must be 0 or 1 (got %d)", her_action_mode);
+  const int64_t M = max_episode_steps;
+  D4PG_REQUIRE(n_draws >= 0 && n_draws <= E * M && (n_draws == 0 || plan), D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: need 0 <= n_draws <= E * max_episode_steps and a plan when n_draws > 0");
+  D4PG_REQUIRE(n_rows >= 0 && n_rows <= 2 * n_draws && n_rows <= h->size, D4PG_EINVAL,
+               "d4pg_replay_add_goal_steps: need 0 <= n_rows <= 2 * n_draws and <= size (n_rows=%lld)", (long long)n_rows);
+  cudaStream_t st = as_stream(stream);
+  const int64_t start = h->next_idx;
+  const int64_t new_len = n_rows ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n_rows)) : h->len;
+  const int64_t new_next = (start + n_rows) % h->size;
+  const GoalLayout l = goal_layout(E, obs_dim, goal_dim, h->act_dim, M);
+  uint8_t* wb = static_cast<uint8_t*>(window);
+  GoalArgs a{};
+  a.obs = obs; a.goal = goal; a.act = act; a.rew = rew; a.obs2 = obs2; a.ag2 = ag2; a.term = terminated; a.end = episode_end;
+  a.E = E; a.So = obs_dim; a.G = goal_dim; a.A = h->act_dim; a.M = max_episode_steps;
+  a.action_mode = her_action_mode; a.no_step = no_step; a.threshold = threshold;
+  a.rec = reinterpret_cast<uint32_t*>(wb + l.rec);
+  a.w_obs = reinterpret_cast<float*>(wb + l.obs); a.w_obs2 = reinterpret_cast<float*>(wb + l.obs2);
+  a.w_act = reinterpret_cast<float*>(wb + l.act); a.w_goal = reinterpret_cast<double*>(wb + l.goal);
+  a.w_ag = reinterpret_cast<double*>(wb + l.ag); a.w_rew = reinterpret_cast<double*>(wb + l.rew); a.w_term = wb + l.term;
+  if (n_draws > 0) { a.step_off = plan; a.future = plan + E; a.dst = plan + E + n_draws; }
+  a.n_draws = n_draws;
+  a.r_obs = h->obs; a.r_act = h->act; a.r_rew = h->rew; a.r_obs2 = h->obs2; a.r_done = h->done;
+  a.size = h->size; a.start = start; a.n_rows = n_rows; a.new_len = new_len; a.new_next = new_next;
+  a.state = reinterpret_cast<ReplayState*>(h->state);
+  if (int rc = zero_horizons(h, start, n_rows, st)) return rc;
+  replay_add_goal_steps_kernel<<<unsigned((E + GOAL_WARPS - 1) / GOAL_WARPS), GOAL_THREADS, 0, st>>>(a);
+  D4PG_LAUNCH_OK();
+  if (n_rows == 0) return D4PG_OK;
   const int64_t n1 = std::min<int64_t>(n_rows, h->size - start);
   return replay_insert_tail(h, n_rows, start, new_len, new_next, h->obs + start * h->obs_dim, n1, h->obs, prioritized, st);
 }

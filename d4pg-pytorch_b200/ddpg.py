@@ -20,7 +20,7 @@ import torch
 from . import _lib
 from .models import actor, critic
 from .obs_norm import make_obs_normalizer
-from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer
+from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer, check_her_params
 from .random_process import AdaptiveParamNoiseSpec, GaussianNoise, OrnsteinUhlenbeckProcess
 from .replay_memory import Replay
 from .shared_adam import SharedAdam, check_max_grad_norm
@@ -186,6 +186,22 @@ class _Learner(object):
             pass
 
 
+HER_DEFAULTS = {"her_ratio": 0.8, "threshold": 0.05, "her_action": "reference", "max_episode_steps": 50, "seed": 0}
+
+
+def _her_params(her):
+    """DDPG(her=...): None / False -> None, True -> the defaults, a dict -> the defaults updated with it, validated."""
+    if her is None or her is False:
+        return None
+    if her is True:
+        her = {}
+    if not isinstance(her, dict) or set(her) - set(HER_DEFAULTS):
+        raise ValueError("her must be None, True or a dict with keys from %s, got %r" % (sorted(HER_DEFAULTS), her))
+    p = dict(HER_DEFAULTS, **her)
+    return dict(zip(("her_ratio", "threshold", "her_action", "max_episode_steps", "seed"),
+                    check_her_params(p["her_ratio"], p["threshold"], p["her_action"], p["max_episode_steps"], p["seed"])))
+
+
 class DDPG:
     replayBuffer = None
 
@@ -196,7 +212,7 @@ class DDPG:
                  device=None, sampling="reference", projection="reference", precision="fp32",
                  use_graph=True, philox_seed=0, comm=None, chain="cluster", prefetch=True, track_weights=True,
                  importance_weighted=False, priority="reference", actor_critic="reference", max_grad_norm=None,
-                 obs_norm=None, param_noise=None, nstep_tails=False):
+                 obs_norm=None, param_noise=None, nstep_tails=False, her=None):
         # adaptive parameter-space exploration noise (random_process.AdaptiveParamNoiseSpec, DESIGN §3): None = off
         if param_noise is not None and not isinstance(param_noise, AdaptiveParamNoiseSpec):
             raise ValueError("param_noise must be None or an AdaptiveParamNoiseSpec, got %r" % (param_noise,))
@@ -221,6 +237,13 @@ class DDPG:
         if self.nstep_tails and projection == "reference" and n_steps > 1:
             raise ValueError('nstep_tails=True with n_steps > 1 needs projection="nstep": the reference projection '
                              'discounts every row with gamma (no per-row horizon)')
+        # streaming hindsight relabelling (DESIGN.md §3 "Streaming hindsight relabelling"): observe_goals() stores goal-
+        # conditioned steps with these parameters.  None = off, True = the defaults, or a dict of some of them.  One-step
+        # rows only, as main.py stores them: n-step returns over relabelled rewards are not defined here
+        self.her = _her_params(her)
+        if self.her is not None and n_steps > 1:
+            raise ValueError("her= stores one-step transitions (main.py:154-184); it cannot be combined with n_steps = %r"
+                             % (n_steps,))
         self.use_graph, self.philox_seed, self.comm = use_graph, philox_seed, comm
         # step plan of the MLP passes: "cluster" (default) cluster-fused layer chains (exact FFMA tiles for fp32,
         # wgmma tiles for tf32x3 / tf32), "levels" one launch per dependency level
@@ -410,6 +433,18 @@ class DDPG:
         stays on the device.  Returns the number of rows inserted.  With DDPG(nstep_tails=True) the last n_steps - 1
         starts of every episode are stored too, at the next call (DESIGN.md §3 "Episode tails")."""
         return self.replayBuffer.add_steps(s, a, r, s2, terminated, truncated, n_steps=self.n_steps, gamma=self.gamma)
+
+    def observe_goals(self, obs, desired_goal, a, r, obs_next, achieved_goal_next, terminated, truncated=None):
+        """Store one vector step of E goal-conditioned environments with hindsight relabelling on the device:
+        `replayBuffer.add_goal_steps(..., **her)` with the parameters of DDPG(her=...) (DESIGN.md §3 "Streaming
+        hindsight relabelling").  obs / obs_next [E, So], desired_goal / achieved_goal_next [E, G], a [E, act_dim],
+        r [E], terminated / truncated bool [E]; numpy, CPU or CUDA tensors; this DDPG's obs_dim is So + G.  An episode
+        that ends is inserted, with its relabelled copies, at the next call (or replayBuffer.flush_goal_steps()).
+        Returns the number of rows inserted."""
+        if self.her is None:
+            raise ValueError("observe_goals needs DDPG(her=True or a dict of HER parameters)")
+        return self.replayBuffer.add_goal_steps(obs, desired_goal, a, r, obs_next, achieved_goal_next, terminated,
+                                                truncated, **self.her)
 
     # ---- action selection -------------------------------------------------------------------
     def act(self, state, explore=True, reset=None):

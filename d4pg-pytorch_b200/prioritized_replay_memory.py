@@ -76,6 +76,91 @@ class StepsMirror(object):
         self.fill[ended] = 0
 
 
+HER_ACTIONS = ("reference", "own")
+
+
+def check_her_params(her_ratio, threshold, her_action, max_episode_steps, seed):
+    """The parameters of add_goal_steps, validated -> (her_ratio, threshold, her_action, max_episode_steps, seed)."""
+    try:
+        ratio, thr = float(her_ratio), float(threshold)
+    except (TypeError, ValueError):
+        raise ValueError("add_goal_steps: her_ratio and threshold must be numbers, got %r / %r" % (her_ratio, threshold))
+    if not 0.0 <= ratio <= 1.0:
+        raise ValueError("add_goal_steps: her_ratio must be in [0, 1], got %r" % (her_ratio,))
+    if not (np.isfinite(thr) and thr >= 0.0):
+        raise ValueError("add_goal_steps: threshold must be finite and >= 0, got %r" % (threshold,))
+    if her_action not in HER_ACTIONS:
+        raise ValueError("add_goal_steps: her_action must be 'reference' (the episode's last action, main.py:184) or "
+                         "'own' (the step's action), got %r" % (her_action,))
+    if isinstance(max_episode_steps, bool) or int(max_episode_steps) != max_episode_steps \
+            or not 1 <= int(max_episode_steps) <= _lib.GOAL_MAX_STEPS:
+        raise ValueError("add_goal_steps: max_episode_steps must be an integer in [1, %d], got %r"
+                         % (_lib.GOAL_MAX_STEPS, max_episode_steps))
+    if isinstance(seed, bool) or int(seed) != seed or int(seed) < 0:
+        raise ValueError("add_goal_steps: seed must be a non-negative integer, got %r" % (seed,))
+    return ratio, thr, her_action, int(max_episode_steps), int(seed)
+
+
+class GoalStepsMirror(object):
+    """add_goal_steps' pending episodes on the host: the fixed parameters, each environment's fill (steps of its current
+    episode), the length of the episode it ended at the last call (0: none), the generator of the relabelling draws and
+    the device state (window bytes, the pinned slot the end flags of a call with CUDA flags are copied back into, and
+    that copy's event).  An ended episode is emitted at the next call, so the rows of a call, and the draws that make
+    them, are known before it without a device read."""
+
+    def __init__(self, E, So, G, A, her_ratio, threshold, her_action, max_episode_steps, seed):
+        self.E, self.So, self.G, self.A = int(E), int(So), int(G), int(A)
+        self.her_ratio, self.threshold, self.her_action = float(her_ratio), float(threshold), her_action
+        self.M, self.seed = int(max_episode_steps), int(seed)
+        self.key = (self.E, self.So, self.G, self.A, self.her_ratio, self.threshold, self.her_action, self.M, self.seed)
+        self.fill = np.zeros(self.E, dtype=np.int64)
+        self.ended = np.zeros(self.E, dtype=np.int64)
+        self.rng = np.random.default_rng(self.seed)
+        self.window = self.ends = self.event = None
+        self.pending = False
+
+    def check_step(self):
+        """ValueError if this call's step would take an episode past max_episode_steps."""
+        over = np.flatnonzero(self.fill >= self.M)
+        if over.size:
+            raise ValueError("add_goal_steps: the episode of environment %d already has max_episode_steps = %d steps and "
+                             "did not end" % (int(over[0]), self.M))
+
+    def draw(self):
+        """The relabelling draws of the episodes that ended at the last call -> (plan i32 or None, n_draws, n_rows).
+        Ended episodes in ascending e; one rng.random(sum L) gives select = u < her_ratio, then one rng.integers(t, L)
+        over the selected (e, t) in that order gives their future steps.  plan = {step_off [E], future [n_draws] (-1: no
+        copy), dst [n_draws] (rank of the original row in this call)}, the layout of d4pg_replay_add_goal_steps."""
+        em = np.flatnonzero(self.ended)
+        if em.size == 0:
+            return None, 0, 0
+        L = self.ended[em]
+        n = int(L.sum())
+        starts = np.cumsum(L) - L
+        sel = self.rng.random(n) < self.her_ratio
+        future = np.full(n, -1, dtype=np.int64)
+        if sel.any():
+            t = np.arange(n, dtype=np.int64) - np.repeat(starts, L)
+            future[sel] = self.rng.integers(t[sel], np.repeat(L, L)[sel])
+        counts = 1 + sel.astype(np.int64)
+        dst = np.cumsum(counts) - counts
+        step_off = np.zeros(self.E, dtype=np.int64)
+        step_off[em] = starts
+        return np.concatenate([step_off, future, dst]).astype(np.int32), n, int(counts.sum())
+
+    def advance(self, step=True):
+        """The ended episodes were emitted; with `step`, every environment took one step."""
+        self.ended[:] = 0
+        if step:
+            self.fill += 1
+
+    def end(self, ended):
+        """The episodes of the environments in `ended` (bool [E]) ended at this call: emitted at the next."""
+        ended = np.asarray(ended, dtype=bool)
+        self.ended[ended] = self.fill[ended]
+        self.fill[ended] = 0
+
+
 class _DeviceReplay(object):
     """Device storage + trees + the C handle.  Allocated lazily on the first add (the
     reference constructors do not know obs/act dims)."""
@@ -98,6 +183,7 @@ class _DeviceReplay(object):
         self._len = 0
         self._next_idx = 0
         self._steps = None               # add_steps: the device windows and the host mirror of their fills
+        self._goals = None               # add_goal_steps: the device episode windows and their GoalStepsMirror
         # host pipeline (a learner's ingest stream, ddpg.py): add_batch_host is issued there; every other device
         # operation runs on the caller's stream -- the two are kept in program order by events, only when they interleave
         self._ingest_stream = None
@@ -384,6 +470,8 @@ class _DeviceReplay(object):
             raise ValueError("add_steps: shapes must be obs / obs_next [E, obs_dim], action [E, act_dim], reward / "
                              "terminated / truncated [E]; got %s %s %s %s %s %s" % (so, sa, shape(reward), shape(obs_next),
                                                                                  shape(terminated), shape(truncated)))
+        if self._goals is not None:
+            raise ValueError("add_steps: add_goal_steps has pending episodes (drop_goal_steps() discards them)")
         if self.obs_dim is not None and (S, A) != (self.obs_dim, self.act_dim):
             raise ValueError("add_steps: rows of (%d, %d) into a buffer of (%d, %d)" % (S, A, self.obs_dim, self.act_dim))
         if E > self.size:
@@ -459,6 +547,130 @@ class _DeviceReplay(object):
         """Discard the pending n-step windows (and pending episode tails); the next add_steps may use another E, n_steps
         or gamma."""
         self._steps = None
+
+    # -- streaming hindsight relabelling (DESIGN.md §3 "Streaming hindsight relabelling") ------------------------------
+    def _check_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated,
+                          params):
+        """Shapes, parameters and the fixed key of the pending episodes, before any device work -> (E, So, G, A)."""
+        params = check_her_params(*params)
+        shape = lambda x: tuple(x.shape) if hasattr(x, "shape") else np.shape(x)
+        so, sg, sa = shape(obs), shape(desired_goal), shape(action)
+        if len(so) != 2 or len(sg) != 2 or len(sa) != 2 or so[0] < 1:
+            raise ValueError("add_goal_steps: obs, desired_goal and action must be [E, obs_dim] / [E, goal_dim] / "
+                             "[E, act_dim], got %s / %s / %s" % (so, sg, sa))
+        E, So, G, A = so[0], so[1], sg[1], sa[1]
+        if sg[0] != E or sa[0] != E or shape(obs_next) != (E, So) or shape(achieved_goal_next) != (E, G) \
+                or shape(reward) != (E,) or shape(terminated) != (E,) or (truncated is not None and shape(truncated) != (E,)):
+            raise ValueError("add_goal_steps: shapes must be obs / obs_next [E, obs_dim], desired_goal / "
+                             "achieved_goal_next [E, goal_dim], action [E, act_dim], reward / terminated / truncated [E]; "
+                             "got %s %s %s %s %s %s %s %s" % (so, sg, sa, shape(reward), shape(obs_next),
+                                                              shape(achieved_goal_next), shape(terminated), shape(truncated)))
+        if self._steps is not None:
+            raise ValueError("add_goal_steps: add_steps has pending windows (drop_steps() discards them)")
+        if self.obs_dim is not None and (So + G, A) != (self.obs_dim, self.act_dim):
+            raise ValueError("add_goal_steps: rows of (%d + %d, %d) into a buffer of (%d, %d)"
+                             % (So, G, A, self.obs_dim, self.act_dim))
+        w = self._goals
+        key = (E, So, G, A) + params
+        if w is None and E * 2 * params[3] > self.size:
+            raise ValueError("add_goal_steps: one call can insert E * 2 * max_episode_steps = %d rows, more than the "
+                             "buffer size %d" % (E * 2 * params[3], self.size))
+        if w is not None and w.key != key:
+            names = ("E", "obs_dim", "goal_dim", "act_dim", "her_ratio", "threshold", "her_action", "max_episode_steps",
+                     "seed")
+            diff = ", ".join("%s %r -> %r" % (k, x, y) for k, x, y in zip(names, w.key, key) if x != y)
+            raise ValueError("add_goal_steps: the pending episodes were started with other parameters (%s); "
+                             "drop_goal_steps() discards them" % diff)
+        return key
+
+    def _goal_resolve(self, w):
+        """Apply the end flags of the previous call when they were CUDA tensors (copied back asynchronously)."""
+        if w.pending:
+            w.event.synchronize()
+            e = w.ends.numpy()
+            w.end((e[0] | e[1]) != 0)
+            w.pending = False
+
+    def _goal_launch(self, w, inputs, plan, n_draws, n_rows, no_step):
+        plan_dev = None
+        if plan is not None:                      # the draws and row offsets: one host-to-device copy
+            plan_dev = torch.from_numpy(plan).pin_memory().to(self.device, non_blocking=True)
+        _lib.check(_lib.lib().d4pg_replay_add_goal_steps(
+            self.handle, w.E, w.So, w.G, *[_lib.ptr(t) for t in inputs], w.M, _lib.ptr(w.window), _lib.ptr(plan_dev),
+            n_draws, n_rows, w.threshold, 0 if w.her_action == "reference" else 1, 1 if no_step else 0,
+            1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add_goal_steps")
+        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
+        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+
+    def add_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated=None,
+                       her_ratio=0.8, threshold=0.05, her_action="reference", max_episode_steps=50, seed=0):
+        """One vector step of E goal-conditioned environments into per-environment episode windows on the device;
+        episodes that ended at the previous call are relabelled and inserted first, in one launch.  Returns the number
+        of rows inserted, known on the host without a device read.  See ReplayBuffer.add_goal_steps."""
+        key = self._check_goal_steps(obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated,
+                                     truncated, (her_ratio, threshold, her_action, max_episode_steps, seed))
+        E, So, G, A = key[:4]
+        w = self._goals
+        if w is not None:                         # the fills are exact once the previous call's flags are in
+            self._goal_resolve(w)
+            w.check_step()
+        if self.handle is None:
+            self._allocate(So + G, A)
+        self.flush()
+        dev = self.device
+        if w is None:
+            w = self._goals = GoalStepsMirror(*key)
+        if w.window is None:
+            nbytes = int(_lib.lib().d4pg_replay_goal_window_bytes(E, So, G, A, w.M))
+            w.window = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+            w.ends = torch.zeros(2, E, dtype=torch.uint8, pin_memory=True)
+            w.event = torch.cuda.Event()
+        plan, n_draws, n_rows = w.draw()
+
+        def dev_flags(x):
+            x = torch.as_tensor(x, device=dev).reshape(E)
+            return (x if x.dtype == torch.bool else x != 0).contiguous().view(torch.uint8)
+        on_dev = (torch.is_tensor(terminated) and terminated.is_cuda) or (torch.is_tensor(truncated) and truncated.is_cuda)
+        term = dev_flags(terminated)
+        trunc = dev_flags(truncated) if truncated is not None else None
+        f32 = lambda x: torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
+        f64 = lambda x: torch.as_tensor(x, dtype=torch.float64).to(dev).contiguous()       # widened exactly
+        inputs = [f32(obs), f64(desired_goal), f32(action), f64(reward).reshape(E), f32(obs_next),
+                  f64(achieved_goal_next), term, trunc]
+        self._goal_launch(w, inputs, plan, n_draws, n_rows, False)
+        w.advance(True)
+        if on_dev:                                # the episode ends are applied at the next call
+            w.ends[0].copy_(term, non_blocking=True)
+            if trunc is not None:
+                w.ends[1].copy_(trunc, non_blocking=True)
+            else:
+                w.ends[1].zero_()                 # host memory: no copy into it is in flight (waited for above)
+            w.event.record()
+            w.pending = True
+        else:
+            ended = np.asarray(terminated).reshape(E).astype(bool)
+            if truncated is not None:
+                ended = ended | np.asarray(truncated).reshape(E).astype(bool)
+            w.end(ended)
+        return n_rows
+
+    def flush_goal_steps(self):
+        """Insert the episodes that have ended without taking a step; running episodes stay pending.  Returns the
+        number of rows inserted."""
+        w = self._goals
+        if w is None:
+            return 0
+        self.flush()
+        self._goal_resolve(w)
+        plan, n_draws, n_rows = w.draw()
+        if n_rows:
+            self._goal_launch(w, [None] * 8, plan, n_draws, n_rows, True)
+        w.advance(False)
+        return n_rows
+
+    def drop_goal_steps(self):
+        """Discard the pending episodes of add_goal_steps; the next call may use other shapes or parameters."""
+        self._goals = None
 
     def _add_device(self, n, tensors):
         _lib.check(_lib.lib().d4pg_replay_add(self.handle, n, *[_lib.ptr(t) for t in tensors],
@@ -708,6 +920,43 @@ class ReplayBuffer(object):
     def drop_steps(self):
         """Discard the pending n-step windows of add_steps."""
         self._store.drop_steps()
+
+    def add_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated=None,
+                       her_ratio=0.8, threshold=0.05, her_action="reference", max_episode_steps=50, seed=0):
+        """One vector step of E goal-conditioned environments, with hindsight relabelling on the device (DESIGN.md §3
+        "Streaming hindsight relabelling").  obs / obs_next [E, So], desired_goal / achieved_goal_next [E, G] (the goal
+        achieved after the step), action [E, A], reward [E], terminated / truncated bool [E] (truncated=None: no
+        truncation); numpy, CPU or CUDA tensors.  The buffer's obs_dim is So + G.  Returns the number of rows inserted.
+
+        Environment e appends the step to its current episode, which ends on terminated or truncated.  An episode of L
+        steps that ends at one call is inserted at the next (or by flush_goal_steps()), before that call's step: for
+        every t the row (obs_t || goal_t, a_t, r_t, obs_next_t || goal_t, terminated_t), and, with probability
+        her_ratio, directly after it the copy whose goal is the achieved goal after a uniformly drawn future step
+        f in [t, L), with reward -(||achieved_t - goal'|| > threshold) and done = (reward == 0) -- main.py:154-184, the
+        rows add_her_episode stores.  The copy's action is the episode's last action (her_action="reference", as
+        main.py:184 stores it) or a_t ("own").  Unlike main.py, an episode that ends in success is stored too.  Rows go
+        in ascending e, then t; goals and rewards are stored widened to f64 exactly.
+
+        The draws come from numpy.random.default_rng(seed), per call over the ended episodes in ascending e: one
+        random(sum L) for the selection, then one integers(t, L) over the selected steps.  A vectorized stream cannot
+        keep the interleaved np.random order of main.py; add_her_episode keeps it for one episode.
+
+        The first call fixes E, the dims, her_ratio, threshold, her_action, max_episode_steps and seed; a call that
+        changes one raises ValueError until drop_goal_steps().  So do an episode longer than max_episode_steps,
+        E * 2 * max_episode_steps > size, and add_steps while these episodes are pending (or the reverse).  CUDA
+        terminated / truncated are read back asynchronously and waited for at the next call.  The pending episodes
+        are not part of any checkpoint."""
+        return self._store.add_goal_steps(obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated,
+                                          truncated, her_ratio, threshold, her_action, max_episode_steps, seed)
+
+    def flush_goal_steps(self):
+        """Insert the episodes of add_goal_steps that have ended, without taking a step (e.g. before training on them).
+        Returns the number of rows inserted."""
+        return self._store.flush_goal_steps()
+
+    def drop_goal_steps(self):
+        """Discard the pending episodes of add_goal_steps."""
+        self._store.drop_goal_steps()
 
     def _encode_sample(self, idxes):
         return _to_host_batch(self._store.gather(idxes))

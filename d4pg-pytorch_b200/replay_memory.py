@@ -66,6 +66,22 @@ class Replay(object):
         """Discard the pending n-step windows of add_steps."""
         self._store.drop_steps()
 
+    def add_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated=None,
+                       her_ratio=0.8, threshold=0.05, her_action="reference", max_episode_steps=50, seed=0):
+        """One vector step of E goal-conditioned environments with hindsight relabelling on the device
+        (ReplayBuffer.add_goal_steps has the semantics).  One-step rows: this Replay's n_steps is not applied.  Returns
+        the number of rows inserted."""
+        return self._store.add_goal_steps(obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated,
+                                          truncated, her_ratio, threshold, her_action, max_episode_steps, seed)
+
+    def flush_goal_steps(self):
+        """Insert the episodes of add_goal_steps that have ended, without taking a step."""
+        return self._store.flush_goal_steps()
+
+    def drop_goal_steps(self):
+        """Discard the pending episodes of add_goal_steps."""
+        self._store.drop_goal_steps()
+
     def initialize(self, init_length):
         """Random-policy filler with n-step return accumulation at insert time (replay_memory.py:21-59).  Needs a
         gym-style `env`.  The rollout is host glue; every finished (or cut-off) episode goes to the device in one

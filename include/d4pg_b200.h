@@ -262,6 +262,41 @@ int32_t d4pg_her_relabel(int32_t T, int32_t obs_dim, int32_t goal_dim, int32_t a
                          float* out_s, float* out_a, double* out_r, float* out_s2, uint8_t* out_d,
                          d4pg_stream_t stream);
 
+/* Streaming hindsight relabelling (DESIGN.md §3 "Streaming hindsight relabelling"): one vector step of E
+ * goal-conditioned environments per call, each environment's current episode kept in a window on the device.
+ *   obs, obs2 f32 [E, obs_dim]   goal, ag2 f64 [E, goal_dim]   act f32 [E, act_dim]   rew f64 [E]
+ *   terminated u8 [E]   episode_end u8 [E] or NULL
+ * ag2 is the achieved goal after the step.  The replay's obs_dim must be obs_dim + goal_dim; its act_dim is used.
+ * Environment e appends (obs, goal, act, rew, obs2, ag2, terminated) as step t of its episode; the episode ends on
+ * terminated_e != 0 or episode_end_e != 0.  An episode of L steps that ended at call k is emitted at call k+1 (or by a
+ * call with no_step = 1), before that call's step is appended: for every t the original row
+ * (obs_t || goal_t, act_t, rew_t, obs2_t || goal_t, terminated_t), directly followed, where the plan selects it, by the
+ * copy with goal' = ag2_f (f = future[t], t <= f < L), reward -(||ag2_t - goal'||_2 > threshold) in f64 (the
+ * arithmetic of d4pg_her_relabel) and done = (reward == 0); its action is act_{L-1} (her_action_mode 0, main.py:184)
+ * or act_t (1).  Rows go in ascending e, then t, and take ring rows next_idx, next_idx + 1, ...; the leaves, the
+ * normalizer's fold and len / next_idx follow as for d4pg_replay_add of those rows; their horizons are cleared.
+ *   window: caller-owned device memory of d4pg_replay_goal_window_bytes(E, obs_dim, goal_dim, act_dim,
+ *           max_episode_steps) bytes (-1 on bad arguments), zero-filled before the first call; zero-filling it again
+ *           discards the pending episodes.  E, the dims and max_episode_steps stay the same between zero-fills, and
+ *           no episode may grow past max_episode_steps steps (the caller counts them).
+ *   plan:   the host's draws, i32, NULL when n_draws = 0: step_off [E] (first draw of e's emitted episode, draws in
+ *           ascending e then t), future [n_draws] (-1 = no copy), dst [n_draws] (rank in this call of the original row
+ *           of each step; a copy takes the next rank).  n_draws = the summed length of the emitted episodes.
+ *   n_rows: n_draws + the selected steps; the kernel writes no ring row outside [next_idx, next_idx + n_rows).
+ *   no_step: 1 = emit the ended episodes only (the step inputs may be NULL); running episodes keep their windows.
+ * One kernel per call, plus the d4pg_replay_add tail when n_rows > 0.  Stream-ordered, no allocation.  A call with
+ * n_rows = 0 leaves the replay's generation unchanged.  D4PG_EINVAL: null pointers, E outside (0, size], a dim
+ * mismatch, max_episode_steps outside [1, D4PG_GOAL_MAX_STEPS], a threshold that is negative or not finite, n_draws
+ * outside [0, E * max_episode_steps], n_rows outside [0, min(2 * n_draws, size)]. */
+#define D4PG_GOAL_MAX_STEPS 65536
+int64_t d4pg_replay_goal_window_bytes(int64_t E, int32_t obs_dim, int32_t goal_dim, int32_t act_dim, int32_t max_episode_steps);
+int32_t d4pg_replay_add_goal_steps(d4pg_replay_t* h, int64_t E, int32_t obs_dim, int32_t goal_dim,
+                                   const float* obs, const double* goal, const float* act, const double* rew,
+                                   const float* obs2, const double* ag2, const uint8_t* terminated,
+                                   const uint8_t* episode_end, int32_t max_episode_steps, void* window,
+                                   const int32_t* plan, int64_t n_draws, int64_t n_rows, double threshold,
+                                   int32_t her_action_mode, int32_t no_step, int32_t prioritized, d4pg_stream_t stream);
+
 /* Running per-feature observation normalizer (mean / variance over every stored row, with clipping).
  *   stats  f64 [1 + 2*obs_dim] = {n, mean[S], M2[S]}      affine f32 [2*obs_dim] = {shift[S], scale[S]}
  * Update: every row an insert stores contributes its s once, in insertion order (rows later overwritten by the ring
