@@ -344,26 +344,13 @@ int learner_sample(d4pg_replay* h, int B, int prioritized, const double* uniform
   return launch_sample(h, sa, st, dependent);
 }
 
-void learner_sample_args(d4pg_replay* h, int B, int prioritized, const double* uniforms, const int32_t* positions,
-                         uint64_t seed, LearnerClock* clock, const ClockParams& cp,
-                         int32_t* idx, float* weights, float* s, float* a, double* r, float* s2, uint8_t* d,
-                         int ld_obs, int ld_act, SampleArgs& sa) {
-  sa = SampleArgs{};
-  sa.ld_obs = ld_obs; sa.ld_act = ld_act; sa.pipe_slot = -1;
-  sa.uniforms = uniforms; sa.seed = seed; sa.counter = 0; sa.clock = clock; sa.clock_params = cp;
-  sa.beta = 1.f; sa.B = B; sa.idx = idx; sa.weights = prioritized ? weights : nullptr;
-  sa.s = s; sa.a = a; sa.r = r; sa.s2 = s2; sa.d = d;
-  if (!prioritized) { sa.idx_in = positions; sa.uniform_mode = positions ? 0 : 1; }
-  sa.sum = h->sum; sa.mn = h->mn; sa.cap = h->cap; sa.state = reinterpret_cast<const ReplayState*>(h->state);
-  sa.obs = h->obs; sa.act = h->act; sa.rew = h->rew; sa.obs2 = h->obs2; sa.done = h->done;
-  sa.obs_dim = h->obs_dim; sa.act_dim = h->act_dim;
-}
-void tree_update_args(d4pg_replay* h, int B, const int32_t* idx, const float* prio, TreeArgs& a) {
-  a = TreeArgs{};
+// The tree kernels' view of the store, writing the n leaves idx with the values v0 (priorities, or a set's sums)
+static TreeArgs tree_args(const d4pg_replay* h, int n, const int32_t* idx, const float* v0) {
+  TreeArgs a{};
   a.sum = h->sum; a.mn = h->mn; a.cap = h->cap; a.log2cap = h->log2cap; a.size = h->size;
-  a.n = B; a.idx = idx; a.v0 = prio; a.alpha_f32 = h->alpha_f32; a.scratch = h->scratch;
+  a.n = n; a.idx = idx; a.v0 = v0; a.alpha_f32 = h->alpha_f32; a.scratch = h->scratch;
   a.state = reinterpret_cast<ReplayState*>(h->state);
-  h->pristine = 0;
+  return a;
 }
 
 int64_t replay_generation(const d4pg_replay* h) { return h->gen; }
@@ -372,9 +359,7 @@ const uint8_t* replay_horizons(const d4pg_replay* h) { return h->horizon; }
 
 int launch_gate_signal(unsigned long long* flag, cudaStream_t st);
 int launch_tree_update(d4pg_replay* h, int B, const int32_t* idx, const float* prio, cudaStream_t st, unsigned long long* gate) {
-  TreeArgs a{};
-  a.sum = h->sum; a.mn = h->mn; a.cap = h->cap; a.log2cap = h->log2cap; a.size = h->size;
-  a.n = B; a.idx = idx; a.v0 = prio; a.alpha_f32 = h->alpha_f32; a.scratch = h->scratch; a.state = reinterpret_cast<ReplayState*>(h->state);
+  TreeArgs a = tree_args(h, B, idx, prio);
   a.trace = (st_is_side(st) && debug_trace_buffer()) ? debug_trace_buffer() + STEP_TRACE_BASE : nullptr;
   if (B <= TREE_FAST_MAX && h->log2cap < TREE_FAST_LEVELS) {
     int hs = 64;
@@ -447,14 +432,17 @@ extern "C" int32_t d4pg_replay_destroy(d4pg_replay_t* h) {
 }
 
 namespace {
+// the staging and window layouts start every array that needs it on a 16-byte boundary
+int64_t up16(int64_t b) { return (b + 15) & ~int64_t(15); }
+
 struct PackLayout { int64_t obs, obs2, act, rew, done, total; };
 PackLayout pack_layout(const d4pg_replay* h, int64_t n) {
   PackLayout p;
   const int64_t S = int64_t(h->obs_dim) * 4, A = int64_t(h->act_dim) * 4;
   p.obs = 0; p.obs2 = p.obs + n * S; p.act = p.obs2 + n * S;
-  p.rew = (p.act + n * A + 15) & ~int64_t(15);
+  p.rew = up16(p.act + n * A);
   p.done = p.rew + n * 8;
-  p.total = (p.done + n + 15) & ~int64_t(15);
+  p.total = up16(p.done + n);
   return p;
 }
 }  // namespace
@@ -858,11 +846,20 @@ extern "C" int32_t d4pg_replay_obs_norm_refresh(d4pg_replay_t* h, d4pg_stream_t 
 }
 
 namespace {
-// What every insert runs after its ring write of n rows at [start, start + n) (mod size): the normalizer's fold over
-// the same rows in insertion order (rows1 [n1, obs_dim], then rows2 [n - n1, obs_dim]), then, prioritized, the ingest
-// gate and the tree add of the new leaves; last, the host mirror of len / next_idx.
-int replay_insert_tail(d4pg_replay* h, int64_t n, int64_t start, int64_t new_len, int64_t new_next,
-                       const float* rows1, int64_t n1, const float* rows2, int32_t prioritized, cudaStream_t st) {
+// The ring slots of an insert of n rows, [start, start + n) (mod size) from next_idx, and len / next_idx after it; an
+// insert of no row leaves len as it is
+struct RingRange { int64_t start, new_len, new_next; };
+RingRange ring_range(const d4pg_replay* h, int64_t n) {
+  const int64_t start = h->next_idx;
+  return {start, n ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n)) : h->len, (start + n) % h->size};
+}
+
+// What every insert runs after its ring write of n rows at r: the normalizer's fold over the same rows in insertion
+// order (rows1 [n1, obs_dim], then rows2 [n - n1, obs_dim]), then, prioritized, the ingest gate and the tree add of the
+// new leaves; last, the host mirror of len / next_idx.
+int replay_insert_tail(d4pg_replay* h, int64_t n, const RingRange& r, const float* rows1, int64_t n1, const float* rows2,
+                       int32_t prioritized, cudaStream_t st) {
+  const int64_t start = r.start;
   if (h->norm_stats) {
     // the normalizer's statistics: the same rows, in the same order.  Before the ingest gate and the tree kernels, so
     // the host pipeline's tree add stays the kernel the presample is programmatically dependent on
@@ -914,21 +911,28 @@ int replay_insert_tail(d4pg_replay* h, int64_t n, int64_t start, int64_t new_len
       }
     }
   }
-  h->len = new_len;
-  h->next_idx = new_next;
+  h->len = r.new_len;
+  h->next_idx = r.new_next;
   return D4PG_OK;
+}
+
+// The insert tail of a kernel that wrote its n rows straight into the ring: the rows are read back from the ring in
+// insertion order, [start, size) then [0, ...).  A call that inserted no row has no tail.
+int ring_rows_insert_tail(d4pg_replay* h, int64_t n, const RingRange& r, int32_t prioritized, cudaStream_t st) {
+  if (n == 0) return D4PG_OK;
+  const int64_t n1 = std::min<int64_t>(n, h->size - r.start);
+  return replay_insert_tail(h, n, r, h->obs + r.start * h->obs_dim, n1, h->obs, prioritized, st);
 }
 
 struct StepsLayout { int64_t rec, wr, ws, wa, wo, total; };
 StepsLayout steps_layout(int64_t E, int64_t S, int64_t A, int64_t n, bool tails) {
-  auto up = [](int64_t b) { return (b + 15) & ~int64_t(15); };
   StepsLayout l;
   l.rec = 0;
-  l.wr = up(l.rec + E * 8);
-  l.ws = up(l.wr + E * 2 * n * 8);
-  l.wa = up(l.ws + E * n * S * 4);
-  l.wo = up(l.wa + E * n * A * 4);
-  l.total = up(l.wo + (tails ? E * S * 4 : 0));
+  l.wr = up16(l.rec + E * 8);
+  l.ws = up16(l.wr + E * 2 * n * 8);
+  l.wa = up16(l.ws + E * n * S * 4);
+  l.wo = up16(l.wa + E * n * A * 4);
+  l.total = up16(l.wo + (tails ? E * S * 4 : 0));
   return l;
 }
 
@@ -950,16 +954,14 @@ extern "C" int32_t d4pg_replay_add(d4pg_replay_t* h, int64_t n, const float* obs
   D4PG_REQUIRE(h && obs && act && rew && obs2 && done, D4PG_EINVAL, "d4pg_replay_add: null argument");
   D4PG_REQUIRE(n > 0 && n <= h->size, D4PG_EINVAL, "d4pg_replay_add: need 0 < n <= size (n=%lld)", (long long)n);
   cudaStream_t st = as_stream(stream);
-  const int64_t start = h->next_idx;
-  const int64_t new_len = std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n));
-  const int64_t new_next = (start + n) % h->size;
+  const RingRange r = ring_range(h, n);
   const int blocks = int(std::min<int64_t>(4 * device_sm_count(), (n * h->obs_dim + 255) / 256));   // grid-stride
-  if (int rc = zero_horizons(h, start, n, st)) return rc;
+  if (int rc = zero_horizons(h, r.start, n, st)) return rc;
   ring_write_kernel<<<blocks, 256, 0, st>>>(h->obs, h->act, h->rew, h->obs2, h->done, obs, act, rew, obs2, done,
-                                             n, h->obs_dim, h->act_dim, h->size, start,
-                                             reinterpret_cast<ReplayState*>(h->state), new_len, new_next, step_trace());
+                                             n, h->obs_dim, h->act_dim, h->size, r.start,
+                                             reinterpret_cast<ReplayState*>(h->state), r.new_len, r.new_next, step_trace());
   D4PG_LAUNCH_OK();
-  return replay_insert_tail(h, n, start, new_len, new_next, obs, n, nullptr, prioritized, st);
+  return replay_insert_tail(h, n, r, obs, n, nullptr, prioritized, st);
 }
 
 extern "C" int64_t d4pg_replay_steps_window_bytes(int64_t E, int32_t obs_dim, int32_t act_dim, int32_t n_steps) {
@@ -1004,9 +1006,7 @@ extern "C" int32_t d4pg_replay_add_steps_ex(d4pg_replay_t* h, int64_t E, const f
                "d4pg_replay_add_steps: need 0 <= n_rows <= %s (%lld) and <= size (n_rows=%lld)",
                tails ? "E * max(1, n_steps - 1)" : "E", (long long)max_rows, (long long)n_rows);
   cudaStream_t st = as_stream(stream);
-  const int64_t start = h->next_idx;
-  const int64_t new_len = n_rows ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n_rows)) : h->len;
-  const int64_t new_next = (start + n_rows) % h->size;
+  const RingRange r = ring_range(h, n_rows);
   const StepsLayout l = steps_layout(E, h->obs_dim, h->act_dim, n_steps, tails != 0);
   uint8_t* wb = static_cast<uint8_t*>(window);
   StepsArgs a{};
@@ -1016,21 +1016,18 @@ extern "C" int32_t d4pg_replay_add_steps_ex(d4pg_replay_t* h, int64_t E, const f
   a.ws = reinterpret_cast<float*>(wb + l.ws); a.wa = reinterpret_cast<float*>(wb + l.wa);
   a.r_obs = h->obs; a.r_act = h->act; a.r_rew = h->rew; a.r_obs2 = h->obs2; a.r_done = h->done;
   if (tails) { a.wo = reinterpret_cast<float*>(wb + l.wo); a.r_hz = h->horizon; }
-  a.size = h->size; a.start = start; a.n_rows = n_rows; a.new_len = new_len; a.new_next = new_next;
+  a.size = h->size; a.start = r.start; a.n_rows = n_rows; a.new_len = r.new_len; a.new_next = r.new_next;
   a.state = reinterpret_cast<ReplayState*>(h->state);
   // a CTA takes a contiguous chunk of environments, one warp per environment; the grid is at most 4 CTAs per SM
   const int64_t blocks = std::min<int64_t>((E + STEPS_WARPS - 1) / STEPS_WARPS, 4 * device_sm_count());
   a.chunk = (E + blocks - 1) / blocks;
   if (tails) replay_add_steps_kernel<true><<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
   else {
-    if (int rc = zero_horizons(h, start, n_rows, st)) return rc;
+    if (int rc = zero_horizons(h, r.start, n_rows, st)) return rc;
     replay_add_steps_kernel<false><<<unsigned((E + a.chunk - 1) / a.chunk), STEPS_THREADS, 0, st>>>(a);
   }
   D4PG_LAUNCH_OK();
-  if (n_rows == 0) return D4PG_OK;
-  // the rows just written, read back from the ring in insertion order: [start, size) then [0, ...)
-  const int64_t n1 = std::min<int64_t>(n_rows, h->size - start);
-  return replay_insert_tail(h, n_rows, start, new_len, new_next, h->obs + start * h->obs_dim, n1, h->obs, prioritized, st);
+  return ring_rows_insert_tail(h, n_rows, r, prioritized, st);
 }
 
 // ---- device-side ingest: streaming hindsight relabelling (DESIGN.md §3 "Streaming hindsight relabelling") ----------
@@ -1126,17 +1123,16 @@ __global__ void __launch_bounds__(GOAL_THREADS) replay_add_goal_steps_kernel(con
 namespace {
 struct GoalLayout { int64_t rec, obs, obs2, act, goal, ag, rew, term, total; };
 GoalLayout goal_layout(int64_t E, int64_t So, int64_t G, int64_t A, int64_t M) {
-  auto up = [](int64_t b) { return (b + 15) & ~int64_t(15); };
   GoalLayout l;
   l.rec = 0;
-  l.obs = up(l.rec + E * 4);
-  l.obs2 = up(l.obs + E * M * So * 4);
-  l.act = up(l.obs2 + E * M * So * 4);
-  l.goal = up(l.act + E * M * A * 4);
-  l.ag = up(l.goal + E * M * G * 8);
-  l.rew = up(l.ag + E * M * G * 8);
-  l.term = up(l.rew + E * M * 8);
-  l.total = up(l.term + E * M);
+  l.obs = up16(l.rec + E * 4);
+  l.obs2 = up16(l.obs + E * M * So * 4);
+  l.act = up16(l.obs2 + E * M * So * 4);
+  l.goal = up16(l.act + E * M * A * 4);
+  l.ag = up16(l.goal + E * M * G * 8);
+  l.rew = up16(l.ag + E * M * G * 8);
+  l.term = up16(l.rew + E * M * 8);
+  l.total = up16(l.term + E * M);
   return l;
 }
 }  // namespace
@@ -1176,9 +1172,7 @@ extern "C" int32_t d4pg_replay_add_goal_steps(d4pg_replay_t* h, int64_t E, int32
   D4PG_REQUIRE(n_rows >= 0 && n_rows <= 2 * n_draws && n_rows <= h->size, D4PG_EINVAL,
                "d4pg_replay_add_goal_steps: need 0 <= n_rows <= 2 * n_draws and <= size (n_rows=%lld)", (long long)n_rows);
   cudaStream_t st = as_stream(stream);
-  const int64_t start = h->next_idx;
-  const int64_t new_len = n_rows ? std::min<int64_t>(h->size, std::max<int64_t>(h->len, start + n_rows)) : h->len;
-  const int64_t new_next = (start + n_rows) % h->size;
+  const RingRange r = ring_range(h, n_rows);
   const GoalLayout l = goal_layout(E, obs_dim, goal_dim, h->act_dim, M);
   uint8_t* wb = static_cast<uint8_t*>(window);
   GoalArgs a{};
@@ -1192,14 +1186,12 @@ extern "C" int32_t d4pg_replay_add_goal_steps(d4pg_replay_t* h, int64_t E, int32
   if (n_draws > 0) { a.step_off = plan; a.future = plan + E; a.dst = plan + E + n_draws; }
   a.n_draws = n_draws;
   a.r_obs = h->obs; a.r_act = h->act; a.r_rew = h->rew; a.r_obs2 = h->obs2; a.r_done = h->done;
-  a.size = h->size; a.start = start; a.n_rows = n_rows; a.new_len = new_len; a.new_next = new_next;
+  a.size = h->size; a.start = r.start; a.n_rows = n_rows; a.new_len = r.new_len; a.new_next = r.new_next;
   a.state = reinterpret_cast<ReplayState*>(h->state);
-  if (int rc = zero_horizons(h, start, n_rows, st)) return rc;
+  if (int rc = zero_horizons(h, r.start, n_rows, st)) return rc;
   replay_add_goal_steps_kernel<<<unsigned((E + GOAL_WARPS - 1) / GOAL_WARPS), GOAL_THREADS, 0, st>>>(a);
   D4PG_LAUNCH_OK();
-  if (n_rows == 0) return D4PG_OK;
-  const int64_t n1 = std::min<int64_t>(n_rows, h->size - start);
-  return replay_insert_tail(h, n_rows, start, new_len, new_next, h->obs + start * h->obs_dim, n1, h->obs, prioritized, st);
+  return ring_rows_insert_tail(h, n_rows, r, prioritized, st);
 }
 
 extern "C" int32_t d4pg_replay_sample(d4pg_replay_t* h, int32_t B, const double* uniforms,
@@ -1235,9 +1227,8 @@ extern "C" int32_t d4pg_replay_set_leaves(d4pg_replay_t* h, int32_t n, const int
                                           const float* min_vals, d4pg_stream_t stream) {
   if (h) ++h->gen;
   D4PG_REQUIRE(h && n > 0 && idx && sum_vals && min_vals, D4PG_EINVAL, "d4pg_replay_set_leaves: null/empty argument");
-  TreeArgs a{};
-  a.sum = h->sum; a.mn = h->mn; a.cap = h->cap; a.log2cap = h->log2cap; a.size = h->size;
-  a.n = n; a.idx = idx; a.v0 = sum_vals; a.v1 = min_vals; a.scratch = h->scratch; a.state = reinterpret_cast<ReplayState*>(h->state);
+  TreeArgs a = tree_args(h, n, idx, sum_vals);
+  a.v1 = min_vals;
   tree_write_kernel<TREE_SET><<<1, TREE_THREADS, 0, as_stream(stream)>>>(a);
   D4PG_LAUNCH_OK();
   return D4PG_OK;

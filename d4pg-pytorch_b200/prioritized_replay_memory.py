@@ -41,20 +41,75 @@ class LinearSchedule(object):
         return self.initial_p + fraction * (self.final_p - self.initial_p)
 
 
-class StepsMirror(object):
-    """add_steps' pending n-step windows: the fixed (E, n, gamma), the host mirror of each window's fill (steps of the
-    current episode, capped at n - 1, which is all the emit decision needs) and the device state (window bytes, the
-    pinned slot the end flags of a call with CUDA flags are copied back into, and that copy's event).  Environment e
-    emits a row at a call iff fill[e] == n - 1 before it, so the count is exact before the call without a device read.
-    With episode tails (`tails`), an episode that ended also leaves tails[e] = min(its length, n - 1) rows, which e
-    emits at its next call."""
+def dev_flags(x, E, device):
+    """terminated / truncated flags (numpy, CPU or CUDA) -> u8 [E] on `device`."""
+    x = torch.as_tensor(x, device=device).reshape(E)
+    return (x if x.dtype == torch.bool else x != 0).contiguous().view(torch.uint8)
+
+
+def _shape(x):
+    return tuple(x.shape) if hasattr(x, "shape") else np.shape(x)
+
+
+def _step_vectors_ok(E, reward, terminated, truncated):
+    """reward, terminated and (unless None) truncated of a vector step are [E]."""
+    return _shape(reward) == (E,) and _shape(terminated) == (E,) and (truncated is None or _shape(truncated) == (E,))
+
+
+class _StreamMirror(object):
+    """The device state of a streaming insert (add_steps, add_goal_steps) and its end-flag protocol.  The window bytes
+    live on the device; the episode ends of a call with CUDA flags are copied back into a pinned slot and applied, by
+    the subclass's end(), at the next call, so no call waits for its own flags."""
+
+    def __init__(self):
+        self.window = self.ends = self.event = None
+        self.pending = False
+
+    def ensure_window(self, nbytes, device):
+        """On first use: the zero-filled window of nbytes() bytes, the pinned end-flag slot and its event."""
+        if self.window is None:
+            self.window = torch.zeros(int(nbytes()), dtype=torch.uint8, device=device)
+            self.ends = torch.zeros(2, self.E, dtype=torch.uint8, pin_memory=True)
+            self.event = torch.cuda.Event()
+
+    def resolve(self):
+        """Apply the end flags of the previous call when they were CUDA tensors (copied back asynchronously)."""
+        if self.pending:
+            self.event.synchronize()
+            e = self.ends.numpy()
+            self.end((e[0] | e[1]) != 0)
+            self.pending = False
+
+    def record_ends(self, term, trunc, terminated, truncated):
+        """Close a call: its episode ends (term / trunc: the u8 device flags the launch read, terminated / truncated: the
+        caller's) are applied now when they are host flags, else copied back and applied at the next call."""
+        if (torch.is_tensor(terminated) and terminated.is_cuda) or (torch.is_tensor(truncated) and truncated.is_cuda):
+            self.ends[0].copy_(term, non_blocking=True)
+            if trunc is not None:
+                self.ends[1].copy_(trunc, non_blocking=True)
+            else:
+                self.ends[1].zero_()                 # host memory: no copy into it is in flight (resolved before)
+            self.event.record()
+            self.pending = True
+        else:
+            ended = np.asarray(terminated).reshape(self.E).astype(bool)
+            if truncated is not None:
+                ended = ended | np.asarray(truncated).reshape(self.E).astype(bool)
+            self.end(ended)
+
+
+class StepsMirror(_StreamMirror):
+    """add_steps' pending n-step windows: the fixed (E, n, gamma) and the host mirror of each window's fill (steps of
+    the current episode, capped at n - 1, which is all the emit decision needs).  Environment e emits a row at a call
+    iff fill[e] == n - 1 before it, so the count is exact before the call without a device read.  With episode tails
+    (`tails`), an episode that ended also leaves tails[e] = min(its length, n - 1) rows, which e emits at its next
+    call."""
 
     def __init__(self, E, n, gamma, tails=False):
+        super(StepsMirror, self).__init__()
         self.E, self.n, self.gamma = int(E), int(n), float(gamma)
         self.fill = np.zeros(self.E, dtype=np.int64)
         self.tails = np.zeros(self.E, dtype=np.int64) if tails else None
-        self.window = self.ends = self.event = None
-        self.pending = False
 
     def rows(self):
         """Rows the next call inserts."""
@@ -101,14 +156,14 @@ def check_her_params(her_ratio, threshold, her_action, max_episode_steps, seed):
     return ratio, thr, her_action, int(max_episode_steps), int(seed)
 
 
-class GoalStepsMirror(object):
+class GoalStepsMirror(_StreamMirror):
     """add_goal_steps' pending episodes on the host: the fixed parameters, each environment's fill (steps of its current
-    episode), the length of the episode it ended at the last call (0: none), the generator of the relabelling draws and
-    the device state (window bytes, the pinned slot the end flags of a call with CUDA flags are copied back into, and
-    that copy's event).  An ended episode is emitted at the next call, so the rows of a call, and the draws that make
-    them, are known before it without a device read."""
+    episode), the length of the episode it ended at the last call (0: none) and the generator of the relabelling draws.
+    An ended episode is emitted at the next call, so the rows of a call, and the draws that make them, are known before
+    it without a device read."""
 
     def __init__(self, E, So, G, A, her_ratio, threshold, her_action, max_episode_steps, seed):
+        super(GoalStepsMirror, self).__init__()
         self.E, self.So, self.G, self.A = int(E), int(So), int(G), int(A)
         self.her_ratio, self.threshold, self.her_action = float(her_ratio), float(threshold), her_action
         self.M, self.seed = int(max_episode_steps), int(seed)
@@ -116,8 +171,6 @@ class GoalStepsMirror(object):
         self.fill = np.zeros(self.E, dtype=np.int64)
         self.ended = np.zeros(self.E, dtype=np.int64)
         self.rng = np.random.default_rng(self.seed)
-        self.window = self.ends = self.event = None
-        self.pending = False
 
     def check_step(self):
         """ValueError if this call's step would take an episode past max_episode_steps."""
@@ -300,16 +353,6 @@ class _DeviceReplay(object):
         if self._n_staged == self.STAGE_ROWS or self._n_staged == self.size:
             self.flush()
 
-    def _pack_layout(self, n):
-        """Byte offsets of (obs, act, rew, obs2, done) for n rows packed into one staging buffer."""
-        S, A = self.obs_dim * 4, self.act_dim * 4
-        o_obs = 0
-        o_obs2 = o_obs + n * S
-        o_act = o_obs2 + n * S
-        o_rew = (o_act + n * A + 15) & ~15
-        o_done = o_rew + n * 8
-        return o_obs, o_act, o_rew, o_obs2, o_done, (o_done + n + 15) & ~15
-
     def add_batch_host(self, s, a, r, s2, done):
         """Fast ingest of n <= STAGE_ROWS host transitions through ONE library call
         (`d4pg_replay_add_host`): packed into a pinned staging buffer, one async H2D copy, ring +
@@ -323,82 +366,64 @@ class _DeviceReplay(object):
                 and done.is_contiguous()):
             # host tensors of the right types (e.g. slices of a pinned rollout buffer): no numpy round trip
             n = s.shape[0]
-            rc = _lib.lib().d4pg_replay_add_host(self.handle, n, s.data_ptr(), a.data_ptr(), r.data_ptr(), s2.data_ptr(),
-                                                 done.data_ptr(), 1 if self.prioritized else 0, self._ingest_ptr())
-            if rc:
-                _lib.check(rc, "d4pg_replay_add_host")
-            self._next_idx = (self._next_idx + n) % self.size
-            self._len = min(self.size, self._len + n)
-            return
-        s = np.ascontiguousarray(s, dtype=np.float32)
-        n = s.shape[0] if s.ndim == 2 else 1
-        a = np.ascontiguousarray(a, dtype=np.float32)
-        if self.handle is None:
-            self._allocate(s.reshape(n, -1).shape[1], a.reshape(n, -1).shape[1])
-        if n > self.STAGE_ROWS or n > self.size:
-            return self.add_batch(s, a, r, s2, done)
-        if self._n_staged:
-            self.flush()
-        L = _lib.lib()
-        if getattr(self, "_pack_host", None) is None:
-            nbytes = int(L.d4pg_replay_staging_bytes(self.handle, self.STAGE_ROWS))
-            self._pack_host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
-            self._pack_dev = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            _lib.check(L.d4pg_replay_set_staging(self.handle, _lib.ptr(self._pack_host), _lib.ptr(self._pack_dev), nbytes),
-                       "d4pg_replay_set_staging")
-        r = np.ascontiguousarray(r, dtype=np.float64)
-        s2 = np.ascontiguousarray(s2, dtype=np.float32)
-        d = np.ascontiguousarray(done)
-        if d.dtype != np.uint8:
-            d = d.astype(np.uint8)
-        rc = L.d4pg_replay_add_host(self.handle, n, s.ctypes.data, a.ctypes.data, r.ctypes.data, s2.ctypes.data,
-                                    d.ctypes.data, 1 if self.prioritized else 0, self._ingest_ptr())
+            ptrs = [t.data_ptr() for t in (s, a, r, s2, done)]
+        else:
+            s = np.ascontiguousarray(s, dtype=np.float32)
+            n = s.shape[0] if s.ndim == 2 else 1
+            a = np.ascontiguousarray(a, dtype=np.float32)
+            if self.handle is None:
+                self._allocate(s.reshape(n, -1).shape[1], a.reshape(n, -1).shape[1])
+            if n > self.STAGE_ROWS or n > self.size:
+                return self.add_batch(s, a, r, s2, done)
+            if self._n_staged:
+                self.flush()
+            if getattr(self, "_pack_host", None) is None:
+                L = _lib.lib()
+                nbytes = int(L.d4pg_replay_staging_bytes(self.handle, self.STAGE_ROWS))
+                self._pack_host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+                self._pack_dev = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+                _lib.check(L.d4pg_replay_set_staging(self.handle, _lib.ptr(self._pack_host), _lib.ptr(self._pack_dev),
+                                                     nbytes), "d4pg_replay_set_staging")
+            r = np.ascontiguousarray(r, dtype=np.float64)
+            s2 = np.ascontiguousarray(s2, dtype=np.float32)
+            done = np.ascontiguousarray(done)
+            if done.dtype != np.uint8:
+                done = done.astype(np.uint8)
+            ptrs = [x.ctypes.data for x in (s, a, r, s2, done)]
+        rc = _lib.lib().d4pg_replay_add_host(self.handle, n, *ptrs, 1 if self.prioritized else 0, self._ingest_ptr())
         if rc:
             _lib.check(rc, "d4pg_replay_add_host")
         self._next_idx = (self._next_idx + n) % self.size
         self._len = min(self.size, self._len + n)
 
-    def add_batch(self, s, a, r, s2, done):
-        """Vectorised ingest of n transitions (host numpy / CPU or CUDA tensors)."""
+    def _rows_to_device(self, s, a, r, s2, done, non_blocking):
+        """n rows (host numpy / CPU or CUDA tensors) -> (n, contiguous device tensors s, a, r f64, s2, done u8); the
+        copies from host memory are asynchronous with `non_blocking`."""
         self.flush()
         s = torch.as_tensor(s, dtype=torch.float32)
-        a = torch.as_tensor(a, dtype=torch.float32)
         if s.dim() == 1:
             s = s.view(1, -1)
         n = s.shape[0]
-        a = a.reshape(n, -1)
+        a = torch.as_tensor(a, dtype=torch.float32).reshape(n, -1)
         if self.handle is None:
             self._allocate(s.shape[1], a.shape[1])
-        dev = self.device
-        nb = not s.is_cuda
-        done_t = torch.as_tensor(done)
-        args = [s.to(dev, non_blocking=nb).contiguous(), a.to(dev, non_blocking=nb).contiguous(),
-                torch.as_tensor(r, dtype=torch.float64).reshape(n).to(dev, non_blocking=nb).contiguous(),
-                torch.as_tensor(s2, dtype=torch.float32).reshape(n, -1).to(dev, non_blocking=nb).contiguous(),
-                done_t.reshape(n).to(torch.uint8).to(dev, non_blocking=nb).contiguous()]
+        dev, nb = self.device, non_blocking and not s.is_cuda
+        return n, [s.to(dev, non_blocking=nb).contiguous(), a.to(dev, non_blocking=nb).contiguous(),
+                   torch.as_tensor(r, dtype=torch.float64).reshape(n).to(dev, non_blocking=nb).contiguous(),
+                   torch.as_tensor(s2, dtype=torch.float32).reshape(n, -1).to(dev, non_blocking=nb).contiguous(),
+                   torch.as_tensor(done).reshape(n).to(torch.uint8).to(dev, non_blocking=nb).contiguous()]
+
+    def add_batch(self, s, a, r, s2, done):
+        """Vectorised ingest of n transitions (host numpy / CPU or CUDA tensors)."""
+        n, args = self._rows_to_device(s, a, r, s2, done, non_blocking=True)
         for lo in range(0, n, self.size):
             hi = min(n, lo + self.size)
             self._add_device(hi - lo, [t[lo:hi] for t in args])
 
-    def _episode_to_device(self, s, a, r, s2, done):
-        self.flush()
-        s = torch.as_tensor(s, dtype=torch.float32)
-        if s.dim() == 1:
-            s = s.view(1, -1)
-        T = s.shape[0]
-        a = torch.as_tensor(a, dtype=torch.float32).reshape(T, -1)
-        if self.handle is None:
-            self._allocate(s.shape[1], a.shape[1])
-        dev = self.device
-        return T, [s.to(dev).contiguous(), a.to(dev).contiguous(),
-                   torch.as_tensor(r, dtype=torch.float64).reshape(T).to(dev).contiguous(),
-                   torch.as_tensor(s2, dtype=torch.float32).reshape(T, -1).to(dev).contiguous(),
-                   torch.as_tensor(done).reshape(T).to(torch.uint8).to(dev).contiguous()]
-
     def add_episode_nstep(self, s, a, r, s2, done, n_steps, gamma):
         """One episode of T consecutive steps with the n-step return accumulated ON THE DEVICE at insert
         (replay_memory.py:38-45): transition i = (s_i, a_i, sum_k gamma^k r_{i+k}, s'_{i+n-1}, done_{i+n-1})."""
-        T, args = self._episode_to_device(s, a, r, s2, done)
+        T, args = self._rows_to_device(s, a, r, s2, done, non_blocking=False)
         n_steps = int(n_steps)
         if T < n_steps:
             return 0
@@ -409,8 +434,7 @@ class _DeviceReplay(object):
         _lib.check(_lib.lib().d4pg_replay_add_nstep(self.handle, T, *[_lib.ptr(t) for t in args], n_steps, float(gamma),
                                                     _lib.ptr(scratch), 1 if self.prioritized else 0, _lib.stream_ptr()),
                    "d4pg_replay_add_nstep")
-        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
-        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+        self._sync_ring()
         return m
 
     def add_her_episode(self, obs, obs_next, goal, ag_next, act, rew, done, her_ratio=0.8, threshold=0.05,
@@ -460,16 +484,14 @@ class _DeviceReplay(object):
         """Shapes and the fixed (E, n_steps, gamma) of the pending windows, before any device work -> (E, S, A)."""
         if isinstance(n_steps, bool) or int(n_steps) != n_steps or not 1 <= int(n_steps) <= _lib.STEPS_MAX_N:
             raise ValueError("add_steps: n_steps must be an integer in [1, %d], got %r" % (_lib.STEPS_MAX_N, n_steps))
-        shape = lambda x: tuple(x.shape) if hasattr(x, "shape") else np.shape(x)
-        so, sa = shape(obs), shape(action)
+        so, sa = _shape(obs), _shape(action)
         if len(so) != 2 or len(sa) != 2 or so[0] < 1:
             raise ValueError("add_steps: obs and action must be [E, obs_dim] / [E, act_dim], got %s / %s" % (so, sa))
         E, S, A = so[0], so[1], sa[1]
-        if sa[0] != E or shape(obs_next) != (E, S) or shape(reward) != (E,) or shape(terminated) != (E,) \
-                or (truncated is not None and shape(truncated) != (E,)):
+        if sa[0] != E or _shape(obs_next) != (E, S) or not _step_vectors_ok(E, reward, terminated, truncated):
             raise ValueError("add_steps: shapes must be obs / obs_next [E, obs_dim], action [E, act_dim], reward / "
-                             "terminated / truncated [E]; got %s %s %s %s %s %s" % (so, sa, shape(reward), shape(obs_next),
-                                                                                 shape(terminated), shape(truncated)))
+                             "terminated / truncated [E]; got %s %s %s %s %s %s" % (so, sa, _shape(reward), _shape(obs_next),
+                                                                                 _shape(terminated), _shape(truncated)))
         if self._goals is not None:
             raise ValueError("add_steps: add_goal_steps has pending episodes (drop_goal_steps() discards them)")
         if self.obs_dim is not None and (S, A) != (self.obs_dim, self.act_dim):
@@ -491,56 +513,30 @@ class _DeviceReplay(object):
         that are full go straight into the ring in one launch.  Returns the number of rows inserted, known on the host
         without a device read (a mirror of the window fills).  See ReplayBuffer.add_steps."""
         E, S, A = self._check_steps(obs, action, reward, obs_next, terminated, truncated, n_steps, gamma)
-        n, gamma = int(n_steps), float(gamma)
+        n, gamma, tails = int(n_steps), float(gamma), 1 if self.nstep_tails else 0
+        w = self._steps
+        if w is not None:                         # the fills are exact once the previous call's flags are in
+            w.resolve()
         if self.handle is None:
             self._allocate(S, A)
         self.flush()
         dev = self.device
-        w = self._steps
         if w is None:
             w = self._steps = StepsMirror(E, n, gamma, self.nstep_tails)
-        if w.window is None:
-            nbytes = int(_lib.lib().d4pg_replay_steps_window_bytes_ex(E, S, A, n, 1 if self.nstep_tails else 0))
-            w.window = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-            w.ends = torch.zeros(2, E, dtype=torch.uint8, pin_memory=True)
-            w.event = torch.cuda.Event()
-        if w.pending:                             # the end flags of the previous call, copied back asynchronously
-            w.event.synchronize()
-            e = w.ends.numpy()
-            w.end((e[0] | e[1]) != 0)
-            w.pending = False
+        w.ensure_window(lambda: _lib.lib().d4pg_replay_steps_window_bytes_ex(E, S, A, n, tails), dev)
         n_rows = w.rows()
-
-        def dev_flags(x):
-            x = torch.as_tensor(x, device=dev).reshape(E)
-            return (x if x.dtype == torch.bool else x != 0).contiguous().view(torch.uint8)
-        on_dev = (torch.is_tensor(terminated) and terminated.is_cuda) or (torch.is_tensor(truncated) and truncated.is_cuda)
-        term = dev_flags(terminated)
-        trunc = dev_flags(truncated) if truncated is not None else None
+        term = dev_flags(terminated, E, dev)
+        trunc = dev_flags(truncated, E, dev) if truncated is not None else None
         args = [torch.as_tensor(obs, dtype=torch.float32).to(dev).contiguous(),
                 torch.as_tensor(action, dtype=torch.float32).to(dev).contiguous(),
                 torch.as_tensor(reward, dtype=torch.float64).to(dev).contiguous(),
                 torch.as_tensor(obs_next, dtype=torch.float32).to(dev).contiguous(), term, trunc]
         _lib.check(_lib.lib().d4pg_replay_add_steps_ex(self.handle, E, *[_lib.ptr(t) for t in args], n, gamma,
-                                                       _lib.ptr(w.window), n_rows, 1 if self.nstep_tails else 0,
-                                                       1 if self.prioritized else 0, _lib.stream_ptr()),
-                   "d4pg_replay_add_steps_ex")
+                                                       _lib.ptr(w.window), n_rows, tails, 1 if self.prioritized else 0,
+                                                       _lib.stream_ptr()), "d4pg_replay_add_steps_ex")
+        self._sync_ring()
         w.advance()
-        if on_dev:                                # the episode ends are applied at the next call
-            w.ends[0].copy_(term, non_blocking=True)
-            if trunc is not None:
-                w.ends[1].copy_(trunc, non_blocking=True)
-            else:
-                w.ends[1].zero_()                 # host memory: no copy into it is in flight (waited for above)
-            w.event.record()
-            w.pending = True
-        else:
-            ended = np.asarray(terminated).reshape(E).astype(bool)
-            if truncated is not None:
-                ended = ended | np.asarray(truncated).reshape(E).astype(bool)
-            w.end(ended)
-        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
-        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+        w.record_ends(term, trunc, terminated, truncated)
         return n_rows
 
     def drop_steps(self):
@@ -553,18 +549,18 @@ class _DeviceReplay(object):
                           params):
         """Shapes, parameters and the fixed key of the pending episodes, before any device work -> (E, So, G, A)."""
         params = check_her_params(*params)
-        shape = lambda x: tuple(x.shape) if hasattr(x, "shape") else np.shape(x)
-        so, sg, sa = shape(obs), shape(desired_goal), shape(action)
+        so, sg, sa = _shape(obs), _shape(desired_goal), _shape(action)
         if len(so) != 2 or len(sg) != 2 or len(sa) != 2 or so[0] < 1:
             raise ValueError("add_goal_steps: obs, desired_goal and action must be [E, obs_dim] / [E, goal_dim] / "
                              "[E, act_dim], got %s / %s / %s" % (so, sg, sa))
         E, So, G, A = so[0], so[1], sg[1], sa[1]
-        if sg[0] != E or sa[0] != E or shape(obs_next) != (E, So) or shape(achieved_goal_next) != (E, G) \
-                or shape(reward) != (E,) or shape(terminated) != (E,) or (truncated is not None and shape(truncated) != (E,)):
+        if sg[0] != E or sa[0] != E or _shape(obs_next) != (E, So) or _shape(achieved_goal_next) != (E, G) \
+                or not _step_vectors_ok(E, reward, terminated, truncated):
             raise ValueError("add_goal_steps: shapes must be obs / obs_next [E, obs_dim], desired_goal / "
                              "achieved_goal_next [E, goal_dim], action [E, act_dim], reward / terminated / truncated [E]; "
-                             "got %s %s %s %s %s %s %s %s" % (so, sg, sa, shape(reward), shape(obs_next),
-                                                              shape(achieved_goal_next), shape(terminated), shape(truncated)))
+                             "got %s %s %s %s %s %s %s %s" % (so, sg, sa, _shape(reward), _shape(obs_next),
+                                                              _shape(achieved_goal_next), _shape(terminated),
+                                                              _shape(truncated)))
         if self._steps is not None:
             raise ValueError("add_goal_steps: add_steps has pending windows (drop_steps() discards them)")
         if self.obs_dim is not None and (So + G, A) != (self.obs_dim, self.act_dim):
@@ -583,14 +579,6 @@ class _DeviceReplay(object):
                              "drop_goal_steps() discards them" % diff)
         return key
 
-    def _goal_resolve(self, w):
-        """Apply the end flags of the previous call when they were CUDA tensors (copied back asynchronously)."""
-        if w.pending:
-            w.event.synchronize()
-            e = w.ends.numpy()
-            w.end((e[0] | e[1]) != 0)
-            w.pending = False
-
     def _goal_launch(self, w, inputs, plan, n_draws, n_rows, no_step):
         plan_dev = None
         if plan is not None:                      # the draws and row offsets: one host-to-device copy
@@ -599,8 +587,7 @@ class _DeviceReplay(object):
             self.handle, w.E, w.So, w.G, *[_lib.ptr(t) for t in inputs], w.M, _lib.ptr(w.window), _lib.ptr(plan_dev),
             n_draws, n_rows, w.threshold, 0 if w.her_action == "reference" else 1, 1 if no_step else 0,
             1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add_goal_steps")
-        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
-        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+        self._sync_ring()
 
     def add_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated=None,
                        her_ratio=0.8, threshold=0.05, her_action="reference", max_episode_steps=50, seed=0):
@@ -612,7 +599,7 @@ class _DeviceReplay(object):
         E, So, G, A = key[:4]
         w = self._goals
         if w is not None:                         # the fills are exact once the previous call's flags are in
-            self._goal_resolve(w)
+            w.resolve()
             w.check_step()
         if self.handle is None:
             self._allocate(So + G, A)
@@ -620,38 +607,17 @@ class _DeviceReplay(object):
         dev = self.device
         if w is None:
             w = self._goals = GoalStepsMirror(*key)
-        if w.window is None:
-            nbytes = int(_lib.lib().d4pg_replay_goal_window_bytes(E, So, G, A, w.M))
-            w.window = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-            w.ends = torch.zeros(2, E, dtype=torch.uint8, pin_memory=True)
-            w.event = torch.cuda.Event()
+        w.ensure_window(lambda: _lib.lib().d4pg_replay_goal_window_bytes(E, So, G, A, w.M), dev)
         plan, n_draws, n_rows = w.draw()
-
-        def dev_flags(x):
-            x = torch.as_tensor(x, device=dev).reshape(E)
-            return (x if x.dtype == torch.bool else x != 0).contiguous().view(torch.uint8)
-        on_dev = (torch.is_tensor(terminated) and terminated.is_cuda) or (torch.is_tensor(truncated) and truncated.is_cuda)
-        term = dev_flags(terminated)
-        trunc = dev_flags(truncated) if truncated is not None else None
+        term = dev_flags(terminated, E, dev)
+        trunc = dev_flags(truncated, E, dev) if truncated is not None else None
         f32 = lambda x: torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
         f64 = lambda x: torch.as_tensor(x, dtype=torch.float64).to(dev).contiguous()       # widened exactly
         inputs = [f32(obs), f64(desired_goal), f32(action), f64(reward).reshape(E), f32(obs_next),
                   f64(achieved_goal_next), term, trunc]
         self._goal_launch(w, inputs, plan, n_draws, n_rows, False)
         w.advance(True)
-        if on_dev:                                # the episode ends are applied at the next call
-            w.ends[0].copy_(term, non_blocking=True)
-            if trunc is not None:
-                w.ends[1].copy_(trunc, non_blocking=True)
-            else:
-                w.ends[1].zero_()                 # host memory: no copy into it is in flight (waited for above)
-            w.event.record()
-            w.pending = True
-        else:
-            ended = np.asarray(terminated).reshape(E).astype(bool)
-            if truncated is not None:
-                ended = ended | np.asarray(truncated).reshape(E).astype(bool)
-            w.end(ended)
+        w.record_ends(term, trunc, terminated, truncated)
         return n_rows
 
     def flush_goal_steps(self):
@@ -661,7 +627,7 @@ class _DeviceReplay(object):
         if w is None:
             return 0
         self.flush()
-        self._goal_resolve(w)
+        w.resolve()
         plan, n_draws, n_rows = w.draw()
         if n_rows:
             self._goal_launch(w, [None] * 8, plan, n_draws, n_rows, True)
@@ -675,8 +641,13 @@ class _DeviceReplay(object):
     def _add_device(self, n, tensors):
         _lib.check(_lib.lib().d4pg_replay_add(self.handle, n, *[_lib.ptr(t) for t in tensors],
                                               1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add")
-        self._len = int(_lib.lib().d4pg_replay_len(self.handle))
-        self._next_idx = int(_lib.lib().d4pg_replay_next_idx(self.handle))
+        self._sync_ring()
+
+    def _sync_ring(self):
+        """len / next_idx after a device insert, read from the handle's host mirror (no device read)."""
+        L = _lib.lib()
+        self._len = int(L.d4pg_replay_len(self.handle))
+        self._next_idx = int(L.d4pg_replay_next_idx(self.handle))
 
     def flush(self):
         self._join_ingest()
