@@ -16,7 +16,8 @@ Bound.  An element computed as sum_k a_k b_k (+ bias) from K products, with S = 
 
 Kc is the number of rows one tensor-core accumulator sums (0 for the FFMA kernels; see TRUNC).  beta = 0 where the oracle reproduces the operand rounding (fp32, tf32, bf16), BETA_3XTF32 for the 3xTF32 split, which
 the oracle does not reproduce (it takes the fp32 operands as exact).  A bias gradient is sum_k delta_k: S = sum |delta|.
-ReLU and tanh are 1-Lipschitz and keep the pre-activation bound; tanh adds 4 ulp of its output, and the tanh' factor of
+ReLU and tanh are monotone: the bound maps through them as max(f(z + e) - f(z), f(z) - f(z - e)), at most the
+pre-activation bound e and zero where the unit is off by more than e; tanh adds 4 ulp of its output, and the tanh' factor of
 d action (computed in fp32 from y) adds 4 ulp of its input sum.  On the CPU (test_gpu_step_edges.py), fp32 matmul,
 8-way split-K and sequential fp32 accumulation reach at most 0.99 x 2^-24 sqrt(K) S (at K = 1), the 3xTF32 split
 with rz hi/lo 1.23 x 2^-20 S; dropping one row's contribution exceeds the bound by > 100x.
@@ -24,10 +25,29 @@ with rz hi/lo 1.23 x 2^-20 S; dropping one row's contribution exceeds the bound 
 Power.  A bound is only worth what it rejects: for every weight and bias gradient, the reference with the contribution
 of the last batch row that contributes anything removed must be at least POWER_MIN x the bound away from the device.
 
-Layers the wgmma chains keep inside the cluster (the target chains' hidden planes, p_dz22 and p_dz2) are not written
-row-major, so actor_target_out, target_logits and a_dz3 are checked through the float64 chain (each layer cast to fp32
-as the device stores it) at relative L2 (`CHAINED_TOL`).  actor_critic="post_update" sends the policy pass through the
-critic AFTER its Adam step, whose h1 the device recomputes without storing: h2_p is checked through that chain too.
+Chained layers.  Layers the wgmma chains keep inside the cluster (the target chains' hidden planes, p_dz22 and p_dz2)
+are not written row-major, and actor_critic="post_update" sends the policy pass through the critic AFTER its Adam step,
+whose h1 the device recomputes without storing.  So actor_target_out, target_logits, a_dz3 and (post_update) h2_p are
+checked through a chain: each chained layer's reference input x_ref is the previous layer's reference cast to fp32, and
+the device's unobserved input x differs from it by at most e componentwise (e = 0 for a plane read back from the
+device).  A layer y = f(rho(x) W^T + b) then carries the bound forward (`chained_layer`):
+
+    d   = max |rho(x) - rho(x_ref)| over |x - x_ref| <= e           (`operand_error`: rho is monotone, so the ends of
+                                                                     the interval, rounded outward to fp32, give it)
+    e_y = |rho(W)| d + bound(|rho(W)| (|rho(x_ref)| + d) + |b|, K)   (the operand error, then the accumulation of the
+                                                                     device's own operands, whose |.| sum is at most S)
+
+mapped through f as above (monotone and 1-Lipschitz, so no mask flip needs a case of its own, and a unit that is off by
+more than e_y passes no error on), plus 4 ulp for tanh, and, where the next layer consumes it, |y_ref - fp32(y_ref)|
+for the fp32 store of the reference.  Mapping through the ReLUs, rather than carrying e_y past them, keeps the bound
+~5x tighter over three chained layers, where |W| d grows it by up to ~sqrt(256) per layer against W x.  This holds
+row by row, so it is valid at every batch size.
+Under one TF32 pass an e of one fp32 ulp may move an operand to the neighbouring TF32 value (2^-10 relative), so the
+bound grows toward the one-pass error itself over three chained layers: it cannot separate one pass from three
+(test_gpu_tf32.py), which the teacher-forced planes already do.  Power: the reference without the last chained layer's
+bias (a_dz3, which has none: without the ReLU mask of p_dz2, the last layer the cluster keeps) must land POWER_MIN x
+outside the bound.  From batch 200 on, where it was measured, the relative L2 error of the same outputs is also held to
+`CHAINED_TOL`, as a separation statistic.
 """
 import math
 
@@ -71,10 +91,12 @@ def kslice(K):
     return -(-(-(-K // ksplit)) // 64) * 64
 # kernels of one eager step, by plan (no post-update critic)
 KERNELS = {"tc_chain": 9, "chain": 7, "levels": 18}
-# relative L2 of the chained checks: a one-pass TF32 chain may truncate a chained operand whose fp32 value differs in
-# the last bit to the neighbouring TF32 value (test_gpu_tf32.py); an unrounded chain differs by fp32 casts only
+# relative L2 of the chained outputs, a separation statistic from CHAINED_L2_MIN_B rows on (a batch statistic: nothing
+# averages it over a few rows).  A one-pass TF32 chain may truncate a chained operand whose fp32 value differs in the
+# last bit to the neighbouring TF32 value (test_gpu_tf32.py); an unrounded chain differs by fp32 casts only
 CHAINED_TOL = {None: {"actor_target_out*": 1e-5, "target_logits*": 1e-5, "a_dz3*": 1e-5, "h2_p*": 1e-5},
                "rz": {"actor_target_out*": 5e-5, "target_logits*": 5e-6, "a_dz3*": 1e-4, "h2_p*": 5e-5}}
+CHAINED_L2_MIN_B = 200
 
 
 def rnd(t, rho):
@@ -121,11 +143,68 @@ def drop_row_ratio(dev, ref, tol, a, b, rho):
     return ratio(dev, ref - contrib.reshape(ref.shape), tol)
 
 
+def rel_l2(dev, ref):
+    return float((dev.double() - ref.double()).norm()) / max(float(ref.norm()), 1e-30)
+
+
+def _fp32_outward(v, up):
+    """The nearest fp32 value >= v (up) or <= v of a float64 tensor."""
+    f = v.float()
+    past = f.double() < v if up else f.double() > v
+    return torch.where(past, torch.nextafter(f, torch.full_like(f, math.inf if up else -math.inf)), f)
+
+
+def operand_error(x, e, rho):
+    """The largest |rho(x') - rho(x)| over fp32 x' with |x' - x| <= e, componentwise: rho is monotone, so it is
+    reached at an end of [x - e, x + e] rounded outward to fp32 (rho None: e itself)."""
+    e = e.double()
+    if rho is None:
+        return e
+    xd = x.float().double()
+    r0 = rnd(x.float(), rho)
+    hi, lo = rnd(_fp32_outward(xd + e, True), rho), rnd(_fp32_outward(xd - e, False), rho)
+    return torch.maximum((hi - r0).abs(), (r0 - lo).abs())
+
+
+def chained_layer(x, e, wt, b, rho, beta=0.0, kc=0, act=None, mask=None, tanh_y=None):
+    """One layer act(rho(x) @ rho(wt) + b) (b None: no bias), then * mask or * (1 - tanh_y^2), on the fp32 input x whose
+    device value may differ from it by up to e componentwise (e = 0: the device's own plane).  Returns the float64
+    reference and the componentwise bound of |device - reference| (module docstring)."""
+    d = operand_error(x, e, rho)
+    rx, aw = rnd(x, rho), rnd(wt, rho)
+    ref = rx @ aw
+    aw = aw.abs()
+    S = (rx.abs() + d) @ aw
+    if b is not None:
+        ref, S = ref + b.double(), S + b.double().abs()
+    tol = d @ aw + bound(S, x.shape[1], beta, kc=kc)
+    if act is not None:            # monotone: the device's z within [ref - tol, ref + tol] maps into [f(.), f(.)]
+        f = torch.relu if act == "relu" else torch.tanh
+        y = f(ref)
+        tol, ref = torch.maximum(f(ref + tol) - y, y - f(ref - tol)), y
+        if act == "tanh":
+            tol = tol + 4 * 2.0 ** -23 * ref.abs()
+    if mask is not None:
+        ref, tol = ref * mask, tol * mask
+    if tanh_y is not None:         # the tanh' factor, computed in fp32 from y, adds 4 ulp of its input sum
+        f = 1 - tanh_y.double() ** 2
+        ref, tol = ref * f, tol * f.abs() + 4 * U * S
+    return ref, tol
+
+
+def stored(ref, tol):
+    """A chained layer's output as the next layer's input: the reference cast to fp32 and the bound widened by that
+    cast, so that it bounds |device fp32 value - fp32 reference|."""
+    x = ref.float()
+    return x, tol + (ref - x.double()).abs()
+
+
 class Report:
-    """(name, ratio to the bound) of every check and the power ratios; all printed before the first failure."""
+    """(name, ratio to the bound) of every check and the power ratios; all printed before the first failure.  `chained`
+    holds (name, relative L2, its tolerance or None where the batch is too small to hold it to one)."""
 
     def __init__(self, label):
-        self.label, self.rows, self.power, self.chained = label, [], [], []
+        self.label, self.rows, self.power, self.chained, self.sep = label, [], [], [], []
 
     def add(self, name, r):
         self.rows.append((name, r))
@@ -134,14 +213,16 @@ class Report:
         for name, r in self.rows:
             print("%s %-20s %.3f of bound" % (self.label, name, r))
         for name, r, tol in self.chained:
-            print("%s %-20s rel L2 %.3e (bound %.1e)" % (self.label, name, r, tol))
+            print("%s %-20s rel L2 %.3e (%s)" % (self.label, name, r, "bound %.1e" % tol if tol else "not held"))
         for name, r in self.power:
-            print("%s %-20s last contributing row dropped: %.3g x bound" % (self.label, name, r))
+            print("%s %-20s power: %.3g x bound" % (self.label, name, r if r is not None else math.nan))
+        for kind, name, r in self.sep:
+            print("%s %-20s %s: %.3g x bound from the unrounded layer" % (self.label, name, kind, r))
         worst = max((r for _, r in self.rows), default=0.0)
         pmin = min((r for _, r in self.power if r is not None), default=math.inf)
         print("%s worst %.3f of bound, smallest power ratio %.3g" % (self.label, worst, pmin))
         bad = ["%s %.3g" % (n, r) for n, r in self.rows if not r <= 1.0]
-        bad += ["%s rel L2 %.3e > %.1e" % (n, r, tol) for n, r, tol in self.chained if not r <= tol]
+        bad += ["%s rel L2 %.3e > %.1e" % (n, r, tol) for n, r, tol in self.chained if tol and not r <= tol]
         bad += ["%s power %s" % (n, r) for n, r in self.power if r is None or not r >= POWER_MIN]
         assert not bad, "%s: %s" % (self.label, ", ".join(bad))
         return worst, pmin
@@ -183,30 +264,24 @@ class StepCheck:
         return self.t(name, self._width(name))
 
     # ---- one layer ------------------------------------------------------------------------------------------------
+    def layer(self, name, kind, x, wt, b=None, act=None, mask=None, tanh_y=None):
+        """act(x @ wt + b) (* mask, or * (1 - tanh_y^2)) on the device's own input x against the device plane `name`.
+        A one-pass precision also records in `rep.sep` how far the device lands from the UNROUNDED layer, in units of
+        that layer's bound: far outside it where the operands really are rounded."""
+        kc = x.shape[1] if self.tc_fwd else 0
+        e = torch.zeros(x.shape, dtype=torch.float64, device=x.device)
+        dev = self.dev(name)
+        self.rep.add(name, ratio(dev, *chained_layer(x, e, wt, b, self.rho, self.beta, kc, act, mask, tanh_y)))
+        if self.rho is not None:
+            self.rep.sep.append((kind, name, ratio(dev, *chained_layer(x, e, wt, b, None, 0.0, kc, act, mask, tanh_y))))
+
     def forward(self, name, x, w, layer, act):
         """y = act(x @ W^T + b) against the device plane `name`."""
-        W, b = w[layer + ".weight"], w[layer + ".bias"]
-        kc = x.shape[1] if self.tc_fwd else 0
-        ref, tol = matmul_bound(x, W.T, self.rho, self.beta, kc)
-        ref = ref + b.double()
-        tol = tol + bound(b.double().abs(), x.shape[1], self.beta, kc=kc)
-        if act == "relu":
-            ref = torch.relu(ref)
-        elif act == "tanh":
-            ref = torch.tanh(ref)
-            tol = tol + 4 * 2.0 ** -23 * ref.abs()
-        self.rep.add(name, ratio(self.dev(name), ref, tol))
+        self.layer(name, "fwd", x, w[layer + ".weight"].T, w[layer + ".bias"], act)
 
     def backward(self, name, g, w, mask=None, tanh_y=None):
         """dX = (g @ W) * mask (or * (1 - y^2)) against the device plane `name`."""
-        ref, tol = matmul_bound(g, w, self.rho, self.beta, g.shape[1] if self.tc_fwd else 0)
-        if mask is not None:
-            ref, tol = ref * mask, tol * mask
-        if tanh_y is not None:
-            f = 1 - tanh_y.double() ** 2
-            S = rnd(g, self.rho).abs() @ rnd(w, self.rho).abs()
-            ref, tol = ref * f, tol * f.abs() + 4 * U * S
-        self.rep.add(name, ratio(self.dev(name), ref, tol))
+        self.layer(name, "dX", g, w, mask=mask, tanh_y=tanh_y)
 
     def grad(self, name, dev, delta, x):
         """dW = delta^T x (x None: the bias gradient, sum of the fp32 delta) against the device gradient `dev`, and the
@@ -222,16 +297,59 @@ class StepCheck:
         self.rep.add(name, ratio(dev, ref, tol))
         self.rep.power.append((name, drop_row_ratio(dev, ref, tol, delta, x, rho)))
 
-    def chained(self, name, dev, ref):
-        r = float((dev.double() - ref).norm()) / max(float(ref.norm()), 1e-30)
-        self.rep.chained.append((name, r, CHAINED_TOL["rz" if self.rho else None][name]))
+    # ---- chained layers ---------------------------------------------------------------------------------------------
+    def chain(self, x, e, w, layers, rho):
+        """Forward layers [(layer, act)] of `w` from the fp32 input x (device error e): (reference, bound, reference
+        without the last layer's bias) of the last layer, each earlier one `stored` as the next one's input."""
+        kc = lambda x: x.shape[1] if self.tc_fwd else 0
+        for i, (l, act) in enumerate(layers):
+            if i:
+                x, e = stored(ref, tol)
+            ref, tol = chained_layer(x, e, w[l + ".weight"].T, w[l + ".bias"], rho, self.beta, kc(x), act)
+        return ref, tol, chained_layer(x, e, w[l + ".weight"].T, None, rho, self.beta, kc(x), act)[0]
 
-    def chain(self, x, w, layers):
-        """Layers in float64 on rho-rounded operands, each cast to fp32 as the device stores it."""
-        for l, act in layers:
-            y = rnd(x, self.rho) @ rnd(w[l + ".weight"], self.rho).T + w[l + ".bias"].double()
-            x = (torch.relu(y) if act == "relu" else torch.tanh(y) if act == "tanh" else y).float()
-        return x
+    def chained_refs(self, rho="plan"):
+        """{output: (reference, bound, power reference)} of every output this plan computes through layers it does
+        not write row-major (module docstring), from the device's planes; rho=None gives the unrounded chains."""
+        rho = self.rho if rho == "plan" else rho
+        t, dev, W = self.t, self.dev, self.W
+        zero = lambda x: torch.zeros(x.shape, dtype=torch.float64, device=x.device)
+        out = {}
+        if self.post_update:      # h1 of the updated critic is recomputed on the device, not stored
+            s, aout = t("s", self.S), dev("actor_out")
+            h1, e1 = stored(*self.chain(s, zero(s), W["p"], (("fc1", "relu"),), rho)[:2])
+            out["h2_p*"] = self.chain(torch.cat([h1, aout], 1), torch.cat([e1, zero(aout)], 1), W["p"], (("fc2", "relu"),), rho)
+        if not self.tc:
+            return out
+        s2, at_out = t("s2", self.S), dev("actor_target_out")
+        out["actor_target_out*"] = self.chain(s2, zero(s2), W["at"], (("fc1", "relu"), ("fc2", None), ("fc2_2", "relu"),
+                                                                      ("fc3", "tanh")), rho)
+        h1, e1 = stored(*self.chain(s2, zero(s2), W["ct"], (("fc1", "relu"),), rho)[:2])
+        out["target_logits*"] = self.chain(torch.cat([h1, at_out], 1), torch.cat([e1, zero(at_out)], 1), W["ct"],
+                                           (("fc2", "relu"), ("fc2_2", "relu"), ("fc3", None)), rho)
+        # the dX chain p_dz22 -> p_dz2 -> a_dz3 from the device's dlogits_pi, masks and actor output
+        Wp, dpi, aout = W["p"], dev("dlogits_pi"), dev("actor_out")
+        m2, m3 = (dev("h2_p") > 0).double(), (dev("h3_p") > 0).double()
+        kc = lambda x: x.shape[1] if self.tc_fwd else 0
+        p22, e22 = stored(*chained_layer(dpi, zero(dpi), Wp["fc3.weight"], None, rho, self.beta, kc(dpi), mask=m3))
+        p2 = chained_layer(p22, e22, Wp["fc2_2.weight"], None, rho, self.beta, kc(p22), mask=m2)
+        p2, e2 = stored(*p2)
+        w3 = Wp["fc2.weight"][:, H_:]
+        ref, tol = chained_layer(p2, e2, w3, None, rho, self.beta, kc(p2), tanh_y=aout)
+        # power: a_dz3 has no bias; drop the ReLU mask of p_dz2, the last layer the cluster keeps
+        p2_unmasked = stored(*chained_layer(p22, e22, Wp["fc2_2.weight"], None, rho, self.beta, kc(p22)))[0]
+        out["a_dz3*"] = (ref, tol, chained_layer(p2_unmasked, zero(p2), w3, None, rho, self.beta, kc(p2), tanh_y=aout)[0])
+        return out
+
+    def chained(self, refs):
+        """Every output of `refs` (chained_refs) against its device plane: the propagated bound and its power at every
+        batch size, the relative L2 error from CHAINED_L2_MIN_B rows on."""
+        for name, (ref, tol, ref_power) in refs.items():
+            dev = self.dev(name[:-1])
+            self.rep.add(name, ratio(dev, ref, tol))
+            self.rep.power.append((name, ratio(dev, ref_power, tol)))
+            held = self.B >= CHAINED_L2_MIN_B
+            self.rep.chained.append((name, rel_l2(dev, ref), CHAINED_TOL["rz" if self.rho else None][name] if held else None))
 
     # ---- the step ---------------------------------------------------------------------------------------------------
     def run(self):
@@ -251,10 +369,7 @@ class StepCheck:
         f("h3_c", ch2, Wc, "fc2_2", "relu")
         f("q_logits", ch3, Wc, "fc3", None)
         ph2, ph3 = dev("h2_p"), dev("h3_p")
-        if self.post_update:      # h1 of the updated critic is recomputed on the device, not stored
-            self.chained("h2_p*", ph2, self.chain(torch.cat([self.chain(s, Wp, (("fc1", "relu"),)), aout], 1), Wp,
-                                                  (("fc2", "relu"),)).double())
-        else:                     # the policy pass's critic h1 is h1_c
+        if not self.post_update:  # the policy pass's critic h1 is h1_c (post_update: chained_refs)
             f("h2_p", torch.cat([ch1, aout], 1), Wp, "fc2", "relu")
         f("h3_p", ph2, Wp, "fc2_2", "relu")
         f("pi_logits", ph3, Wp, "fc3", None)
@@ -270,12 +385,7 @@ class StepCheck:
             f("h2_ct", torch.cat([ct1, at_out], 1), Wct, "fc2", "relu")
             f("h3_ct", ct2, Wct, "fc2_2", "relu")
             f("target_logits", ct3, Wct, "fc3", None)
-        else:
-            self.chained("actor_target_out*", at_out,
-                         self.chain(s2, Wat, (("fc1", "relu"), ("fc2", None), ("fc2_2", "relu"), ("fc3", "tanh"))).double())
-            ct1 = self.chain(s2, Wct, (("fc1", "relu"),))
-            self.chained("target_logits*", dev("target_logits"),
-                         self.chain(torch.cat([ct1, at_out], 1), Wct, (("fc2", "relu"), ("fc2_2", "relu"), ("fc3", None))).double())
+        self.chained(self.chained_refs())
 
         # backward: from the device's logit gradients, deltas and masks
         dq, dpi = dev("dlogits_q"), dev("dlogits_pi")
@@ -286,12 +396,7 @@ class StepCheck:
         bw("c_dz2", c_dz22, Wc["fc2_2.weight"], m(ch2))
         bw("c_dz1", c_dz2, Wc["fc2.weight"][:, :H_], m(ch1))
         a_dz3 = dev("a_dz3")
-        if self.tc:               # p_dz22 / p_dz2 stay in the cluster
-            p22 = (rnd(dpi, self.rho) @ rnd(Wp["fc3.weight"], self.rho) * m(ph3)).float()
-            p2 = (rnd(p22, self.rho) @ rnd(Wp["fc2_2.weight"], self.rho) * m(ph2)).float()
-            ref = rnd(p2, self.rho) @ rnd(Wp["fc2.weight"][:, H_:], self.rho) * (1 - aout.double() ** 2)
-            self.chained("a_dz3*", a_dz3, ref)
-        else:
+        if not self.tc:           # tc: p_dz22 / p_dz2 stay in the cluster (chained_refs)
             p_dz22, p_dz2 = dev("p_dz22"), dev("p_dz2")
             bw("p_dz22", dpi, Wp["fc3.weight"], m(ph3))
             bw("p_dz2", p_dz22, Wp["fc2_2.weight"], m(ph2))

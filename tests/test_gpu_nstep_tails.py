@@ -2,7 +2,8 @@
 bit-exact against the oracle (tests/nstep_tails_oracle.py) over window lengths, environment counts, shapes, ring wraps
 and both kinds of end flags, with the trees, max_priority and the normalizer equal to add_batch of the oracle's rows;
 n = 1 and the full rows equal to a tails-off buffer; other insert paths clearing horizons; the learner's per-row
-discounts in the categorical, mixture and quantile heads against their oracles; a tails-on learner over all-zero
+discounts in the categorical, mixture and quantile heads against their oracles; every layer of one-pass TF32 and bf16
+learner steps over tail rows; a tails-on learner over all-zero
 horizons bit-identical to a tails-off one; and the launches per call."""
 import random
 
@@ -14,6 +15,7 @@ from tests import mog_oracle as MO
 from tests import nstep_stream_oracle as SO
 from tests import nstep_tails_oracle as TO
 from tests import qr_oracle as QO
+from tests import step_check as SC
 
 pytestmark = pytest.mark.gpu
 
@@ -273,6 +275,39 @@ def test_categorical_projection_per_row():
     tp = dd.debug_tensor("target_probs", shape=(B, 51)).cpu().numpy()
     m, _, _ = TO.project_disc(tp, r, d, INFO["v_min"], INFO["v_max"], 51, TO.row_discounts(h, dd.gamma, n))
     assert np.abs(dd.debug_tensor("m", shape=(B, 51)).cpu().numpy() - m).max() <= 2e-7
+
+
+# (plan, precision, |s|, |a|, DDPG options): the one-pass precisions on each plan they run (csrc/learner.cu step_plan)
+ONE_PASS = [("tc_chain", "tf32", 17, 6, {}), ("chain", "tf32", 33, 6, {}),
+            ("levels", "tf32", 17, 6, {"chain": "levels"}), ("levels", "bf16", 17, 6, {})]
+
+
+@pytest.mark.parametrize("plan,precision,S,A,opts", ONE_PASS, ids=["%s_%s" % c[:2] for c in ONE_PASS])
+def test_one_pass_learner_tails(plan, precision, S, A, opts):
+    """One TF32 pass and bf16 with tails, fed by observe() with many truncations: after each step the projected rows
+    equal the f64 per-row-discount projection of the learner's own target probabilities to within one f32 rounding,
+    every layer of the step passes tests/step_check.py for its plan and precision, and the batch holds tail rows."""
+    import d4pg_b200 as d4pg
+    E, n, B = 32, 5, 64
+    torch.manual_seed(0)
+    dd = d4pg.DDPG(S, A, memory_size=4096, batch_size=B, critic_dist_info=INFO, n_steps=n, projection="nstep",
+                   nstep_tails=True, gamma=0.95, precision=precision, sampling="device", prefetch=False, **opts)
+    dd.assign_global_optimizer(d4pg.SharedAdam(dd.actor.parameters(), lr=1e-3),
+                               d4pg.SharedAdam(dd.critic.parameters(), lr=1e-3))
+    rng = np.random.RandomState(8)
+    _learner_stream(dd, rng, 12, E, trunc_p=0.4)
+    for step in range(3):
+        _learner_stream(dd, rng, 1, E, trunc_p=0.4)
+        W = SC.snapshot(dd)
+        dd.train()
+        torch.cuda.synchronize()
+        assert dd.kernels_per_step() == SC.KERNELS[plan], (plan, dd.kernels_per_step())
+        s, a, r, s2, d, h = _batch(dd)
+        assert ((h > 0) & ~d).any(), step
+        tp = dd.debug_tensor("target_probs", shape=(B, 51)).cpu().numpy()
+        m, _, _ = TO.project_disc(tp, r, d, INFO["v_min"], INFO["v_max"], 51, TO.row_discounts(h, dd.gamma, n))
+        assert np.abs(dd.debug_tensor("m", shape=(B, 51)).cpu().numpy() - m).max() <= 2e-7, step
+        SC.check_step(dd, W, plan, precision, label="tails %s/%s step %d" % (plan, precision, step))
 
 
 @pytest.mark.parametrize("kind", ["mixture", "quantile"])
