@@ -2,6 +2,10 @@
 DDPG.train() recomputed in float64 from the DEVICE's own input to that layer (teacher forcing), and held to a
 componentwise bound.
 
+`LayerCheck` holds the per-layer part (the `MODES` row, one layer, one weight or bias gradient, chained layers and the
+`Report`) and checks whatever device tensor it is handed (tests/test_gpu_module_edges.py: the actor and critic entry
+points); `StepCheck` reads the step's planes through `dd.debug_tensor`.
+
 Teacher forcing.  Each layer is fed the device's input plane, the device's ReLU mask (h > 0) and the device's upstream
 delta, and the tanh' factor is 1 - y^2 of the device's own actor output.  A pre-activation within rounding of zero then
 masks the same element on both sides, so no delta element can flip and a tight bound survives any batch size.
@@ -234,11 +238,61 @@ def snapshot(dd):
             for k, net in (("a", dd.actor), ("at", dd.actor_target), ("c", dd.critic), ("ct", dd.critic_target))}
 
 
-class StepCheck:
+class LayerCheck:
+    """Teacher-forced checks of single layers computed by the kernels of (plan, precision) (`MODES`), each against the
+    device tensor it is handed; every result goes to `rep`."""
+
+    def __init__(self, plan, precision, label):
+        self.rho, self.beta, self.tc_fwd, self.rho_dw, self.beta_dw, self.tc_dw = MODES[plan, precision]
+        self.rep = Report(label)
+
+    def layer(self, name, kind, dev, x, wt, b=None, act=None, mask=None, tanh_y=None):
+        """act(x @ wt + b) (* mask, or * (1 - tanh_y^2)) on the device's own input x against the device tensor `dev`.
+        A one-pass precision also records in `rep.sep` how far the device lands from the UNROUNDED layer, in units of
+        that layer's bound: far outside it where the operands really are rounded."""
+        kc = x.shape[1] if self.tc_fwd else 0
+        e = torch.zeros(x.shape, dtype=torch.float64, device=x.device)
+        self.rep.add(name, ratio(dev, *chained_layer(x, e, wt, b, self.rho, self.beta, kc, act, mask, tanh_y)))
+        if self.rho is not None:
+            self.rep.sep.append((kind, name, ratio(dev, *chained_layer(x, e, wt, b, None, 0.0, kc, act, mask, tanh_y))))
+
+    def grad(self, name, dev, delta, x, e=None, sep=False):
+        """dW = delta^T x (x None: the bias gradient, sum of the fp32 delta) against the device gradient `dev`, and the
+        power of the bound against a dropped row.  e: the componentwise bound of |device delta - delta| where the
+        device's delta is not observed (a chained layer's `stored` output), carried through the sum as `chained_layer`
+        carries an input error.  sep: record in `rep.sep` (kind "dW") how far the device lands from the unrounded dW.
+        Returns (reference, bound)."""
+        rho = None if x is None else self.rho_dw
+        if x is None:
+            err = 0.0 if e is None else e.sum(0)
+            ref, tol = delta.double().sum(0), err + bound(delta.double().abs().sum(0) + err, delta.shape[0])
+        else:
+            kc = kslice(delta.shape[0]) if self.tc_dw else 0
+            dw = lambda rho, beta: (matmul_bound(delta.T, x, rho, beta, kc) if e is None
+                                    else chained_layer(delta.T, e.T, x, None, rho, beta, kc))
+            ref, tol = dw(rho, self.beta_dw)
+        dev = dev.to(ref.device).reshape(ref.shape)
+        self.rep.add(name, ratio(dev, ref, tol))
+        self.rep.power.append((name, drop_row_ratio(dev, ref, tol, delta, x, rho)))
+        if sep and rho is not None:
+            self.rep.sep.append(("dW", name, ratio(dev, *dw(None, 0.0))))
+        return ref, tol
+
+    def chain(self, x, e, w, layers, rho):
+        """Forward layers [(layer, act)] of `w` from the fp32 input x (device error e): (reference, bound, reference
+        without the last layer's bias) of the last layer, each earlier one `stored` as the next one's input."""
+        kc = lambda x: x.shape[1] if self.tc_fwd else 0
+        for i, (l, act) in enumerate(layers):
+            if i:
+                x, e = stored(ref, tol)
+            ref, tol = chained_layer(x, e, w[l + ".weight"].T, w[l + ".bias"], rho, self.beta, kc(x), act)
+        return ref, tol, chained_layer(x, e, w[l + ".weight"].T, None, rho, self.beta, kc(x), act)[0]
+
+
+class StepCheck(LayerCheck):
     """The teacher-forced restatement of the step `dd` just ran from the weights `W` (a `snapshot` taken before it)."""
 
     def __init__(self, dd, W, plan, precision, post_update=False, label=None):
-        self.rho, self.beta, self.tc_fwd, self.rho_dw, self.beta_dw, self.tc_dw = MODES[plan, precision]
         self.tc, self.post_update = plan == "tc_chain", post_update
         dev = dd.critic.fc3.weight.device
         self.W = {k: {n_: v.to(dev) for n_, v in w.items()} for k, w in W.items()}
@@ -251,7 +305,7 @@ class StepCheck:
         B = dd.batch_size
         self.B = B
         self.t = lambda name, w=None: dd.debug_tensor(name, (B, w) if w else None)
-        self.rep = Report(label or "%s/%s(%d,%d,%d,%d)" % (plan, precision, B, self.S, self.A, self.N))
+        super().__init__(plan, precision, label or "%s/%s(%d,%d,%d,%d)" % (plan, precision, B, self.S, self.A, self.N))
 
     def _width(self, name):
         if name in ("actor_out", "actor_target_out", "a_dz3"):
@@ -264,50 +318,15 @@ class StepCheck:
         return self.t(name, self._width(name))
 
     # ---- one layer ------------------------------------------------------------------------------------------------
-    def layer(self, name, kind, x, wt, b=None, act=None, mask=None, tanh_y=None):
-        """act(x @ wt + b) (* mask, or * (1 - tanh_y^2)) on the device's own input x against the device plane `name`.
-        A one-pass precision also records in `rep.sep` how far the device lands from the UNROUNDED layer, in units of
-        that layer's bound: far outside it where the operands really are rounded."""
-        kc = x.shape[1] if self.tc_fwd else 0
-        e = torch.zeros(x.shape, dtype=torch.float64, device=x.device)
-        dev = self.dev(name)
-        self.rep.add(name, ratio(dev, *chained_layer(x, e, wt, b, self.rho, self.beta, kc, act, mask, tanh_y)))
-        if self.rho is not None:
-            self.rep.sep.append((kind, name, ratio(dev, *chained_layer(x, e, wt, b, None, 0.0, kc, act, mask, tanh_y))))
-
     def forward(self, name, x, w, layer, act):
         """y = act(x @ W^T + b) against the device plane `name`."""
-        self.layer(name, "fwd", x, w[layer + ".weight"].T, w[layer + ".bias"], act)
+        self.layer(name, "fwd", self.dev(name), x, w[layer + ".weight"].T, w[layer + ".bias"], act)
 
     def backward(self, name, g, w, mask=None, tanh_y=None):
         """dX = (g @ W) * mask (or * (1 - y^2)) against the device plane `name`."""
-        self.layer(name, "dX", g, w, mask=mask, tanh_y=tanh_y)
-
-    def grad(self, name, dev, delta, x):
-        """dW = delta^T x (x None: the bias gradient, sum of the fp32 delta) against the device gradient `dev`, and the
-        power of the bound against a dropped row."""
-        if x is None:
-            ref, tol = delta.double().sum(0), bound(delta.double().abs().sum(0), delta.shape[0])
-            rho = None
-        else:
-            kc = kslice(delta.shape[0]) if self.tc_dw else 0
-            ref, tol = matmul_bound(delta.T, x, self.rho_dw, self.beta_dw, kc)
-            rho = self.rho_dw
-        dev = dev.to(ref.device).reshape(ref.shape)
-        self.rep.add(name, ratio(dev, ref, tol))
-        self.rep.power.append((name, drop_row_ratio(dev, ref, tol, delta, x, rho)))
+        self.layer(name, "dX", self.dev(name), g, w, mask=mask, tanh_y=tanh_y)
 
     # ---- chained layers ---------------------------------------------------------------------------------------------
-    def chain(self, x, e, w, layers, rho):
-        """Forward layers [(layer, act)] of `w` from the fp32 input x (device error e): (reference, bound, reference
-        without the last layer's bias) of the last layer, each earlier one `stored` as the next one's input."""
-        kc = lambda x: x.shape[1] if self.tc_fwd else 0
-        for i, (l, act) in enumerate(layers):
-            if i:
-                x, e = stored(ref, tol)
-            ref, tol = chained_layer(x, e, w[l + ".weight"].T, w[l + ".bias"], rho, self.beta, kc(x), act)
-        return ref, tol, chained_layer(x, e, w[l + ".weight"].T, None, rho, self.beta, kc(x), act)[0]
-
     def chained_refs(self, rho="plan"):
         """{output: (reference, bound, power reference)} of every output this plan computes through layers it does
         not write row-major (module docstring), from the device's planes; rho=None gives the unrounded chains."""

@@ -69,67 +69,6 @@ def _lin(x, w, b=None, bf16=True):
     return y if b is None else y + b.double()
 
 
-def _forward_case(d4pg, S, A, N, B):
-    """d4pg_actor_forward / d4pg_critic_forward at precision 3 on one shape.  Each layer is checked against the float64
-    restatement on the bf16-rounded operands, fed the device's own input to that layer (read back from the workspace),
-    so an operand that rounds to bf16 from equal fp32 values is equal on both sides: bound 1e-4 absolute.  Returns each
-    output's distance from the UNROUNDED float64 chain."""
-    info = {"type": "categorical", "v_min": -50.0, "v_max": 0.0, "n_atoms": N}
-    torch.manual_seed(31)
-    act = d4pg.models.actor(S, A, device="cuda")
-    cri = d4pg.models.critic(S, A, info, device="cuda")
-    with torch.no_grad():                     # output layers at the hidden layers' scale: rounding visible at 1e-4
-        act.fc3.weight.normal_(0.0, 1.0 / 16); cri.fc3.weight.normal_(0.0, 0.25)
-    act.precision = 3; cri.precision = 3
-    g = torch.Generator().manual_seed(32)
-    s = torch.randn(B, S, generator=g).cuda(); a = (torch.rand(B, A, generator=g) * 2 - 1).cuda()
-    wa = {k: v.detach().cpu() for k, v in act.state_dict().items()}
-    wc = {k: v.detach().cpu() for k, v in cri.state_dict().items()}
-    relu = torch.relu
-    s_c, a_c = s.cpu(), a.cpu()
-
-    out = act(s)
-    torch.cuda.synchronize()
-    ws = act._ws[:3 * B * H_].view(3, B, H_).cpu()
-    _close("actor h1", ws[0], relu(_lin(s_c, wa["fc1.weight"], wa["fc1.bias"])), 1e-4)
-    _close("actor h2", ws[1], _lin(ws[0], wa["fc2.weight"], wa["fc2.bias"]), 1e-4)
-    _close("actor h3", ws[2], relu(_lin(ws[1], wa["fc2_2.weight"], wa["fc2_2.bias"])), 1e-4)
-    ref = torch.tanh(_lin(ws[2], wa["fc3.weight"], wa["fc3.bias"]))
-    assert float((out.double().cpu() - ref).abs().max()) <= 1e-4
-    x = s_c.double()
-    for l, w in enumerate(("fc1", "fc2", "fc2_2", "fc3")):
-        x = _lin(x, wa[w + ".weight"], wa[w + ".bias"], bf16=False)
-        x = relu(x) if l in (0, 2) else (torch.tanh(x) if l == 3 else x)
-    far = {"action": float((out.double().cpu() - x).abs().max())}
-
-    probs, logits = cri(s, a, return_logits=True)
-    torch.cuda.synchronize()
-    ws = cri._ws[:3 * B * H_].view(3, B, H_).cpu()
-    _close("critic h1", ws[0], relu(_lin(s_c, wc["fc1.weight"], wc["fc1.bias"])), 1e-4)
-    _close("critic h2", ws[1], relu(_lin(torch.cat([ws[0], a_c], 1), wc["fc2.weight"], wc["fc2.bias"])), 1e-4)
-    _close("critic h3", ws[2], relu(_lin(ws[1], wc["fc2_2.weight"], wc["fc2_2.bias"])), 1e-4)
-    ref_z = _lin(ws[2], wc["fc3.weight"], wc["fc3.bias"])
-    assert float((logits.double().cpu() - ref_z).abs().max()) <= 1e-4
-    assert float((probs.double().cpu() - torch.softmax(ref_z, 1)).abs().max()) <= 1e-4
-    h = relu(_lin(s_c, wc["fc1.weight"], wc["fc1.bias"], bf16=False))
-    h = relu(_lin(torch.cat([h, a_c.double()], 1), wc["fc2.weight"], wc["fc2.bias"], bf16=False))
-    h = relu(_lin(h, wc["fc2_2.weight"], wc["fc2_2.bias"], bf16=False))
-    z = _lin(h, wc["fc3.weight"], wc["fc3.bias"], bf16=False)
-    far["logits"] = float((logits.double().cpu() - z).abs().max())
-    far["probs"] = float((probs.double().cpu() - torch.softmax(z, 1)).abs().max())
-    return far
-
-
-@pytest.mark.gpu
-def test_bf16_forward_entry_points_vs_rounded_restatement():
-    """Shapes (|s|, |a|, N, B); and each output is farther than the 1e-4 bound from the unrounded float64 chain for at
-    least one of them: the operands really are rounded to bf16."""
-    import d4pg_b200 as d4pg
-    far = {shape: _forward_case(d4pg, *shape) for shape in ((17, 6, 51, 256), (376, 17, 101, 200), (3, 1, 51, 64), (17, 6, 101, 4096))}
-    for out in ("action", "logits", "probs"):
-        assert max(f[out] for f in far.values()) > 1e-4, (out, {k: f[out] for k, f in far.items()})
-
-
 def _ddpg(d4pg, B, S, A, N, n=None, graph=False, chain="cluster", projection="reference", n_steps=1, seed=12, **kw):
     info = {"type": "categorical", "v_min": -50.0, "v_max": 0.0, "n_atoms": N}
     torch.manual_seed(seed); np.random.seed(seed); random.seed(seed)

@@ -185,9 +185,14 @@ def test_clipped_update_bit_exact_every_step(case):
     post = case[6].get("actor_critic") == "post_update"
     stats = CC.ClipStats()
     pads = None
+    # The layers of the first step, whose weights and batch the seeds fix, and of the last one where the run repeats
+    # bit for bit.  Split-K dW (the level plan from batch 1024) adds its slices with fp32 atomics in any order, and
+    # Adam turns those last-bit differences into different weights: the last step's planes, and the power of the bound
+    # on them, then change from run to run.
+    layer_steps = (0,) if plan == "levels" and case[2] >= 1024 else (0, STEPS - 1)
     for i in range(STEPS):
         before = UC.read(dd, grads=False)
-        W = SC.snapshot(dd) if i == STEPS - 1 else None
+        W = SC.snapshot(dd) if i in layer_steps else None
         random.seed(100 + i)
         dd.train()
         if pads is None:

@@ -313,24 +313,3 @@ def test_models_seeded_init_and_forward_vs_golden(d4pg):
     a2 = d4pg.actor(17, 6)
     a2.load_state_dict(sd)
     assert torch.equal(a2.flat_params(), a.flat_params())
-
-
-@pytest.mark.parametrize("precision,tol", [(1, 2e-6), (2, 5e-3)])
-def test_tensor_core_forward_vs_fp32_kernels(d4pg, precision, tol):
-    """wgmma path (1 = 3xTF32, 2 = single-pass TF32) against the exact-fp32 FFMA kernels, odd shapes
-    included (|s|=376 not a multiple of 32, N=101 atoms, batch not a multiple of 128)."""
-    for (S, A, N, B) in ((17, 6, 51, 256), (376, 17, 101, 200), (3, 1, 51, 64)):
-        torch.manual_seed(7)
-        info = {"type": "categorical", "v_min": -50.0, "v_max": 0.0, "n_atoms": N}
-        a, c = d4pg.actor(S, A), d4pg.critic(S, A, info)
-        x = torch.randn(B, S, device="cuda")
-        act = torch.rand(B, A, device="cuda") * 2 - 1
-        ref_a = a(x).clone()
-        ref_q, ref_z = c(x, act, return_logits=True)
-        ref_q, ref_z = ref_q.clone(), ref_z.clone()
-        a.precision = c.precision = precision
-        out_a = a(x)
-        q, z = c(x, act, return_logits=True)
-        assert (out_a - ref_a).abs().max().item() <= tol
-        assert (z - ref_z).abs().max().item() <= tol
-        assert (q - ref_q).abs().max().item() <= tol
