@@ -37,11 +37,12 @@ __device__ __forceinline__ double head_discount(const HeadCommon& h, int row) {
 struct HeadsArgs {
   HeadCommon h;
   int N; int flags;
-  double v_min, v_max, delta;
+  double v_min, v_max, delta;     // v_max: the top of the return clip, proj_clip_top(v_min, v_max, N, delta)
   float* m; int32_t* bins_l; int32_t* bins_u; float* target_probs; float* q_probs;
   int ce_priority;               // 1: priority = CE_i + eps instead of |sum_j m_ij q_ij| + eps (the reference does not, H4)
 };
 int launch_heads(const HeadsArgs& a, int mode, cudaStream_t st);
+double proj_clip_top(double v_min, double v_max, int N, double delta);
 
 // mixture-of-Gaussians head (mog_heads.cu): K components, raw planes of 3K columns
 struct MogArgs {

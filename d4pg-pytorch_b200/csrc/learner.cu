@@ -564,7 +564,8 @@ static int launch_step_heads(Step& x, bool only_policy) {
   } else {
     HeadsArgs ha{};
     ha.h = h; ha.N = x.N; ha.ce_priority = ce_priority;
-    ha.v_min = c.v_min; ha.v_max = c.v_max; ha.delta = (c.v_max - c.v_min) / double(x.N - 1);
+    ha.v_min = c.v_min; ha.delta = (c.v_max - c.v_min) / double(x.N - 1);
+    ha.v_max = proj_clip_top(c.v_min, c.v_max, x.N, ha.delta);
     ha.m = w.m; ha.target_probs = w.target_probs; ha.q_probs = w.q_probs;
     RUN("launch_heads", rep, launch_heads(ha, c.proj_mode, x.st));
   }

@@ -14,9 +14,30 @@
 // round-to-nearest intrinsics (no FMA contraction of r + c_j); the projected mass of mode 0 is
 // accumulated per bin in atom order j=0..N-1, each add done in fp64 and rounded to fp32, which
 // is exactly what NumPy does for `proj_distr[rows, l] += p * (u - b)` on an fp32 array.
+#include <cstring>
+
 #include "heads_dev.cuh"
 
 namespace d4pg {
+
+// The top of the projection's return clip.  b = (tz - v_min) / delta of a return clipped at v_max can round past N - 1
+// (on [-50, 0] with 32 atoms delta = 50 / 31 and b(0) = 31.000000000000004), and u = ceil(b) would then name bin N, past
+// the row.  There the clip moves down to the largest double whose b is at most N - 1; everywhere else it is v_max.
+// b is monotone in tz (a rounded subtract, then a rounded divide), so the heads' own clip keeps every b in [0, N - 1] at
+// no cost in the kernel.
+double proj_clip_top(double v_min, double v_max, int N, double delta) {
+  const auto over = [&](double t) { return (t - v_min) / delta > double(N - 1); };
+  if (!over(v_max)) return v_max;
+  // bisection over the doubles in (v_min, v_max]: keys ordered as the values are (-0.0 and +0.0 share key 0)
+  const auto key = [](double x) { int64_t k; memcpy(&k, &x, 8); return k < 0 ? INT64_MIN - k : k; };
+  const auto val = [](int64_t k) { if (k < 0) k = INT64_MIN - k; double x; memcpy(&x, &k, 8); return x; };
+  int64_t lo = key(v_min), hi = key(v_max);                // over(v_min) is false, over(v_max) true
+  while (uint64_t(hi) - uint64_t(lo) > 1) {                 // unsigned: the keys may span more than INT64_MAX
+    const int64_t mid = lo + int64_t((uint64_t(hi) - uint64_t(lo)) / 2);
+    if (over(val(mid))) hi = mid; else lo = mid;
+  }
+  return val(lo);
+}
 
 int launch_heads(const HeadsArgs& a_in, int mode, cudaStream_t st) {
   HeadsArgs a = a_in;
@@ -55,8 +76,9 @@ extern "C" int32_t d4pg_proj_loss(const float* target_logits, const float* q_log
   HeadsArgs a{};
   a.h.target = target_logits; a.h.q = q_logits; a.h.pi = pi_logits;
   a.h.rewards = rewards; a.h.dones = dones; a.h.B = B; a.N = N; a.flags = flags; a.h.ld = N;
-  a.v_min = v_min; a.v_max = v_max;
+  a.v_min = v_min;
   a.delta = (v_max - v_min) / double(N - 1);        // ddpg.py:46
+  a.v_max = proj_clip_top(v_min, v_max, N, a.delta);
   a.h.discount = discount; a.h.prio_eps = prio_eps; a.h.grad_scale = grad_scale;
   a.m = m; a.bins_l = bins_l; a.bins_u = bins_u; a.target_probs = target_probs; a.q_probs = q_probs;
   a.h.loss_rows = loss_rows; a.h.td = td; a.h.prio = prio; a.h.dq = dlogits_q;

@@ -81,7 +81,7 @@ def project_disc(target_probs, rewards, dones, v_min, v_max, n_atoms, disc):
     B = r.shape[0]
     delta, centers = O.atom_support(v_min, v_max, n_atoms)
     tz = r + disc * (1 - d) * centers.reshape(1, -1)
-    tz = np.minimum(v_max, np.maximum(v_min, tz))
+    tz = np.minimum(O.atom_clip_top(v_min, v_max, n_atoms), np.maximum(v_min, tz))
     b = (tz - v_min) / delta
     l = np.floor(b).astype(np.int64)
     u = np.ceil(b).astype(np.int64)
