@@ -25,28 +25,31 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-static NetDims make_dims(const int* in, const int* out) {
+static NetDims make_dims(const int* in, const int* out, const int* epi) {
   NetDims d{};
   int64_t off = 0;
   for (int l = 0; l < 4; ++l) {
-    d.in[l] = in[l]; d.out[l] = out[l]; d.ld[l] = pitch4(in[l]);
+    d.in[l] = in[l]; d.out[l] = out[l]; d.ld[l] = pitch4(in[l]); d.epi[l] = epi[l];
     d.w_off[l] = off; off = align4(off + int64_t(d.ld[l]) * out[l]);
     d.b_off[l] = off; off = align4(off + out[l]);
   }
   d.total = off;
   return d;
 }
-// models.py:18-23
+// models.py:33-40: fc1 -> relu -> fc2 -> fc2_2 -> relu -> fc3 -> tanh (no relu after fc2, SURVEY.md H9)
 NetDims actor_dims(int obs_dim, int act_dim) {
   const int in[4] = {obs_dim, D4PG_HIDDEN, D4PG_HIDDEN, D4PG_HIDDEN};
   const int out[4] = {D4PG_HIDDEN, D4PG_HIDDEN, D4PG_HIDDEN, act_dim};
-  return make_dims(in, out);
+  const int epi[4] = {EPI_BIAS_RELU, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_TANH};
+  return make_dims(in, out, epi);
 }
-// models.py:56-62
+// models.py:77-83: fc1 -> relu -> cat(., a) -> fc2 -> relu -> fc2_2 -> relu -> fc3, the raw head (fc2 contracts
+// cat(h1, a): in[1] = H + |a|, the action columns from column H on)
 NetDims critic_dims(int obs_dim, int act_dim, int n_atoms) {
   const int in[4] = {obs_dim, D4PG_HIDDEN + act_dim, D4PG_HIDDEN, D4PG_HIDDEN};
   const int out[4] = {D4PG_HIDDEN, D4PG_HIDDEN, D4PG_HIDDEN, n_atoms};
-  return make_dims(in, out);
+  const int epi[4] = {EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS};
+  return make_dims(in, out, epi);
 }
 
 static void fill_layout(const NetDims& d, d4pg_net_layout_t* out) {
@@ -68,6 +71,25 @@ __global__ void softmax_rows_kernel(const float* logits, float* probs, int B, in
   for (int k = lane; k < N; k += 32) s += expf(x[k] - mx);
   s = warp_sum(s);
   for (int k = lane; k < N; k += 32) probs[size_t(warp) * N + k] = expf(x[k] - mx) / s;
+}
+
+// The four forward levels of a network, one grouped launch each.  fc1 reads s [B, in[0]]; the critic's fc2 (a != NULL)
+// also reads the action rows a [B, |a|] as its columns H.. (as learner.cu level_fwd does).  fc1..fc2_2 write the [B, H]
+// planes h1..h3 of `workspace`, fc3 writes y [B, out[3]].
+static int net_forward(const NetDims& d, const float* params, const float* s, const float* a, int B, float* workspace,
+                       float* y, int precision, cudaStream_t st) {
+  const int H = D4PG_HIDDEN, A = a ? d.in[1] - H : 0;
+  float* h[3] = {workspace, workspace + size_t(B) * H, workspace + size_t(B) * 2 * H};
+  for (int l = 0; l < 4; ++l) {
+    const float* X2 = l == 1 ? a : nullptr;
+    GemmBatch b; gemm_batch_begin(b);
+    gemm_batch_add(b, gemm_fwd(l ? h[l - 1] : s, d.in[l] - (X2 ? A : 0), X2, X2 ? A : 0, X2 ? H : 0,
+                               params + d.w_off[l], d.ld[l], params + d.b_off[l], l < 3 ? h[l] : y, d.out[l], B,
+                               d.out[l], d.in[l], d.epi[l]));
+    const int rc = gemm_launch(b, precision, st);
+    if (rc) return rc;
+  }
+  return D4PG_OK;
 }
 
 }  // namespace d4pg
@@ -114,56 +136,27 @@ extern "C" int32_t d4pg_critic_layout(int32_t obs_dim, int32_t act_dim, int32_t 
   return D4PG_OK;
 }
 
-// actor.forward, models.py:32-41: fc1 -> relu -> fc2 -> fc2_2 -> relu -> fc3 -> tanh  (no relu after fc2, H9)
+// actor.forward, models.py:32-41
 extern "C" int32_t d4pg_actor_forward(const float* params, int32_t obs_dim, int32_t act_dim,
                                       const float* s, int32_t B, float* action, float* workspace,
                                       int32_t precision, d4pg_stream_t stream) {
   D4PG_REQUIRE(params && s && action && workspace && B > 0, D4PG_EINVAL, "d4pg_actor_forward: null/empty argument");
   D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_actor_forward: unknown precision %d", precision);
-  const NetDims d = actor_dims(obs_dim, act_dim);
-  const int H = D4PG_HIDDEN;
-  float* h1 = workspace; float* h2 = h1 + size_t(B) * H; float* h3 = h2 + size_t(B) * H;
-  cudaStream_t st = as_stream(stream);
-  const float* X[4] = {s, h1, h2, h3};
-  float* Y[4] = {h1, h2, h3, action};
-  const int epi[4] = {EPI_BIAS_RELU, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_TANH};
-  for (int l = 0; l < 4; ++l) {
-    GemmBatch b; gemm_batch_begin(b);
-    gemm_batch_add(b, gemm_fwd(X[l], d.in[l], nullptr, 0, 0, params + d.w_off[l], d.ld[l], params + d.b_off[l],
-                               Y[l], d.out[l], B, d.out[l], d.in[l], epi[l]));
-    int rc = gemm_launch(b, precision, st);
-    if (rc) return rc;
-  }
-  return D4PG_OK;
+  return net_forward(actor_dims(obs_dim, act_dim), params, s, nullptr, B, workspace, action, precision, as_stream(stream));
 }
 
-// critic.forward, models.py:76-88: fc1 -> relu -> cat(.,a) -> fc2 -> relu -> fc2_2 -> relu -> fc3 -> softmax
+// critic.forward, models.py:76-88: the raw head, then softmax
 extern "C" int32_t d4pg_critic_forward(const float* params, int32_t obs_dim, int32_t act_dim, int32_t n_atoms,
                                        const float* s, const float* a, int32_t B, float* probs, float* logits,
                                        float* workspace, int32_t precision, d4pg_stream_t stream) {
   D4PG_REQUIRE(params && s && a && workspace && B > 0 && (probs || logits), D4PG_EINVAL, "d4pg_critic_forward: null/empty argument");
   D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_critic_forward: unknown precision %d", precision);
   D4PG_REQUIRE(n_atoms >= 2 && n_atoms <= D4PG_MAX_ATOMS, D4PG_EINVAL, "d4pg_critic_forward: n_atoms out of range");
-  const NetDims d = critic_dims(obs_dim, act_dim, n_atoms);
-  const int H = D4PG_HIDDEN;
-  float* h1 = workspace; float* h2 = h1 + size_t(B) * H; float* h3 = h2 + size_t(B) * H;
-  // logits scratch lives behind h3 when the caller only wants probabilities
-  float* z = logits ? logits : h1;   // h1 is dead after fc2
+  // the logits go to h1 when the caller only wants probabilities: h1 is dead after fc2
+  float* z = logits ? logits : workspace;
   cudaStream_t st = as_stream(stream);
-  int rc;
-  GemmBatch b;
-  gemm_batch_begin(b);
-  gemm_batch_add(b, gemm_fwd(s, obs_dim, nullptr, 0, 0, params + d.w_off[0], d.ld[0], params + d.b_off[0], h1, H, B, H, obs_dim, EPI_BIAS_RELU));
-  if ((rc = gemm_launch(b, precision, st))) return rc;
-  gemm_batch_begin(b);
-  gemm_batch_add(b, gemm_fwd(h1, H, a, act_dim, H, params + d.w_off[1], d.ld[1], params + d.b_off[1], h2, H, B, H, H + act_dim, EPI_BIAS_RELU));
-  if ((rc = gemm_launch(b, precision, st))) return rc;
-  gemm_batch_begin(b);
-  gemm_batch_add(b, gemm_fwd(h2, H, nullptr, 0, 0, params + d.w_off[2], H, params + d.b_off[2], h3, H, B, H, H, EPI_BIAS_RELU));
-  if ((rc = gemm_launch(b, precision, st))) return rc;
-  gemm_batch_begin(b);
-  gemm_batch_add(b, gemm_fwd(h3, H, nullptr, 0, 0, params + d.w_off[3], H, params + d.b_off[3], z, n_atoms, B, n_atoms, H, EPI_BIAS));
-  if ((rc = gemm_launch(b, precision, st))) return rc;
+  const int rc = net_forward(critic_dims(obs_dim, act_dim, n_atoms), params, s, a, B, workspace, z, precision, st);
+  if (rc) return rc;
   if (probs) {
     softmax_rows_kernel<<<cdiv(B * 32, 256), 256, 0, st>>>(z, probs, B, n_atoms);
     D4PG_LAUNCH_OK();

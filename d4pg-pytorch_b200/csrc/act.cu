@@ -198,9 +198,8 @@ extern "C" int32_t d4pg_act(const float* actor_params, int32_t obs_dim, int32_t 
 
   const NetDims d = actor_dims(obs_dim, act_dim);
   ActArgs a{};
-  const int epi[ACT_SLOTS] = {EPI_BIAS_RELU, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_TANH};     // models.py:32-41
   for (int l = 0; l < ACT_SLOTS; ++l) {
-    a.slot[l] = chain_fwd(actor_params + d.w_off[l], d.ld[l], actor_params + d.b_off[l], d.out[l], d.in[l], epi[l],
+    a.slot[l] = chain_fwd(actor_params + d.w_off[l], d.ld[l], actor_params + d.b_off[l], d.out[l], d.in[l], d.epi[l],
                           nullptr, 0, l + 1 < ACT_SLOTS);
     if (l > 0) chain_src_plane(a.slot[l], l - 1);
   }

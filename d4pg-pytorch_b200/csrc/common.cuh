@@ -127,13 +127,25 @@ struct Philox {
 };
 
 // ---- network layout ------------------------------------------------------------------
+// GEMM epilogues: a forward layer's bias + activation, or the activation derivative a dX applies to its output
+enum GemmEpi {
+  EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_RELU = 2, EPI_BIAS_TANH = 3,
+  EPI_RELU_MASK = 4,   // C *= (aux > 0)
+  EPI_TANH_MASK = 5    // C *= (1 - aux^2)
+};
 struct NetDims {
   int in[4], out[4];        // per layer fc1, fc2, fc2_2, fc3
   int ld[4];                // row pitch of each weight matrix in floats: in[] rounded up to 4 (16-B rows,
                             // so every operand is TMA- and float4-addressable); pad columns stay zero
+  int epi[4];               // forward epilogue of each layer
   int64_t w_off[4], b_off[4];
   int64_t total;
 };
+// The mask the dX of layer l applies to its input: the derivative of the activation that produced that input.  A ReLU
+// on layer l-1 gives (input > 0); no activation (the actor's fc2), or the network input (l = 0), gives none.
+static inline int dx_mask(const NetDims& d, int l) {
+  return l > 0 && d.epi[l - 1] == EPI_BIAS_RELU ? EPI_RELU_MASK : EPI_NONE;
+}
 __host__ __device__ static inline int pitch4(int x) { return (x + 3) & ~3; }
 NetDims actor_dims(int obs_dim, int act_dim);
 NetDims critic_dims(int obs_dim, int act_dim, int n_atoms);

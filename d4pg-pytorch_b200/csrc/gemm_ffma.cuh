@@ -10,12 +10,6 @@ enum GemmMode {
   GEMM_DX = 1,    // C[M,N] = dZ[M,K] . W[K,N]    (* act')         autograd of the above, ddpg.py:230,242
   GEMM_DW = 2     // C[M,N] = dZ[K,M]^T . X[K,N]  (+ column sums -> bias grad)
 };
-enum GemmEpi {
-  EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_RELU = 2, EPI_BIAS_TANH = 3,
-  EPI_RELU_MASK = 4,   // C *= (aux > 0)
-  EPI_TANH_MASK = 5    // C *= (1 - aux^2)
-};
-
 struct GemmProblem {
   const float* A; const float* A2; const float* Bm; const float* bias; const float* aux;
   float* C; float* bias_grad;

@@ -218,11 +218,7 @@ static Layer layer(const d4pg_learner* L, Net net, int l) {
   const bool critic = net >= CRITIC;
   const NetDims& d = critic ? L->dc : L->da;
   const float* P[4] = {L->buf.actor, L->buf.actor_target, L->buf.critic, L->buf.critic_target};
-  // actor (models.py:33-40): fc2 has no activation, fc3 ends in tanh; critic (models.py:77-83): fc2 contracts
-  // cat(h1, a) (k_in = H + |a|), fc3 gives the raw head
-  const int epi_actor[4] = {EPI_BIAS_RELU, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_TANH};
-  const int epi_critic[4] = {EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS_RELU, EPI_BIAS};
-  return Layer{P[net] + d.w_off[l], d.ld[l], P[net] + d.b_off[l], d.out[l], d.in[l], (critic ? epi_critic : epi_actor)[l]};
+  return Layer{P[net] + d.w_off[l], d.ld[l], P[net] + d.b_off[l], d.out[l], d.in[l], d.epi[l]};
 }
 // critic fc2's action columns start H floats into each row of its weight (and weight-gradient) matrix
 static int64_t critic_fc2_action_off(const d4pg_learner* L) { return L->dc.w_off[1] + D4PG_HIDDEN; }

@@ -49,21 +49,47 @@ __global__ void head_backward_kernel(const float* __restrict__ y, const float* _
 int launch_mog_head_backward(const float* raw, int ldr, const float* gw, const float* gmu, const float* gsig, int B, int K,
                              float* dz, int ldz, cudaStream_t st);      // mog_heads.cu
 
-static int launch_level(GemmBatch& b, int precision, cudaStream_t st) {
-  return b.n ? gemm_launch(b, precision, st) : D4PG_OK;
+// The levels fc3 -> fc2_2 -> fc2 -> fc1 of a network from the output layer's dZ plane `dz` [B, pitch4(out[3])], held in
+// scratch behind the two [B, H] delta planes p0 / p1, which the levels use in turn.  Level l is one grouped launch: the
+// dX of layer l (masked by dx_mask) and the dW of layer l with its bias gradient.  The critic's fc2 (a != NULL) adds its
+// action columns W2[:, H:]: dX = grad_a, dW without bias.  grad_params is cleared first (pads stay zero; split-K dW
+// adds); a NULL gradient drops the problems that only it needs.  The caller checked the arguments.
+static int net_backward(const NetDims& d, const float* params, const float* s, const float* a, int B,
+                        const float* workspace, const float* dz, float* grad_params, float* grad_s, float* grad_a,
+                        float* scratch, int precision, cudaStream_t st) {
+  const int H = D4PG_HIDDEN, A = a ? d.in[1] - H : 0;
+  const float* h[3] = {workspace, workspace + size_t(B) * H, workspace + size_t(B) * 2 * H};
+  float* p[2] = {scratch, scratch + size_t(B) * H};
+  const float* W = params; float* G = grad_params;
+  if (G) D4PG_CUDA_OK(cudaMemsetAsync(G, 0, size_t(d.total) * sizeof(float), st));
+  for (int l = 3; l >= 0; --l) {
+    // level l reads the dZ level l+1 wrote (p0 from fc3, p1 from fc2_2, p0 from fc2) and writes the other plane
+    const float* Z = l == 3 ? dz : p[l % 2];
+    const int ldz = l == 3 ? pitch4(d.out[3]) : H;
+    const float* X = l ? h[l - 1] : s;
+    const int n_in = l ? H : d.in[0], mask = dx_mask(d, l);
+    float* dX = l ? p[(l + 1) % 2] : grad_s;
+    GemmBatch g; gemm_batch_begin(g);
+    if (dX && (l != 1 || G || grad_s))     // fc2's dX (fc1's dZ) feeds only dW1 and grad_s
+      gemm_batch_add(g, gemm_dx(Z, ldz, W + d.w_off[l], d.ld[l], dX, n_in, B, n_in, d.out[l], mask,
+                                mask == EPI_NONE ? nullptr : X, mask == EPI_NONE ? 0 : n_in));
+    if (l == 1 && grad_a)
+      gemm_batch_add(g, gemm_dx(Z, ldz, W + d.w_off[1] + H, d.ld[1], grad_a, A, B, A, H, EPI_NONE, nullptr, 0));
+    if (G) gemm_batch_add(g, gemm_dw(Z, ldz, X, n_in, G + d.w_off[l], d.ld[l], G + d.b_off[l], d.out[l], n_in, B));
+    if (l == 1 && G && a) gemm_batch_add(g, gemm_dw(Z, ldz, a, A, G + d.w_off[1] + H, d.ld[1], nullptr, H, A, B));
+    if (g.n) {
+      const int rc = gemm_launch(g, precision, st);
+      if (rc) return rc;
+    }
+  }
+  return D4PG_OK;
 }
 
 }  // namespace d4pg
 
 using namespace d4pg;
 
-#define RUN_LEVEL(b)                                       \
-  do {                                                     \
-    const int _rc = launch_level(b, precision, st);        \
-    if (_rc) return _rc;                                   \
-  } while (0)
-
-// actor: fc1 -> relu -> fc2 -> fc2_2 -> relu -> fc3 -> tanh (no relu after fc2, H9).  Levels fc3 -> fc2_2 -> fc2 -> fc1.
+// actor: tanh' into the fc3 dZ plane, then the levels
 extern "C" int32_t d4pg_actor_backward(const float* params, int32_t obs_dim, int32_t act_dim, const float* s, int32_t B,
                                        const float* action, const float* workspace, const float* grad_action,
                                        float* grad_params, float* grad_s, float* scratch, int32_t precision,
@@ -71,87 +97,17 @@ extern "C" int32_t d4pg_actor_backward(const float* params, int32_t obs_dim, int
   D4PG_REQUIRE(params && s && action && workspace && grad_action && scratch && B > 0 && obs_dim > 0 && act_dim > 0,
                D4PG_EINVAL, "d4pg_actor_backward: null/empty argument");
   D4PG_REQUIRE(precision >= 0 && precision <= 3, D4PG_ENOTSUP, "d4pg_actor_backward: unknown precision %d", precision);
-  const NetDims d = actor_dims(obs_dim, act_dim);
-  const int H = D4PG_HIDDEN, S = obs_dim, A = act_dim, Ap = pitch4(act_dim);
-  const float* h1 = workspace; const float* h2 = h1 + size_t(B) * H; const float* h3 = h2 + size_t(B) * H;
-  // two delta planes + the head plane [B, Ap] (scratch holds B*(2H + max(H, Ap)) floats: act_dim may exceed H)
-  float* p0 = scratch; float* p1 = p0 + size_t(B) * H; float* dz3 = p1 + size_t(B) * H;
-  const float* W = params; float* G = grad_params;
+  if (!grad_params && !grad_s) return D4PG_OK;
+  // scratch holds B*(2H + max(H, Ap)) floats: the fc3 dZ plane [B, Ap] may be wider than H
+  float* dz = scratch + size_t(B) * 2 * D4PG_HIDDEN;
   cudaStream_t st = as_stream(stream);
-  if (!G && !grad_s) return D4PG_OK;
-  if (G) D4PG_CUDA_OK(cudaMemsetAsync(G, 0, size_t(d.total) * sizeof(float), st));   // pads stay zero; split-K dW adds
-
-  head_backward_kernel<<<cdiv(B * 32, 256), 256, 0, st>>>(action, grad_action, nullptr, dz3, B, A, Ap, 0);
+  head_backward_kernel<<<cdiv(B * 32, 256), 256, 0, st>>>(action, grad_action, nullptr, dz, B, act_dim, pitch4(act_dim), 0);
   D4PG_LAUNCH_OK();
-  GemmBatch g;
-  // fc3: dz22 = (dz3 W3) * (h3 > 0);  dW3 = dz3^T h3
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(dz3, Ap, W + d.w_off[3], d.ld[3], p0, H, B, H, A, EPI_RELU_MASK, h3, H));
-  if (G) gemm_batch_add(g, gemm_dw(dz3, Ap, h3, H, G + d.w_off[3], d.ld[3], G + d.b_off[3], A, H, B));
-  RUN_LEVEL(g);
-  // fc2_2: its input h2 has no activation -> plain dX
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(p0, H, W + d.w_off[2], d.ld[2], p1, H, B, H, H, EPI_NONE, nullptr, 0));
-  if (G) gemm_batch_add(g, gemm_dw(p0, H, h2, H, G + d.w_off[2], d.ld[2], G + d.b_off[2], H, H, B));
-  RUN_LEVEL(g);
-  // fc2
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(p1, H, W + d.w_off[1], d.ld[1], p0, H, B, H, H, EPI_RELU_MASK, h1, H));
-  if (G) gemm_batch_add(g, gemm_dw(p1, H, h1, H, G + d.w_off[1], d.ld[1], G + d.b_off[1], H, H, B));
-  RUN_LEVEL(g);
-  // fc1: d state, dW1 = dz1^T s
-  gemm_batch_begin(g);
-  if (grad_s) gemm_batch_add(g, gemm_dx(p0, H, W + d.w_off[0], d.ld[0], grad_s, S, B, S, H, EPI_NONE, nullptr, 0));
-  if (G) gemm_batch_add(g, gemm_dw(p0, H, s, S, G + d.w_off[0], d.ld[0], G + d.b_off[0], H, S, B));
-  RUN_LEVEL(g);
-  return D4PG_OK;
+  return net_backward(actor_dims(obs_dim, act_dim), params, s, nullptr, B, workspace, dz, grad_params, grad_s, nullptr,
+                      scratch, precision, st);
 }
 
-// the critic's levels fc3 -> fc2_2 -> fc2 -> fc1 from the output layer's dZ plane `dz` [B, pitch4(N)] (held in scratch
-// behind the two delta planes); the caller checked the arguments
-static int critic_levels(const float* params, int obs_dim, int act_dim, int n_atoms, const float* s, const float* a, int B,
-                         const float* workspace, const float* dz, float* grad_params, float* grad_s, float* grad_a,
-                         float* scratch, int precision, cudaStream_t st) {
-  const NetDims d = critic_dims(obs_dim, act_dim, n_atoms);
-  const int H = D4PG_HIDDEN, S = obs_dim, A = act_dim, N = n_atoms, Np = pitch4(n_atoms);
-  const float* h1 = workspace; const float* h2 = h1 + size_t(B) * H; const float* h3 = h2 + size_t(B) * H;
-  float* p0 = scratch; float* p1 = p0 + size_t(B) * H;
-  const float* W = params; float* G = grad_params;
-  if (!G && !grad_s && !grad_a) return D4PG_OK;
-  if (G) D4PG_CUDA_OK(cudaMemsetAsync(G, 0, size_t(d.total) * sizeof(float), st));
-  const bool need_dz1 = G || grad_s;
-
-  GemmBatch g;
-  // fc3
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(dz, Np, W + d.w_off[3], d.ld[3], p0, H, B, H, N, EPI_RELU_MASK, h3, H));
-  if (G) gemm_batch_add(g, gemm_dw(dz, Np, h3, H, G + d.w_off[3], d.ld[3], G + d.b_off[3], N, H, B));
-  RUN_LEVEL(g);
-  // fc2_2
-  gemm_batch_begin(g);
-  gemm_batch_add(g, gemm_dx(p0, H, W + d.w_off[2], d.ld[2], p1, H, B, H, H, EPI_RELU_MASK, h2, H));
-  if (G) gemm_batch_add(g, gemm_dw(p0, H, h2, H, G + d.w_off[2], d.ld[2], G + d.b_off[2], H, H, B));
-  RUN_LEVEL(g);
-  // fc2: dh1 (masked), d action, dW2 = [dz2^T h1 | dz2^T a]
-  gemm_batch_begin(g);
-  if (need_dz1) gemm_batch_add(g, gemm_dx(p1, H, W + d.w_off[1], d.ld[1], p0, H, B, H, H, EPI_RELU_MASK, h1, H));
-  if (grad_a) gemm_batch_add(g, gemm_dx(p1, H, W + d.w_off[1] + H, d.ld[1], grad_a, A, B, A, H, EPI_NONE, nullptr, 0));
-  if (G) gemm_batch_add(g, gemm_dw(p1, H, h1, H, G + d.w_off[1], d.ld[1], G + d.b_off[1], H, H, B));
-  if (G) gemm_batch_add(g, gemm_dw(p1, H, a, A, G + d.w_off[1] + H, d.ld[1], nullptr, H, A, B));
-  RUN_LEVEL(g);
-  // fc1
-  if (need_dz1) {
-    gemm_batch_begin(g);
-    if (grad_s) gemm_batch_add(g, gemm_dx(p0, H, W + d.w_off[0], d.ld[0], grad_s, S, B, S, H, EPI_NONE, nullptr, 0));
-    if (G) gemm_batch_add(g, gemm_dw(p0, H, s, S, G + d.w_off[0], d.ld[0], G + d.b_off[0], H, S, B));
-    RUN_LEVEL(g);
-  }
-  return D4PG_OK;
-}
-
-// critic: fc1 -> relu -> cat(., a) -> fc2 -> relu -> fc2_2 -> relu -> fc3 -> softmax.  Levels fc3 -> fc2_2 -> fc2 -> fc1;
-// fc2 splits into its h1 columns (dX masked by h1 > 0, dW with the bias gradient) and its action columns W2[:, H:]
-// (dX = d action, dW without bias).
+// critic: the softmax Jacobian (or the logits' own gradient) into the fc3 dZ plane, then the levels
 extern "C" int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, int32_t act_dim, int32_t n_atoms,
                                         const float* s, const float* a, int32_t B, const float* probs,
                                         const float* workspace, const float* grad_probs, const float* grad_logits,
@@ -168,8 +124,8 @@ extern "C" int32_t d4pg_critic_backward(const float* params, int32_t obs_dim, in
   if (!grad_params && !grad_s && !grad_a) return D4PG_OK;
   head_backward_kernel<<<cdiv(B * 32, 256), 256, 0, as_stream(stream)>>>(probs, grad_probs, grad_logits, dz, B, n_atoms, Np, 1);
   D4PG_LAUNCH_OK();
-  return critic_levels(params, obs_dim, act_dim, n_atoms, s, a, B, workspace, dz, grad_params, grad_s, grad_a, scratch,
-                       precision, as_stream(stream));
+  return net_backward(critic_dims(obs_dim, act_dim, n_atoms), params, s, a, B, workspace, dz, grad_params, grad_s, grad_a,
+                      scratch, precision, as_stream(stream));
 }
 
 // mixture-of-Gaussians critic (mog_heads.cu): the raw head's dZ from (g_w, g_mu, g_sigma), then the same levels
@@ -188,6 +144,6 @@ extern "C" int32_t d4pg_critic_backward_mog(const float* params, int32_t obs_dim
   float* dz = scratch + size_t(B) * 2 * D4PG_HIDDEN;
   const int rc = launch_mog_head_backward(raw, N, grad_w, grad_mu, grad_sigma, B, K, dz, pitch4(N), as_stream(stream));
   if (rc) return rc;
-  return critic_levels(params, obs_dim, act_dim, N, s, a, B, workspace, dz, grad_params, grad_s, grad_a, scratch,
-                       precision, as_stream(stream));
+  return net_backward(critic_dims(obs_dim, act_dim, N), params, s, a, B, workspace, dz, grad_params, grad_s, grad_a,
+                      scratch, precision, as_stream(stream));
 }

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .models import actor, critic
+from .models import CriticHead, actor, critic
 from .obs_norm import make_obs_normalizer
 from .prioritized_replay_memory import LinearSchedule, PrioritizedReplayBuffer, check_her_params
 from .random_process import AdaptiveParamNoiseSpec, GaussianNoise, OrnsteinUhlenbeckProcess
@@ -58,12 +58,10 @@ class _Learner(object):
         B = ddpg.batch_size
         cfg = _lib.LearnerConfig()
         cfg.obs_dim, cfg.act_dim, cfg.n_atoms, cfg.batch = ddpg.obs_dim, ddpg.act_dim, ddpg.n_atoms, B
-        if ddpg.n_components is not None:       # mixture critic: n_atoms / v_min / v_max are ignored by the library
-            cfg.dist_type, cfg.n_components, cfg.v_min, cfg.v_max = 1, ddpg.n_components, 0.0, 0.0
-        elif ddpg.n_quantiles is not None:      # quantile critic: n_atoms = N quantiles, v_min / v_max are ignored
-            cfg.dist_type, cfg.qr_kappa, cfg.v_min, cfg.v_max = 2, ddpg.qr_kappa, 0.0, 0.0
-        else:
-            cfg.v_min, cfg.v_max = float(ddpg.v_min), float(ddpg.v_max)
+        # n_atoms is the head width (3K for a mixture); the library reads v_min / v_max only for a categorical head
+        head = ddpg.critic_head
+        cfg.dist_type, cfg.n_components, cfg.qr_kappa = head.code, head.n_components or 0, head.kappa or 0.0
+        cfg.v_min, cfg.v_max = (float(head.v_min), float(head.v_max)) if head.kind == "categorical" else (0.0, 0.0)
         cfg.gamma = float(ddpg.gamma)
         cfg.n_steps = int(ddpg.n_steps)
         cfg.proj_mode = 1 if ddpg.projection == "nstep" else 0
@@ -272,37 +270,14 @@ class DDPG:
             raise _lib.D4PGError("obs_norm is not supported with a communicator of world size > 1: each rank would "
                                  "normalize with the statistics of its own replay shard")
 
-        self.dist_type = critic_dist_info["type"]
-        self.n_quantiles = self.qr_kappa = None
-        if self.dist_type == "quantile":
-            # {"type": "quantile", "n_quantiles": N, "kappa": 1.0}: quantile regression (QR-DQN).  The critic's fc3 gives
-            # N quantiles at tau_k = (2k+1) / (2N); the critic loss is the quantile-Huber loss against the N bootstrapped
-            # target quantiles (csrc/qr_heads.cu); td = mean(theta) - (r + c mean(theta')).  Validated by the critic.
-            self.n_components = None
-            self.n_quantiles = int(critic_dist_info["n_quantiles"])
-            self.qr_kappa = float(critic_dist_info.get("kappa", 1.0))
-            self.v_min = self.v_max = self.delta = self.bin_centers = None
-            self.n_atoms = self.n_quantiles
-        elif self.dist_type == "mixture_of_gaussian":
-            # {"type": "mixture_of_gaussian", "n_components": K}: the reference stubs this branch (ddpg.py:48-50).  The
-            # critic loss is the cross-entropy of the online mixture under the target mixture, integrated with 8
-            # Gauss-Hermite nodes per target component (csrc/mog_heads.cu); td = E[Q] - (r + c E[Q']).
-            if priority == "ce":
-                raise _lib.D4PGError('priority="ce" is not supported with a mixture_of_gaussian critic: the '
-                                     'cross-entropy of a density can be negative')
-            self.n_components = int(critic_dist_info["n_components"])
-            self.v_min = self.v_max = self.delta = self.bin_centers = None
-            self.n_atoms = 3 * self.n_components        # raw head width of the critic's fc3
-        elif self.dist_type == "categorical":
-            self.n_components = None
-            self.v_min = critic_dist_info["v_min"]
-            self.v_max = critic_dist_info["v_max"]
-            self.n_atoms = critic_dist_info["n_atoms"]
-            self.delta = (self.v_max - self.v_min) / float(self.n_atoms - 1)
-            self.bin_centers = np.array([self.v_min + i * self.delta for i in range(self.n_atoms)]).reshape(-1, 1)
-        else:
-            raise NotImplementedError("critic_dist_info['type'] must be 'categorical', 'mixture_of_gaussian' or "
-                                      "'quantile', got %r" % (self.dist_type,))
+        # the critic head (models.CriticHead); the critic built below checks its ranges
+        if priority == "ce" and critic_dist_info["type"] == "mixture_of_gaussian":
+            raise _lib.D4PGError('priority="ce" is not supported with a mixture_of_gaussian critic: the '
+                                 'cross-entropy of a density can be negative')
+        head = self.critic_head = CriticHead(critic_dist_info, learner=True)
+        self.dist_type, self.n_atoms, self.n_components = head.kind, head.width, head.n_components
+        self.n_quantiles, self.qr_kappa = head.n_quantiles, head.kappa
+        self.v_min, self.v_max, self.delta, self.bin_centers = head.v_min, head.v_max, head.delta, head.bin_centers
 
         # networks, built in the reference's order so a seeded RNG yields the same weights (ddpg.py:56-64)
         self.actor = actor(input_size=obs_dim, output_size=act_dim, device=self.device)

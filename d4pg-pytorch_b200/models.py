@@ -187,10 +187,15 @@ class _FlatNet(nn.Module):
             self._ws = ws
         return ws
 
-    def _as_input(self, x, width):
+    def _input(self, x, width, grad):
+        """An input as the kernels take it: [B, width] contiguous fp32 on this module's device.  With `grad` the
+        conversion stays on the autograd graph (no detach)."""
+        if grad and self._flat.device.type != "cuda":
+            raise _lib.D4PGError("the D4PG kernels run only on a CUDA device (sm_90a); this module lives on %s"
+                                 % self._flat.device)
         if not torch.is_tensor(x):
             x = torch.as_tensor(np.asarray(x))
-        x = x.detach().to(device=self._flat.device, dtype=torch.float32)
+        x = (x if grad else x.detach()).to(device=self._flat.device, dtype=torch.float32)
         if x.dim() == 1:
             x = x.view(1, -1)
         assert x.shape[1] == width, "expected input width %d, got %s" % (width, tuple(x.shape))
@@ -199,7 +204,7 @@ class _FlatNet(nn.Module):
     def _state_input(self, state, width, grad):
         """The `state` input as the kernels take it: through the observation normalizer when one is attached (on the
         autograd graph when `grad`)."""
-        x = self._as_grad_input(state, width) if grad else self._as_input(state, width)
+        x = self._input(state, width, grad)
         norm = self.obs_normalizer
         if norm is None:
             return x
@@ -227,27 +232,18 @@ class _FlatNet(nn.Module):
             self.flat_grads()
         return params
 
-    def _as_grad_input(self, x, width):
-        """_as_input without the detach: the device / dtype conversion stays on the autograd graph."""
-        if self._flat.device.type != "cuda":
-            raise _lib.D4PGError("the D4PG kernels run only on a CUDA device (sm_90a); this module lives on %s"
-                                 % self._flat.device)
-        if not torch.is_tensor(x):
-            x = torch.as_tensor(np.asarray(x))
-        x = x.to(device=self._flat.device, dtype=torch.float32)
-        if x.dim() == 1:
-            x = x.view(1, -1)
-        assert x.shape[1] == width, "expected input width %d, got %s" % (width, tuple(x.shape))
-        return x.contiguous()
-
 
 class actor(_FlatNet):
     """models.py:15-41.  fc1 -> ReLU -> fc2 -> fc2_2 -> ReLU -> fc3 -> tanh
     (no ReLU between fc2 and fc2_2, SURVEY.md H9)."""
 
+    @staticmethod
+    def _layers(input_size, output_size):
+        return [(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)]
+
     def __init__(self, input_size, output_size, device=None, differentiable=False):
         self.input_size, self.output_size = input_size, output_size
-        super().__init__([(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)], device)
+        super().__init__(self._layers(input_size, output_size), device)
         self.differentiable = bool(differentiable)
         self.init_weights()
 
@@ -257,8 +253,7 @@ class actor(_FlatNet):
         fills completely (DDPG.perturbed_actor)."""
         net = cls.__new__(cls)
         net.input_size, net.output_size = input_size, output_size
-        _FlatNet.__init__(net, [(input_size, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, HIDDEN), (HIDDEN, output_size)], device,
-                          empty=True)
+        _FlatNet.__init__(net, cls._layers(input_size, output_size), device, empty=True)
         return net
 
     def init_weights(self, init_w=10e-3):
@@ -280,6 +275,52 @@ class actor(_FlatNet):
         return out
 
 
+class CriticHead(object):
+    """`critic_dist_info` parsed and validated once; the critic module, DDPG and the learner read the head from here.
+
+    kind: "categorical", "mixture_of_gaussian" or "quantile"; width: fc3's output width (N atoms, 3K, N quantiles);
+    code: the learner's dist_type (0, 1, 2); n_components (K), n_quantiles (N) and kappa: None where the kind has none.
+    v_min, v_max, delta and bin_centers: a categorical head's support, None elsewhere.
+
+    learner=True parses the head as DDPG needs it for its learner: with the categorical support (a critic module has
+    none), and without the range checks.  DDPG parses its head before it builds any network and the critic it builds
+    makes those checks, which keeps the order in which a config's faults are reported."""
+
+    def __init__(self, dist_info, learner=False):
+        self.kind = dist_info["type"]
+        self.n_components = self.n_quantiles = self.kappa = None
+        self.v_min = self.v_max = self.delta = self.bin_centers = None
+        if self.kind == "quantile":
+            # QR-DQN: fc3 gives N quantiles at tau_k = (2k+1) / (2N); the learner's loss is the quantile-Huber loss
+            # against the N bootstrapped target quantiles (csrc/qr_heads.cu); td = mean(theta) - (r + c mean(theta'))
+            self.code = 2
+            self.n_quantiles = self.width = int(dist_info["n_quantiles"])
+            if not learner and not 2 <= self.n_quantiles <= _lib.MAX_ATOMS:
+                raise _lib.D4PGError("n_quantiles must be in [2, %d], got %d" % (_lib.MAX_ATOMS, self.n_quantiles))
+            self.kappa = float(dist_info.get("kappa", 1.0))
+            if not learner and not (math.isfinite(self.kappa) and self.kappa > 0.0):
+                raise _lib.D4PGError("kappa must be finite and > 0, got %r" % (self.kappa,))
+        elif self.kind == "mixture_of_gaussian":
+            # the reference stubs this branch (ddpg.py:48-50).  The learner's loss is the cross-entropy of the online
+            # mixture under the target mixture, integrated with 8 Gauss-Hermite nodes per target component
+            # (csrc/mog_heads.cu); td = E[Q] - (r + c E[Q'])
+            self.code = 1
+            self.n_components = int(dist_info["n_components"])
+            if not learner and not 1 <= self.n_components <= _lib.MAX_COMPONENTS:
+                raise _lib.D4PGError("n_components must be in [1, %d], got %d" % (_lib.MAX_COMPONENTS, self.n_components))
+            self.width = 3 * self.n_components          # raw head: K weight logits, K means, K sigma pre-activations
+        elif self.kind == "categorical":
+            self.code = 0
+            if learner:
+                self.v_min, self.v_max, n = dist_info["v_min"], dist_info["v_max"], dist_info["n_atoms"]
+                self.delta = (self.v_max - self.v_min) / float(n - 1)
+                self.bin_centers = np.array([self.v_min + i * self.delta for i in range(n)]).reshape(-1, 1)
+            self.width = int(dist_info["n_atoms"])
+        else:
+            raise NotImplementedError("critic_dist_info['type'] must be 'categorical', 'mixture_of_gaussian' or "
+                                      "'quantile', got %r" % (self.kind,))
+
+
 class critic(_FlatNet):
     """models.py:51-88.  fc1 -> ReLU -> cat(., action) -> fc2 -> ReLU -> fc2_2 -> ReLU -> fc3 -> softmax.
 
@@ -294,29 +335,10 @@ class critic(_FlatNet):
 
     def __init__(self, state_size, action_size, dist_info, device=None, differentiable=False):
         self.dist_info = dist_info
-        self.dist_type = dist_info["type"]
-        self.n_quantiles = self.kappa = None
-        if self.dist_type == "quantile":
-            self.n_components = None
-            self.n_quantiles = int(dist_info["n_quantiles"])
-            if not 2 <= self.n_quantiles <= _lib.MAX_ATOMS:
-                raise _lib.D4PGError("n_quantiles must be in [2, %d], got %d" % (_lib.MAX_ATOMS, self.n_quantiles))
-            self.kappa = float(dist_info.get("kappa", 1.0))
-            if not (math.isfinite(self.kappa) and self.kappa > 0.0):
-                raise _lib.D4PGError("kappa must be finite and > 0, got %r" % (self.kappa,))
-            head = self.n_quantiles
-        elif self.dist_type == "mixture_of_gaussian":
-            self.n_components = int(dist_info["n_components"])
-            if not 1 <= self.n_components <= _lib.MAX_COMPONENTS:
-                raise _lib.D4PGError("n_components must be in [1, %d], got %d" % (_lib.MAX_COMPONENTS, self.n_components))
-            head = 3 * self.n_components
-        elif self.dist_type == "categorical":
-            self.n_components = None
-            head = int(dist_info["n_atoms"])
-        else:
-            raise NotImplementedError("critic_dist_info['type'] must be 'categorical', 'mixture_of_gaussian' or "
-                                      "'quantile', got %r" % (self.dist_type,))
-        self.state_size, self.action_size, self.n_atoms = state_size, action_size, head
+        self.head = CriticHead(dist_info)
+        self.dist_type, self.n_components = self.head.kind, self.head.n_components
+        self.n_quantiles, self.kappa = self.head.n_quantiles, self.head.kappa
+        self.state_size, self.action_size, self.n_atoms = state_size, action_size, self.head.width
         super().__init__([(state_size, HIDDEN), (HIDDEN + action_size, HIDDEN), (HIDDEN, HIDDEN),
                           (HIDDEN, self.n_atoms)], device)
         self.differentiable = bool(differentiable)
@@ -331,64 +353,83 @@ class critic(_FlatNet):
         [B, 3K] as a fourth element with return_logits).  Quantile: theta [B, N], which already is the raw fc3 output
         (return_logits is ignored)."""
         _lib.require_cuda()
-        if self.n_components is not None:
-            return self._forward_mog(state, action, return_logits)
+        grad = self._use_autograd((state, action))
+        x = self._state_input(state, self.state_size, grad)
+        a = self._input(action, self.action_size, grad)
+        if grad:
+            outs = _CriticFn.apply(self, int(self.precision), x, a, *self._grad_params())
+        else:
+            outs = self._head_outputs(x.shape[0], x.device, return_logits)
+            self._head_forward(self._flat, x, a, outs, self._workspace(x.shape[0]), int(self.precision))
         if self.n_quantiles is not None:
-            return self._forward_qr(state, action)
-        if self._use_autograd((state, action)):
-            x = self._state_input(state, self.state_size, True)
-            a = self._as_grad_input(action, self.action_size)
-            probs, logits = _CriticFn.apply(self, int(self.precision), x, a, *self._grad_params())
-            return (probs, logits) if return_logits else probs
-        x = self._state_input(state, self.state_size, False)
-        a = self._as_input(action, self.action_size)
-        B = x.shape[0]
-        probs = torch.empty(B, self.n_atoms, dtype=torch.float32, device=x.device)
-        logits = torch.empty_like(probs) if return_logits else None
-        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(self._flat), self.state_size, self.action_size, self.n_atoms,
-                                                  _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(probs), _lib.ptr(logits),
-                                                  _lib.ptr(self._workspace(B)), int(self.precision), _lib.stream_ptr()),
-                   "d4pg_critic_forward")
-        return (probs, logits) if return_logits else probs
+            return outs[0]
+        if return_logits:
+            return outs
+        return outs[0] if self.n_components is None else outs[:3]
 
-    def _forward_mog(self, state, action, return_raw):
-        if self._use_autograd((state, action)):
-            x = self._state_input(state, self.state_size, True)
-            a = self._as_grad_input(action, self.action_size)
-            w, mu, sigma, raw = _CriticMogFn.apply(self, int(self.precision), x, a, *self._grad_params())
-            return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
-        x = self._state_input(state, self.state_size, False)
-        a = self._as_input(action, self.action_size)
-        B, K = x.shape[0], self.n_components
-        w, mu, sigma = (torch.empty(B, K, dtype=torch.float32, device=x.device) for _ in range(3))
-        raw = torch.empty(B, 3 * K, dtype=torch.float32, device=x.device) if return_raw else None
-        _lib.check(_lib.lib().d4pg_critic_forward_mog(_lib.ptr(self._flat), self.state_size, self.action_size, K,
-                                                      _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(w), _lib.ptr(mu),
-                                                      _lib.ptr(sigma), _lib.ptr(raw), _lib.ptr(self._workspace(B)),
-                                                      int(self.precision), _lib.stream_ptr()), "d4pg_critic_forward_mog")
-        return (w, mu, sigma, raw) if return_raw else (w, mu, sigma)
+    # ---- the three heads: outputs, C forward, what backward keeps, C backward ----------------------------------------
+    def _head_outputs(self, B, device, raw):
+        """Categorical (probs, logits), mixture (w, mu, sigma, raw), quantile (theta,).  Without `raw` the categorical
+        logits and the mixture raw are None: the forward keeps them in its workspace."""
+        def new(n):
+            return torch.empty(B, n, dtype=torch.float32, device=device)
+        if self.n_quantiles is not None:
+            return (new(self.n_atoms),)
+        last = new(self.n_atoms) if raw else None
+        if self.n_components is not None:
+            return (new(self.n_components), new(self.n_components), new(self.n_components), last)
+        return (new(self.n_atoms), last)
 
-    def _forward_qr(self, state, action):
-        if self._use_autograd((state, action)):
-            x = self._state_input(state, self.state_size, True)
-            a = self._as_grad_input(action, self.action_size)
-            return _CriticQrFn.apply(self, int(self.precision), x, a, *self._grad_params())
-        x = self._state_input(state, self.state_size, False)
-        a = self._as_input(action, self.action_size)
-        B = x.shape[0]
-        theta = torch.empty(B, self.n_atoms, dtype=torch.float32, device=x.device)
-        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(self._flat), self.state_size, self.action_size, self.n_atoms,
-                                                  _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(theta),
-                                                  _lib.ptr(self._workspace(B)), int(self.precision), _lib.stream_ptr()),
-                   "d4pg_critic_forward")
-        return theta
+    def _head_forward(self, flat, x, a, outs, ws, precision):
+        L, P, B = _lib.lib(), _lib.ptr, x.shape[0]
+        if self.n_components is not None:
+            w, mu, sigma, raw = outs
+            _lib.check(L.d4pg_critic_forward_mog(P(flat), self.state_size, self.action_size, self.n_components, P(x),
+                                                 P(a), B, P(w), P(mu), P(sigma), P(raw), P(ws), precision,
+                                                 _lib.stream_ptr()), "d4pg_critic_forward_mog")
+            return
+        probs, logits = (None, outs[0]) if self.n_quantiles is not None else outs
+        _lib.check(L.d4pg_critic_forward(P(flat), self.state_size, self.action_size, self.n_atoms, P(x), P(a), B,
+                                         P(probs), P(logits), P(ws), precision, _lib.stream_ptr()), "d4pg_critic_forward")
+
+    def _head_saved(self, outs):
+        """The outputs the head's backward reads: the categorical probs (softmax Jacobian), the mixture raw (softmax /
+        softplus'); a quantile head's backward reads none."""
+        if self.n_quantiles is not None:
+            return ()
+        return (outs[-1],) if self.n_components is not None else (outs[0],)
+
+    def _head_backward(self, flat, x, a, saved, ws, grads, grad_flat, grad_x, grad_a, scratch, precision):
+        L, P, B = _lib.lib(), _lib.ptr, x.shape[0]
+        grads = [P(g) for g in grads]
+        if self.n_components is not None:
+            g_w, g_mu, g_sigma = grads[:3]
+            _lib.check(L.d4pg_critic_backward_mog(P(flat), self.state_size, self.action_size, self.n_components, P(x),
+                                                  P(a), B, P(saved[0]), P(ws), g_w, g_mu, g_sigma, P(grad_flat),
+                                                  P(grad_x), P(grad_a), P(scratch), precision, _lib.stream_ptr()),
+                       "d4pg_critic_backward_mog")
+            return
+        if self.n_quantiles is not None:        # d loss / d theta is the logits' gradient: no head Jacobian
+            probs, g_probs, g_logits = None, None, grads[0]
+        else:
+            probs, (g_probs, g_logits) = P(saved[0]), grads
+        _lib.check(L.d4pg_critic_backward(P(flat), self.state_size, self.action_size, self.n_atoms, P(x), P(a), B,
+                                          probs, P(ws), g_probs, g_logits, P(grad_flat), P(grad_x), P(grad_a),
+                                          P(scratch), precision, _lib.stream_ptr()), "d4pg_critic_backward")
 
 
-def _backward_scratch(B, out_dim, device):
-    """d4pg_*_backward scratch: two [B,256] delta planes and one output-head plane of row pitch pitch4(out_dim), at
-    least [B,256] (include/d4pg_b200.h)."""
+def _backward_buffers(ctx, net, inputs, out_dim):
+    """What a d4pg_*_backward call writes: the flat parameter gradient (None unless a parameter asks for one), a
+    gradient for each of `inputs` (the Function's inputs from index 2) that asks for one, and the scratch -- two
+    [B,256] delta planes and one output-head plane of row pitch pitch4(out_dim), at least [B,256]
+    (include/d4pg_b200.h)."""
+    x = inputs[0]
+    want_p = any(ctx.needs_input_grad[2 + len(inputs):])
+    grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
+    grad_in = [torch.empty_like(t) if ctx.needs_input_grad[2 + i] else None for i, t in enumerate(inputs)]
     head = max(HIDDEN, (out_dim + 3) & ~3)
-    return torch.empty(B * (2 * HIDDEN + head), dtype=torch.float32, device=device)
+    scratch = torch.empty(x.shape[0] * (2 * HIDDEN + head), dtype=torch.float32, device=x.device)
+    return grad_flat, grad_in, scratch
 
 
 def _param_grads(ctx, net, grad_flat, first):
@@ -398,6 +439,10 @@ def _param_grads(ctx, net, grad_flat, first):
         out += [w if ctx.needs_input_grad[first + 2 * i] else None,
                 b if ctx.needs_input_grad[first + 2 * i + 1] else None]
     return out
+
+
+def _f32(g):
+    return g.to(dtype=torch.float32).contiguous() if g is not None else None
 
 
 class _ActorFn(torch.autograd.Function):
@@ -426,141 +471,49 @@ class _ActorFn(torch.autograd.Function):
         net = ctx.net
         if g is None:
             return (None,) * (3 + 8)
-        B = x.shape[0]
-        g = g.to(dtype=torch.float32).contiguous()
-        want_p = any(ctx.needs_input_grad[3:])
-        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
-        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
-        scratch = _backward_scratch(B, net.output_size, x.device)
-        _lib.check(_lib.lib().d4pg_actor_backward(_lib.ptr(ctx.flat), net.input_size, net.output_size, _lib.ptr(x), B,
-                                                  _lib.ptr(out), _lib.ptr(ctx.ws), _lib.ptr(g), _lib.ptr(grad_flat),
-                                                  _lib.ptr(grad_x), _lib.ptr(scratch), ctx.precision,
-                                                  _lib.stream_ptr()), "d4pg_actor_backward")
+        g = _f32(g)
+        grad_flat, (grad_x,), scratch = _backward_buffers(ctx, net, (x,), net.output_size)
+        _lib.check(_lib.lib().d4pg_actor_backward(_lib.ptr(ctx.flat), net.input_size, net.output_size, _lib.ptr(x),
+                                                  x.shape[0], _lib.ptr(out), _lib.ptr(ctx.ws), _lib.ptr(g),
+                                                  _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(scratch),
+                                                  ctx.precision, _lib.stream_ptr()), "d4pg_actor_backward")
         return (None, None, grad_x, *_param_grads(ctx, net, grad_flat, 3))
 
 
 class _CriticFn(torch.autograd.Function):
-    """(probs, logits) = critic(state, action) through d4pg_critic_forward; backward = d4pg_critic_backward."""
+    """critic(state, action) of any head: its outputs (critic._head_outputs, the raw one included) through the head's
+    C forward; backward = the head's C backward.  A mixture's raw output is for inspection only: it is marked
+    non-differentiable and its gradient is not propagated."""
 
     @staticmethod
     def forward(ctx, net, precision, x, a, *params):
         B = x.shape[0]
-        probs = torch.empty(B, net.n_atoms, dtype=torch.float32, device=x.device)
-        logits = torch.empty_like(probs)        # always given: without it the forward reuses h1 as logits scratch
-        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)
-        flat = net._flat
-        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(flat), net.state_size, net.action_size, net.n_atoms,
-                                                  _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(probs), _lib.ptr(logits),
-                                                  _lib.ptr(ws), precision, _lib.stream_ptr()), "d4pg_critic_forward")
-        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
-        ctx.set_materialize_grads(False)
-        ctx.save_for_backward(x, a, probs, *params)
-        return probs, logits
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g_probs, g_logits):
-        x, a, probs = ctx.saved_tensors[:3]
-        net = ctx.net
-        if g_probs is None and g_logits is None:
-            return (None,) * (4 + 8)
-        B = x.shape[0]
-        g_probs = g_probs.to(dtype=torch.float32).contiguous() if g_probs is not None else None
-        g_logits = g_logits.to(dtype=torch.float32).contiguous() if g_logits is not None else None
-        want_p = any(ctx.needs_input_grad[4:])
-        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
-        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
-        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
-        scratch = _backward_scratch(B, net.n_atoms, x.device)
-        _lib.check(_lib.lib().d4pg_critic_backward(_lib.ptr(ctx.flat), net.state_size, net.action_size, net.n_atoms,
-                                                   _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(probs), _lib.ptr(ctx.ws),
-                                                   _lib.ptr(g_probs), _lib.ptr(g_logits), _lib.ptr(grad_flat),
-                                                   _lib.ptr(grad_x), _lib.ptr(grad_a), _lib.ptr(scratch), ctx.precision,
-                                                   _lib.stream_ptr()), "d4pg_critic_backward")
-        return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
-
-
-class _CriticMogFn(torch.autograd.Function):
-    """(w, mu, sigma, raw) = mixture critic(state, action) through d4pg_critic_forward_mog; backward =
-    d4pg_critic_backward_mog.  raw is returned for inspection only: its gradient is not propagated."""
-
-    @staticmethod
-    def forward(ctx, net, precision, x, a, *params):
-        B, K = x.shape[0], net.n_components
-        w, mu, sigma = (torch.empty(B, K, dtype=torch.float32, device=x.device) for _ in range(3))
-        raw = torch.empty(B, 3 * K, dtype=torch.float32, device=x.device)   # kept for backward (softmax / softplus')
-        ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)
-        flat = net._flat
-        _lib.check(_lib.lib().d4pg_critic_forward_mog(_lib.ptr(flat), net.state_size, net.action_size, K, _lib.ptr(x),
-                                                      _lib.ptr(a), B, _lib.ptr(w), _lib.ptr(mu), _lib.ptr(sigma),
-                                                      _lib.ptr(raw), _lib.ptr(ws), precision, _lib.stream_ptr()),
-                   "d4pg_critic_forward_mog")
-        ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
-        ctx.set_materialize_grads(False)
-        ctx.mark_non_differentiable(raw)
-        ctx.save_for_backward(x, a, raw, *params)
-        return w, mu, sigma, raw
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g_w, g_mu, g_sigma, g_raw):
-        x, a, raw = ctx.saved_tensors[:3]
-        net = ctx.net
-        if g_w is None and g_mu is None and g_sigma is None:
-            return (None,) * (4 + 8)
-        B = x.shape[0]
-        g_w, g_mu, g_sigma = (g.to(dtype=torch.float32).contiguous() if g is not None else None for g in (g_w, g_mu, g_sigma))
-        want_p = any(ctx.needs_input_grad[4:])
-        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
-        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
-        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
-        scratch = _backward_scratch(B, net.n_atoms, x.device)
-        _lib.check(_lib.lib().d4pg_critic_backward_mog(_lib.ptr(ctx.flat), net.state_size, net.action_size,
-                                                       net.n_components, _lib.ptr(x), _lib.ptr(a), B, _lib.ptr(raw),
-                                                       _lib.ptr(ctx.ws), _lib.ptr(g_w), _lib.ptr(g_mu), _lib.ptr(g_sigma),
-                                                       _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(grad_a),
-                                                       _lib.ptr(scratch), ctx.precision, _lib.stream_ptr()),
-                   "d4pg_critic_backward_mog")
-        return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
-
-
-class _CriticQrFn(torch.autograd.Function):
-    """theta = quantile critic(state, action) through d4pg_critic_forward without the softmax (probs = NULL); backward =
-    d4pg_critic_backward with grad_logits = d loss / d theta (no head Jacobian)."""
-
-    @staticmethod
-    def forward(ctx, net, precision, x, a, *params):
-        B = x.shape[0]
-        theta = torch.empty(B, net.n_atoms, dtype=torch.float32, device=x.device)
+        outs = net._head_outputs(B, x.device, True)
         ws = torch.empty(3 * B * HIDDEN, dtype=torch.float32, device=x.device)      # h1..h3, kept for backward
         flat = net._flat
-        _lib.check(_lib.lib().d4pg_critic_forward(_lib.ptr(flat), net.state_size, net.action_size, net.n_atoms,
-                                                  _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(theta), _lib.ptr(ws),
-                                                  precision, _lib.stream_ptr()), "d4pg_critic_forward")
+        net._head_forward(flat, x, a, outs, ws, precision)
         ctx.net, ctx.precision, ctx.flat, ctx.ws = net, precision, flat, ws
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(x, a, *params)
-        return theta
+        if net.n_components is not None:
+            ctx.mark_non_differentiable(outs[-1])
+        saved = net._head_saved(outs)
+        ctx.n_saved = len(saved)
+        ctx.save_for_backward(x, a, *saved, *params)
+        return outs
 
     @staticmethod
     @once_differentiable
-    def backward(ctx, g):
-        x, a = ctx.saved_tensors[:2]
+    def backward(ctx, *grads):
+        x, a = ctx.saved_tensors[:2]            # unpacking checks the version counters (parameters included)
+        saved = ctx.saved_tensors[2:2 + ctx.n_saved]
         net = ctx.net
-        if g is None:
+        if net.n_components is not None:
+            grads = grads[:3]                   # the raw output's gradient is not propagated
+        if all(g is None for g in grads):
             return (None,) * (4 + 8)
-        B = x.shape[0]
-        g = g.to(dtype=torch.float32).contiguous()
-        want_p = any(ctx.needs_input_grad[4:])
-        grad_flat = torch.empty(net._total, dtype=torch.float32, device=x.device) if want_p else None
-        grad_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None
-        grad_a = torch.empty_like(a) if ctx.needs_input_grad[3] else None
-        scratch = _backward_scratch(B, net.n_atoms, x.device)
-        _lib.check(_lib.lib().d4pg_critic_backward(_lib.ptr(ctx.flat), net.state_size, net.action_size, net.n_atoms,
-                                                   _lib.ptr(x), _lib.ptr(a), B, None, _lib.ptr(ctx.ws), None,
-                                                   _lib.ptr(g), _lib.ptr(grad_flat), _lib.ptr(grad_x), _lib.ptr(grad_a),
-                                                   _lib.ptr(scratch), ctx.precision, _lib.stream_ptr()),
-                   "d4pg_critic_backward")
+        grads = [_f32(g) for g in grads]
+        grad_flat, (grad_x, grad_a), scratch = _backward_buffers(ctx, net, (x, a), net.n_atoms)
+        net._head_backward(ctx.flat, x, a, saved, ctx.ws, grads, grad_flat, grad_x, grad_a, scratch, ctx.precision)
         return (None, None, grad_x, grad_a, *_param_grads(ctx, net, grad_flat, 4))
 
 
