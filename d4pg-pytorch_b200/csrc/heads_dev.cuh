@@ -256,11 +256,11 @@ __global__ void __launch_bounds__(HEAD_WARPS * 32) heads_kernel(const HeadsArgs 
   pdl_trigger(a.h.pdl);
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = blockIdx.x * HEAD_WARPS + warp;            // warps [0, B): critic part of row g; [B, 2B): policy head of row g - B
+  const int g = blockIdx.x * HEAD_WARPS + warp;            // warps [0, B): critic part of row g; [B, 2B): policy head of row g - B (none when pi is null)
   step_stamp(a.h.trace, 2);
   if (a.h.only_policy) { if (g < a.h.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 2); }
   else if (g < a.h.B) heads_row<MODE, NT>(a, g, lane, ws[warp], 1);
-  else if (g < 2 * a.h.B) heads_row<MODE, NT>(a, g - a.h.B, lane, ws[warp], 2);
+  else if (a.h.pi && g < 2 * a.h.B) heads_row<MODE, NT>(a, g - a.h.B, lane, ws[warp], 2);
   step_stamp(a.h.trace, 2 + 16);
   if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
     a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;

@@ -153,6 +153,8 @@ __device__ __forceinline__ void mog_policy_row(const MogArgs& a, int row, int la
 }
 
 // warps [0, B): critic part of row g; [B, 2B): policy part of row g - B (only_policy: warps [0, B) run the policy part).
+// The post-update plan's first launch has no policy head (pi null): its grid covers B warps only, rounded up to whole
+// blocks, and the warps past B must not run a policy row.
 // Also does what heads_kernel does for the step besides the maths: PDL wait / trigger, the step stamps and the
 // sampler-clock advance of the prefetch / host pipelines.
 // __maxnreg__(255): without it ptxas aims at 64-96 registers and spills the per-point arrays (blocks are 128 threads).
@@ -166,7 +168,7 @@ __global__ void __maxnreg__(255) mog_heads_kernel(const MogArgs a) {
   step_stamp(a.h.trace, 2);
   if (a.h.only_policy) { if (g < a.h.B) mog_policy_row(a, g, lane); }
   else if (g < a.h.B) mog_critic_row<NT, HZ>(a, g, lane);
-  else if (g < 2 * a.h.B) mog_policy_row(a, g - a.h.B, lane);
+  else if (a.h.pi && g < 2 * a.h.B) mog_policy_row(a, g - a.h.B, lane);
   step_stamp(a.h.trace, 2 + 16);
   if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
     a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;

@@ -108,6 +108,8 @@ __device__ __forceinline__ void qr_policy_row(const QrArgs& a, int row, int lane
 }
 
 // warps [0, B): critic part of row g; [B, 2B): policy part of row g - B (only_policy: warps [0, B) run the policy part).
+// The post-update plan's first launch has no policy head (pi null): its grid covers B warps only, rounded up to whole
+// blocks, and the warps past B must not run a policy row.
 // Also does what heads_kernel does for the step besides the maths: PDL wait / trigger, the step stamps and the
 // sampler-clock advance of the prefetch / host pipelines.
 template <int NT>
@@ -120,7 +122,7 @@ __global__ void __launch_bounds__(QR_WARPS * 32) qr_heads_kernel(const QrArgs a)
   step_stamp(a.h.trace, 2);
   if (a.h.only_policy) { if (g < a.h.B) qr_policy_row<NT>(a, g, lane); }
   else if (g < a.h.B) qr_critic_row<NT>(a, g, lane, ys[warp]);
-  else if (g < 2 * a.h.B) qr_policy_row<NT>(a, g - a.h.B, lane);
+  else if (a.h.pi && g < 2 * a.h.B) qr_policy_row<NT>(a, g - a.h.B, lane);
   step_stamp(a.h.trace, 2 + 16);
   if (a.h.sampler_clock && blockIdx.x == 0 && threadIdx.x == 0) {
     a.h.sampler_clock->s_adam_step += 1; a.h.sampler_clock->s_beta_t += 1; a.h.sampler_clock->s_steps_done += 1;

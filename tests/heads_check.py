@@ -437,7 +437,8 @@ def step_planes(dd):
     """The heads' inputs and outputs of the step `dd` just ran, read through the learner's tensors: planes at pitch Np.
     The IS weights are `dd._learner.weights`: without a pipeline (prefetch=False) the learner samples straight into the
     caller's buffers (csrc/learner.cu, d4pg_learner_create: batch[0].wts = buf->weights), and head_common hands that
-    plane to the loss kernel when importance_weighted is set."""
+    plane to the loss kernel when importance_weighted is set on a prioritized replay (a uniform replay's rows all weigh
+    1; the sampler writes no weights there)."""
     L = dd._learner
     B = dd.batch_size
     T = lambda n, dt=torch.float32: L.tensor(n, dt).cpu()
@@ -446,7 +447,8 @@ def step_planes(dd):
     P.update(r=T("r", torch.float64).numpy()[:B], d=T("done", torch.uint8).numpy()[:B].astype(bool),
              h=T("h", torch.uint8).numpy()[:B] if dd.nstep_tails else np.zeros(B, np.uint8),
              loss_rows=T("loss_rows")[:B], pi_rows=T("pi_rows")[:B], td=L.td.cpu(), prio=L.prio.cpu(),
-             losses=L.losses.cpu(), isw=L.weights.cpu().numpy() if dd.importance_weighted else np.ones(B))
+             losses=L.losses.cpu(),
+             isw=L.weights.cpu().numpy() if dd.importance_weighted and dd.prioritized_replay else np.ones(B))
     return P
 
 
@@ -455,7 +457,9 @@ def step_config(dd):
     mode = 1 if dd.projection == "nstep" else 0
     return dict(kind=kind, N=dd.n_atoms, K=dd.n_components, v_min=dd.v_min, v_max=dd.v_max, gamma=dd.gamma,
                 n_steps=dd.n_steps, mode=mode, tails=bool(dd.nstep_tails), kappa=dd.qr_kappa, B=dd.batch_size,
-                gs=float(F32(1.0) / F32(dd.batch_size)), prio_eps=dd.prioritized_replay_eps, ce=dd.priority == "ce")
+                gs=float(F32(1.0) / F32(dd.batch_size)), ce=dd.priority == "ce",
+                # a uniform replay's learner computes its (unused) priorities with eps 1e-6
+                prio_eps=dd.prioritized_replay_eps if dd.prioritized_replay else 1e-6)
 
 
 def step_discounts(cfg, h):

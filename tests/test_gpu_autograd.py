@@ -32,7 +32,8 @@ def _info(N):
 
 
 def _close(name, mine, ref, tol=1e-5):
-    """max abs error <= tol * max(1, |ref|max)  (the bound of test_gpu_tc_chain.py)"""
+    """max abs error <= tol * max(1, |ref|max): a whole-tensor bound (tests/step_check.py, run by
+    tests/test_gpu_step_edges.py, holds the learner step's layers to componentwise ones)"""
     mine, ref = mine.double().cpu(), ref.double().cpu()
     assert mine.shape == ref.shape, (name, mine.shape, ref.shape)
     scale = max(1.0, float(ref.abs().max()))

@@ -220,7 +220,7 @@ def _check_batch(dd, st, all_rows, what):
     idx = dd.last_batch_info()["idx"].cpu().numpy()
     shift, scale = st.affine()
     for name, src in (("s", all_rows[0]), ("s2", all_rows[3])):
-        got = dd.debug_tensor(name, shape=(B, S_DIM)).cpu().numpy()
+        got = dd.debug_tensor(name, shape=(B, dd.obs_dim)).cpu().numpy()
         want = ON.apply(src[idx], shift, scale)
         assert _bits_equal(got, want), "%s: %s differs from the oracle-normalized rows (max |d| %.3g)" % (
             what, name, np.abs(got - want).max())

@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import clip_check as CC
 from tests import step_check as SC
 from tests import update_check as UC
 
@@ -193,11 +194,13 @@ def _rows(rng, n, S, A):
 
 class Checked(object):
     """Steps of one learner, each followed by the update check at the step count the host has taken, the IS-weight
-    check when prioritized, and the teacher-forced layer check when asked."""
+    check when prioritized, and the teacher-forced layer check when asked.  clip: (max_norm, weight_decay, ClipStats)
+    of a learner that clips or decays; its update is then held to tests/clip_check.py."""
 
-    def __init__(self, dd, plan, precision, label, post_update=False, stats=None):
+    def __init__(self, dd, plan, precision, label, post_update=False, stats=None, clip=None):
         self.dd, self.plan, self.precision, self.label, self.post_update = dd, plan, precision, label, post_update
         self.stats = stats if stats is not None else UC.Stats()
+        self.clip = clip
 
     def step(self, how="train", layers=False, seed=None):
         dd = self.dd
@@ -209,7 +212,12 @@ class Checked(object):
             random.seed(seed)
         dd.profile_step() if how == "profile" else dd.train()
         k = dd.optimizer_global_actor.step_count
-        uc.check(dd, k, self.stats, self.label)
+        if self.clip is None:
+            uc.check(dd, k, self.stats, self.label)
+        else:
+            max_norm, wd, cstats = self.clip
+            CC.check_step(uc.before, UC.read(dd, grads=True), uc.pads, uc.h, k, max_norm, wd, dd.last_grad_norms(), cstats,
+                          self.label)
         power = None
         if tr is not None:
             info = dd.last_batch_info()
