@@ -696,6 +696,7 @@ class DDPG:
         store = self.replayBuffer._store
         if store._n_staged:
             store.flush()
+        store.before_step()                   # the ingest stream's sample waits for the caller's replay writes
         f = L._flats
         v = (f[0]._version, f[1]._version, f[2]._version, f[3]._version) if self.track_weights else None
         if v != L.seen_versions or v is None:

@@ -238,10 +238,13 @@ class _DeviceReplay(object):
         self._steps = None               # add_steps: the device windows and the host mirror of their fills
         self._goals = None               # add_goal_steps: the device episode windows and their GoalStepsMirror
         # host pipeline (a learner's ingest stream, ddpg.py): add_batch_host is issued there; every other device
-        # operation runs on the caller's stream -- the two are kept in program order by events, only when they interleave
+        # operation runs on the caller's stream -- the two are kept in program order by events, only when they interleave.
+        # _cs_dirty: the caller's stream touched the buffer (the next host add waits for it); _cs_wrote: it wrote the
+        # buffer (the next step's sample on the ingest stream waits for it, before_step)
         self._ingest_stream = None
         self._ing_dirty = False
         self._cs_dirty = False
+        self._cs_wrote = False
         if obs_dim is not None and act_dim is not None and torch.cuda.is_available():
             self._allocate(obs_dim, act_dim)
 
@@ -305,7 +308,17 @@ class _DeviceReplay(object):
             self._join_ingest()
         self._ingest_stream = raw_stream
         self._ing_dirty = False
-        self._cs_dirty = raw_stream is not None          # whatever the caller's stream did so far comes first
+        self._cs_dirty = self._cs_wrote = raw_stream is not None     # whatever the caller's stream did so far comes first
+
+    def _caller_wrote(self):
+        """A write to the ring, trees, horizons or normalizer statistics was issued on the caller's stream."""
+        self._cs_dirty = self._cs_wrote = True
+
+    def before_step(self):
+        """A host-pipeline step is about to sample on the ingest stream, which does not wait for the caller's stream:
+        order it after the caller's writes since the last ordering.  Reads on the caller's stream need no edge."""
+        if self._cs_wrote:
+            self._order_ingest_after_caller()
 
     def _join_ingest(self):
         """The caller's stream is about to touch the buffer: order it after the ingest stream's adds."""
@@ -317,11 +330,11 @@ class _DeviceReplay(object):
             self._cs_dirty = True
 
     def _order_ingest_after_caller(self):
-        """The caller's stream wrote something the ingest stream's next sample reads (normalizer statistics)."""
+        """Order the ingest stream after everything issued so far on the caller's stream."""
         if self._ingest_stream is not None and self.handle is not None:
             _lib.check(_lib.lib().d4pg_replay_order_after(self.handle, _lib.stream_ptr(), C.c_void_p(self._ingest_stream)),
                        "d4pg_replay_order_after")
-            self._cs_dirty = False
+        self._cs_dirty = self._cs_wrote = False
 
     def _ingest_ptr(self):
         """Stream of a host add: the ingest stream when attached (ordered after the caller's earlier buffer operations)."""
@@ -329,9 +342,7 @@ class _DeviceReplay(object):
         if ing is None:
             return _lib.raw_stream()
         if self._cs_dirty:
-            _lib.check(_lib.lib().d4pg_replay_order_after(self.handle, _lib.stream_ptr(), C.c_void_p(ing)),
-                       "d4pg_replay_order_after")
-            self._cs_dirty = False
+            self._order_ingest_after_caller()
         self._ing_dirty = True
         return ing
 
@@ -434,6 +445,7 @@ class _DeviceReplay(object):
         _lib.check(_lib.lib().d4pg_replay_add_nstep(self.handle, T, *[_lib.ptr(t) for t in args], n_steps, float(gamma),
                                                     _lib.ptr(scratch), 1 if self.prioritized else 0, _lib.stream_ptr()),
                    "d4pg_replay_add_nstep")
+        self._caller_wrote()
         self._sync_ring()
         return m
 
@@ -534,6 +546,7 @@ class _DeviceReplay(object):
         _lib.check(_lib.lib().d4pg_replay_add_steps_ex(self.handle, E, *[_lib.ptr(t) for t in args], n, gamma,
                                                        _lib.ptr(w.window), n_rows, tails, 1 if self.prioritized else 0,
                                                        _lib.stream_ptr()), "d4pg_replay_add_steps_ex")
+        self._caller_wrote()
         self._sync_ring()
         w.advance()
         w.record_ends(term, trunc, terminated, truncated)
@@ -587,6 +600,7 @@ class _DeviceReplay(object):
             self.handle, w.E, w.So, w.G, *[_lib.ptr(t) for t in inputs], w.M, _lib.ptr(w.window), _lib.ptr(plan_dev),
             n_draws, n_rows, w.threshold, 0 if w.her_action == "reference" else 1, 1 if no_step else 0,
             1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add_goal_steps")
+        self._caller_wrote()
         self._sync_ring()
 
     def add_goal_steps(self, obs, desired_goal, action, reward, obs_next, achieved_goal_next, terminated, truncated=None,
@@ -641,6 +655,7 @@ class _DeviceReplay(object):
     def _add_device(self, n, tensors):
         _lib.check(_lib.lib().d4pg_replay_add(self.handle, n, *[_lib.ptr(t) for t in tensors],
                                               1 if self.prioritized else 0, _lib.stream_ptr()), "d4pg_replay_add")
+        self._caller_wrote()
         self._sync_ring()
 
     def _sync_ring(self):
@@ -720,6 +735,7 @@ class _DeviceReplay(object):
             assert bool(((idx >= 0) & (idx < len(self))).all()), "index out of range"
         _lib.check(_lib.lib().d4pg_replay_update_priorities(self.handle, idx.numel(), _lib.ptr(idx), _lib.ptr(pr),
                                                             _lib.stream_ptr()), "d4pg_replay_update_priorities")
+        self._caller_wrote()
 
     def reduce(self, start=0, end=None):
         self.flush()
@@ -781,6 +797,7 @@ class SegmentTree(object):
         v = torch.tensor([val], dtype=torch.float32, device=st.device)
         _lib.check(_lib.lib().d4pg_replay_set_leaves(st.handle, 1, _lib.ptr(i), _lib.ptr(v), _lib.ptr(v),
                                                      _lib.stream_ptr()), "d4pg_replay_set_leaves")
+        st._caller_wrote()
 
     def __getitem__(self, idx):
         assert 0 <= idx < self._capacity

@@ -634,8 +634,12 @@ int64_t d4pg_learner_steps_done(const d4pg_learner_t* h);
 /* host pipeline (cfg.prefetch with sample_mode 0): the stream buffer adds should be issued on so they overlap the
  * running step (NULL when the pipeline is off).  Owned by the learner.  With the pipeline on, d4pg_learner_step_host*
  * samples on this stream and does NOT wait for caller_stream first (that stream is ordered after the whole previous
- * step, which would serialise the pipeline): a caller that touched the buffer on another stream (add, update_priorities,
- * set_leaves ...) calls d4pg_replay_order_after(replay, that_stream, ingest_stream) before the next step. */
+ * step, which would serialise the pipeline): a caller that WROTE the buffer on another stream since the last step (add,
+ * add_steps, add_goal_steps, add_nstep, update_priorities, set_leaves, a normalizer refresh ...) calls
+ * d4pg_replay_order_after(replay, that_stream, ingest_stream) before the next step; without it the step may sample
+ * rows, trees or normalizer statistics from before that write, and on the wgmma plans, whose forward chains poll the
+ * sample's epochs, a sample drawn before the previous step advanced the step clock leaves the step waiting forever.
+ * Reads on another stream need no edge before a step. */
 void* d4pg_learner_ingest_stream(const d4pg_learner_t* h);
 /* The tensor-core plans consume pre-split hi/lo weight IMAGES that the library's Adam / Polyak kernel keeps current.  Every
  * CUDA-graph step that samples in the graph re-packs them from the fp32 parameters first (any external write is picked
