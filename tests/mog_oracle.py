@@ -1,10 +1,10 @@
 """CPU restatement of the mixture-of-Gaussians critic (critic_dist_info type "mixture_of_gaussian") for the tests.
 
 DERIVED oracle: the reference stubs its mixture branch (`TODO: pass`, ddpg.py:48-50, models.py:63-65), so this module
-restates the library's own definition (include/d4pg_b200.h, d4pg_mog_loss) rather than reference lines.  It reuses the
-reference-pinned pieces of oracle/d4pg_oracle.py -- the initialisation, Adam, Polyak and the PER oracle -- and takes
-the linear layer as a parameter (fp32 `F.linear`, or `bf16_oracle.linear("bf16")`).  The head itself is evaluated in
-float64 from the fp32 raw head, as the kernel does:
+restates the library's own definition (include/d4pg_b200.h, d4pg_mog_loss) rather than reference lines.  Its learner
+is oracle/d4pg_oracle.py's LearnerOracle -- the pinned networks, initialisation, Adam, Polyak and step order -- with the
+head replaced, and takes the linear layer as a parameter (fp32 `F.linear`, or `bf16_oracle.linear("bf16")`).  The head
+itself is evaluated in float64 from the fp32 raw head, as the kernel does:
 
   w = softmax(o[:, :K]),  mu = o[:, K:2K],  sigma = softplus(o[:, 2K:]) + 1e-3
   L_i = -sum_{k,q} w'_k h_q / sqrt(pi) * log p(r_i + c (mu'_k + sqrt(2) sigma'_k x_q)),   c = discount * (1 - done_i)
@@ -82,83 +82,30 @@ def heads(target_raw, q_raw, pi_raw, r, done, discount, K, grad_scale, prio_eps=
     return out
 
 
-def actor_forward(w, s, lin=F.linear):
-    h = F.relu(lin(s, w["fc1.weight"], w["fc1.bias"]))
-    h = lin(h, w["fc2.weight"], w["fc2.bias"])                       # no ReLU (H9)
-    h = F.relu(lin(h, w["fc2_2.weight"], w["fc2_2.bias"]))
-    return torch.tanh(lin(h, w["fc3.weight"], w["fc3.bias"]))
+class MogLearnerOracle(O.LearnerOracle):
+    """O.LearnerOracle.train_step with the mixture head: the critic's raw 3K-wide fc3 row, the quadrature loss rows,
+    td and the policy rows above.  `projection` picks the discount (gamma, or gamma ** n_steps for "nstep")."""
 
-
-def critic_raw(w, s, a, lin=F.linear):
-    """The critic MLP up to its 3K-wide fc3 output (no head transform)."""
-    h = F.relu(lin(s, w["fc1.weight"], w["fc1.bias"]))
-    h = F.relu(lin(torch.cat([h, a], 1), w["fc2.weight"], w["fc2.bias"]))
-    h = F.relu(lin(h, w["fc2_2.weight"], w["fc2_2.bias"]))
-    return lin(h, w["fc3.weight"], w["fc3.bias"])
-
-
-class MogLearnerOracle:
-    """One DDPG.train() body with the mixture critic, mirroring `LearnerOracle.train_step` (same Adam, Polyak,
-    pre-update critic for the policy loss unless `post_update_critic`)."""
+    logits = True
+    names = {"target": "target_raw", "q": "q_raw", "pi": "pi_raw", "dq": "dq_raw", "dpi": "dpi_raw"}
 
     def __init__(self, obs_dim, act_dim, K, gamma=0.99, tau=0.001, n_steps=1, lr=1e-3, betas=(0.9, 0.9), eps=1e-8,
                  actor_w=None, critic_w=None, projection="live", linear=F.linear):
-        self.K, self.gamma, self.tau, self.n_steps = K, gamma, tau, n_steps
-        self.lr, self.betas, self.eps, self.lin = lr, betas, eps, linear
-        self.discount = gamma if projection == "live" else gamma ** n_steps
-        self.actor = actor_w if actor_w is not None else O.init_actor(obs_dim, act_dim)
-        self.actor_target = {k: v.clone() for k, v in self.actor.items()}
-        self.critic = critic_w if critic_w is not None else O.init_critic(obs_dim, act_dim, 3 * K)
-        self.critic_target = {k: v.clone() for k, v in self.critic.items()}
-        z = lambda d: {k: torch.zeros_like(v) for k, v in d.items()}
-        self.m_a, self.v_a, self.m_c, self.v_c = z(self.actor), z(self.actor), z(self.critic), z(self.critic)
-        self.step_a = self.step_c = 0
+        super().__init__(obs_dim, act_dim, K, gamma, tau, n_steps, lr, betas, eps, actor_w, critic_w, projection, linear)
 
-    def _adam(self, which, g):
-        p, m, v = (self.critic, self.m_c, self.v_c) if which == "c" else (self.actor, self.m_a, self.v_a)
-        if which == "c":
-            self.step_c += 1
-        else:
-            self.step_a += 1
-        for k in O.PARAM_ORDER:
-            O.adam_step(p[k], g[k], m[k], v[k], self.step_c if which == "c" else self.step_a, self.lr,
-                        self.betas[0], self.betas[1], self.eps)
+    def init_head(self, K):
+        self.K = K
+        self.discount = self.gamma if self.projection == "live" else self.gamma ** self.n_steps
+        return 3 * K
 
-    def train_step(self, s, a, r, s2, done, is_weights=None, post_update_critic=False):
-        lin, K = self.lin, self.K
-        s_t = torch.from_numpy(np.asarray(s, dtype=O.F32))
-        a_t = torch.from_numpy(np.asarray(a, dtype=O.F32))
-        s2_t = torch.from_numpy(np.asarray(s2, dtype=O.F32))
-        with torch.no_grad():
-            traw = critic_raw(self.critic_target, s2_t, actor_forward(self.actor_target, s2_t, lin), lin)
-        cw = {k: v.clone().requires_grad_(True) for k, v in self.critic.items()}
-        qraw = critic_raw(cw, s_t, a_t, lin)
-        qraw.retain_grad()
-        rows = loss_rows(traw, qraw, r, done, self.discount, K)
-        if is_weights is not None:
-            rows = rows * torch.from_numpy(np.asarray(is_weights, dtype=O.F32)).double()
-        loss_c = rows.mean()
-        loss_c.backward()
-        g_c = {k: cw[k].grad.detach().clone() for k in O.PARAM_ORDER}
-        t = td(traw, qraw, r, done, self.discount, K)
-        if post_update_critic:
-            self._adam("c", g_c)
-        aw = {k: v.clone().requires_grad_(True) for k, v in self.actor.items()}
-        act = actor_forward(aw, s_t, lin)
-        praw = critic_raw(self.critic, s_t, act, lin)
-        praw.retain_grad()
-        prow = policy_rows(praw, K)
-        loss_a = prow.mean()
-        loss_a.backward()
-        g_a = {k: aw[k].grad.detach().clone() for k in O.PARAM_ORDER}
-        if not post_update_critic:
-            self._adam("c", g_c)
-        self._adam("a", g_a)
-        for k in O.PARAM_ORDER:
-            O.polyak(self.actor_target[k], self.actor[k], self.tau)
-            O.polyak(self.critic_target[k], self.critic[k], self.tau)
-        prio = (np.abs(t.numpy()).astype(O.F32) + O.F32(1e-6)).astype(O.F32)
-        return dict(target_raw=traw, q_raw=qraw.detach(), pi_raw=praw.detach(), actor_out=act.detach(),
-                    loss_rows=rows.detach(), pi_rows=prow.detach(), loss_critic=float(loss_c.detach()), loss_actor=float(loss_a.detach()),
-                    td=t, prio=prio, dq_raw=qraw.grad.detach(), dpi_raw=praw.grad.detach(),
-                    grads_actor=g_a, grads_critic=g_c)
+    def critic_head(self, target, q, r, done):
+        return (loss_rows(target, q, r, done, self.discount, self.K), td(target, q, r, done, self.discount, self.K),
+                {})
+
+    def policy_head(self, pi):
+        return policy_rows(pi, self.K)
+
+    def priority(self, rows, td, ce_priority):
+        if ce_priority:
+            raise ValueError("the mixture critic has no cross-entropy priority (DDPG rejects priority=\"ce\" with it)")
+        return super().priority(rows, td, False)

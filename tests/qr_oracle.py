@@ -1,10 +1,10 @@
 """CPU restatement of the quantile-regression critic (critic_dist_info type "quantile") for the tests.
 
 DERIVED oracle: the reference has no quantile code, so this module restates the library's own definition
-(include/d4pg_b200.h, d4pg_qr_loss; QR-DQN, Dabney et al. 2018) rather than reference lines.  It reuses the MLP
-restatements of tests/mog_oracle.py and the reference-pinned pieces of oracle/d4pg_oracle.py -- the initialisation, Adam,
-Polyak and the PER oracle -- and takes the linear layer as a parameter (fp32 `F.linear`, `bf16_oracle.linear("bf16")`
-or `tf32_oracle.linear("rz")`).  The head is evaluated in float64 from the fp32 quantile rows, as the kernel does:
+(include/d4pg_b200.h, d4pg_qr_loss; QR-DQN, Dabney et al. 2018) rather than reference lines.  Its learner is
+oracle/d4pg_oracle.py's LearnerOracle -- the pinned networks, initialisation, Adam, Polyak and step order -- with the head
+replaced, and takes the linear layer as a parameter (fp32 `F.linear`, `bf16_oracle.linear("bf16")` or
+`tf32_oracle.linear("rz")`).  The head is evaluated in float64 from the fp32 quantile rows, as the kernel does:
 
   tau_k = (2k+1) / (2N),  y_j = r_i + c theta'_j,  u_jk = y_j - theta_k,  c = discount * (1 - done_i)
   H(u) = u^2/2 if |u| <= kappa else kappa (|u| - kappa/2),  rho_jk = |tau_k - 1{u_jk < 0}| H(u_jk) / kappa
@@ -15,7 +15,6 @@ import torch
 import torch.nn.functional as F
 
 from oracle import d4pg_oracle as O
-from tests.mog_oracle import actor_forward, critic_raw
 
 CHUNK = 512          # rows per pairwise block: [CHUNK, N, N] float64 stays small at B = 4096, N = 128
 
@@ -89,70 +88,25 @@ def heads(target_q, q, pi_q, r, done, discount, kappa, grad_scale, prio_eps=1e-6
     return out
 
 
-class QrLearnerOracle:
-    """One DDPG.train() body with the quantile critic, mirroring `MogLearnerOracle.train_step` (same Adam, Polyak,
-    pre-update critic for the policy loss unless `post_update_critic`)."""
+class QrLearnerOracle(O.LearnerOracle):
+    """O.LearnerOracle.train_step with the quantile head: the critic's raw N-wide fc3 row, the quantile-Huber loss rows,
+    td and the policy rows above.  `projection` picks the discount (gamma, or gamma ** n_steps for "nstep")."""
+
+    logits = True
+    names = {"target": "target_q", "pi": "pi_q"}
 
     def __init__(self, obs_dim, act_dim, N, kappa=1.0, gamma=0.99, tau=0.001, n_steps=1, lr=1e-3, betas=(0.9, 0.9),
                  eps=1e-8, actor_w=None, critic_w=None, projection="live", linear=F.linear):
-        self.N, self.kappa, self.gamma, self.tau, self.n_steps = N, kappa, gamma, tau, n_steps
-        self.lr, self.betas, self.eps, self.lin = lr, betas, eps, linear
-        self.discount = gamma if projection == "live" else gamma ** n_steps
-        self.actor = actor_w if actor_w is not None else O.init_actor(obs_dim, act_dim)
-        self.actor_target = {k: v.clone() for k, v in self.actor.items()}
-        self.critic = critic_w if critic_w is not None else O.init_critic(obs_dim, act_dim, N)
-        self.critic_target = {k: v.clone() for k, v in self.critic.items()}
-        z = lambda d: {k: torch.zeros_like(v) for k, v in d.items()}
-        self.m_a, self.v_a, self.m_c, self.v_c = z(self.actor), z(self.actor), z(self.critic), z(self.critic)
-        self.step_a = self.step_c = 0
+        self.kappa = kappa
+        super().__init__(obs_dim, act_dim, N, gamma, tau, n_steps, lr, betas, eps, actor_w, critic_w, projection, linear)
 
-    def _adam(self, which, g):
-        p, m, v = (self.critic, self.m_c, self.v_c) if which == "c" else (self.actor, self.m_a, self.v_a)
-        if which == "c":
-            self.step_c += 1
-        else:
-            self.step_a += 1
-        for k in O.PARAM_ORDER:
-            O.adam_step(p[k], g[k], m[k], v[k], self.step_c if which == "c" else self.step_a, self.lr,
-                        self.betas[0], self.betas[1], self.eps)
+    def init_head(self, N):
+        self.N = N
+        self.discount = self.gamma if self.projection == "live" else self.gamma ** self.n_steps
+        return N
 
-    def train_step(self, s, a, r, s2, done, is_weights=None, post_update_critic=False, ce_priority=False):
-        lin = self.lin
-        s_t = torch.from_numpy(np.asarray(s, dtype=O.F32))
-        a_t = torch.from_numpy(np.asarray(a, dtype=O.F32))
-        s2_t = torch.from_numpy(np.asarray(s2, dtype=O.F32))
-        with torch.no_grad():
-            tq = critic_raw(self.critic_target, s2_t, actor_forward(self.actor_target, s2_t, lin), lin)
-        cw = {k: v.clone().requires_grad_(True) for k, v in self.critic.items()}
-        q = critic_raw(cw, s_t, a_t, lin)
-        q.retain_grad()
-        raw_rows = loss_rows(tq, q, r, done, self.discount, self.kappa)
-        rows = raw_rows
-        if is_weights is not None:
-            rows = rows * torch.from_numpy(np.asarray(is_weights, dtype=O.F32)).double()
-        loss_c = rows.mean()
-        loss_c.backward()
-        g_c = {k: cw[k].grad.detach().clone() for k in O.PARAM_ORDER}
-        t = td(tq, q, r, done, self.discount)
-        if post_update_critic:
-            self._adam("c", g_c)
-        aw = {k: v.clone().requires_grad_(True) for k, v in self.actor.items()}
-        act = actor_forward(aw, s_t, lin)
-        pq = critic_raw(self.critic, s_t, act, lin)
-        pq.retain_grad()
-        prow = policy_rows(pq)
-        loss_a = prow.mean()
-        loss_a.backward()
-        g_a = {k: aw[k].grad.detach().clone() for k in O.PARAM_ORDER}
-        if not post_update_critic:
-            self._adam("c", g_c)
-        self._adam("a", g_a)
-        for k in O.PARAM_ORDER:
-            O.polyak(self.actor_target[k], self.actor[k], self.tau)
-            O.polyak(self.critic_target[k], self.critic[k], self.tau)
-        base = raw_rows.detach().numpy() if ce_priority else np.abs(t.numpy())
-        prio = (base.astype(O.F32) + O.F32(1e-6)).astype(O.F32)
-        return dict(target_q=tq, q=q.detach(), pi_q=pq.detach(), actor_out=act.detach(),
-                    loss_rows=rows.detach(), pi_rows=prow.detach(), loss_critic=float(loss_c.detach()),
-                    loss_actor=float(loss_a.detach()), td=t, prio=prio, dq=q.grad.detach(), dpi=pq.grad.detach(),
-                    grads_actor=g_a, grads_critic=g_c)
+    def critic_head(self, target, q, r, done):
+        return (loss_rows(target, q, r, done, self.discount, self.kappa), td(target, q, r, done, self.discount), {})
+
+    def policy_head(self, pi):
+        return policy_rows(pi)

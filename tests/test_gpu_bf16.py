@@ -11,6 +11,7 @@ import random
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 from oracle import d4pg_oracle as O
 from tests import bf16_oracle as BO
@@ -42,24 +43,6 @@ def test_bf16_oracle_linear_rounds_operands_and_keeps_fp32_bias_grad():
     assert torch.equal(w.grad, (rb(g).T @ rb(x.detach())).float())
     assert torch.equal(b.grad, g.sum(0))
     assert (y - torch.nn.functional.linear(x, w, b)).abs().max() > 1e-3     # the rounding is visible
-
-
-def test_bf16_oracle_fp32_mode_is_the_oracle():
-    """learner_gradients(gemm="fp32") is LearnerOracle.train_step's gradient half, so the bf16 mode differs from the
-    pinned oracle by the linear layer only."""
-    info = {"type": "categorical", "v_min": -50.0, "v_max": 0.0, "n_atoms": 51}
-    torch.manual_seed(5)
-    rng = np.random.RandomState(5)
-    B = 32
-    s = rng.randn(B, 17).astype(np.float32); a = rng.uniform(-1, 1, (B, 6)).astype(np.float32)
-    r = -3 * rng.rand(B); s2 = rng.randn(B, 17).astype(np.float32); d = rng.rand(B) < 0.1
-    lo = O.LearnerOracle(17, 6, info)
-    mine = BO.learner_gradients(lo, s, a, r, s2, d, gemm="fp32")
-    ref = lo.train_step(s, a, r, s2, d)
-    assert np.array_equal(mine["m"], ref["m"]) and mine["loss_critic"] == ref["loss_critic"]
-    assert mine["loss_actor"] == ref["loss_actor"]
-    for k in O.PARAM_ORDER:
-        assert torch.equal(mine["grads_actor"][k], ref["grads_actor"][k]) and torch.equal(mine["grads_critic"][k], ref["grads_critic"][k])
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------------
@@ -192,14 +175,14 @@ def test_config5_bf16_vs_derived_oracle():
     R = (40 * (rng.rand(n) - 0.5)).astype(np.float32).astype(np.float64); S2 = rng.randn(n, S).astype(np.float32)
     D = rng.rand(n) < 0.05
     dd.replayBuffer.add_batch(Sx, Ax, R, S2, D)
-    lo = O.LearnerOracle(S, A, info, n_steps=5, projection="nstep",
-                         actor_w={k: v.cpu().clone() for k, v in dd.actor.state_dict().items()},
-                         critic_w={k: v.cpu().clone() for k, v in dd.critic.state_dict().items()})
+    oracle = lambda linear: O.LearnerOracle(S, A, info, n_steps=5, projection="nstep", linear=linear,
+                                            actor_w={k: v.cpu().clone() for k, v in dd.actor.state_dict().items()},
+                                            critic_w={k: v.cpu().clone() for k, v in dd.critic.state_dict().items()})
+    lo_b, lo_f = oracle(BO.linear("bf16")), oracle(F.linear)
     dd.train()
     idx = dd.last_batch_info()["idx"].cpu().numpy()
     batch = (Sx[idx], Ax[idx], R[idx], S2[idx], D[idx])
-    ob = BO.learner_gradients(lo, *batch, gemm="bf16")
-    of = lo.train_step(*batch)
+    ob, of = lo_b.train_step(*batch), lo_f.train_step(*batch)
     m = dd.debug_tensor("m", (B, 101)).cpu().numpy()
     assert np.abs(m - ob["m"]).max() <= 1e-5
     lc, la = dd.last_losses()
